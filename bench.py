@@ -57,7 +57,7 @@ def parse():
     ap.add_argument("--bucket-mb", type=float, default=None,
                     help="flat bucket size; default 128 MB on 1 GPU (ResNet-50 = one bucket; BERT-large = 11, overlapped with "
                          "backward) and ONE bucket launched after backward on N > 1 GPUs (a persistent exchange kernel that "
-                         "waits for its peers must not sit on SMs backward needs: BERT-large, 4 GPUs, 39.7 -> 33.1 ms/step, profiles/README.md)")
+                         "waits for its peers must not sit on SMs backward needs)")
     ap.add_argument("--blocks-per-sm", type=int, default=2)
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--breakdown", action="store_true", help="(kept for compatibility: the exchange-kernel timing is always reported)")
@@ -65,22 +65,25 @@ def parse():
                     help="CTAs for exchange kernels launched while backward is still running (0 = whole GPU)")
     ap.add_argument("--no-dense-context", action="store_true", help="skip the dense NCCL all-reduce context measurement")
     ap.add_argument("--no-check", action="store_true", help="skip the multi-GPU correctness self-check (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned to the caller (loss, exchanged "
+                         "gradients, updated parameters; a fixed seeded sample of the large ones) as DIR/<name>.npy")
     return ap.parse_args()
 
 
 def exchange_roofline(exchange_ms, dense_bytes, wire_bytes, world, stage2_bytes=None):
     """Achieved fraction of the exchange kernel's roofline = the slower of (a) its unavoidable HBM traffic at the
-    MEASURED copy bandwidth (read g, read r, write r, write the dense result: 4 x dense bytes) and (b) the bytes it
+    copy bandwidth (read g, read r, write r, write the dense result: 4 x dense bytes) and (b) the bytes it
     sends over NVLink at link bandwidth (the slot to W-1 peers, plus about as much again for the decoded slices of
-    the sharded decode).  Denominators: MEASURED_PEAKS.json (fallback: the profiling recipe's 6 650 GB/s) and the
-    guide's 770 GB/s/direction measured peer copy."""
-    hbm = 6650.0
+    the sharded decode).  Denominators: MEASURED_PEAKS.json when present, else the H100 SXM data-sheet figures
+    (3 350 GB/s HBM3, 450 GB/s per direction of NVLink 4); data-sheet peaks are not reached in practice."""
+    hbm = 3350.0
     try:
         with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "MEASURED_PEAKS.json")) as f:
             hbm = float(json.load(f).get("hbm_gbs", hbm))
     except Exception:
         pass
-    nvlink = 770.0
+    nvlink = 450.0
     t_hbm = 4.0 * dense_bytes / (hbm * 1e9) * 1e3
     # bytes this rank puts on NVLink: its slot to W-1 peers + its decoded slice lists (live count, or ~ as much again)
     nv_bytes = (world - 1) * wire_bytes + (stage2_bytes if stage2_bytes is not None else (world - 1) * wire_bytes)
@@ -92,7 +95,7 @@ def exchange_roofline(exchange_ms, dense_bytes, wire_bytes, world, stage2_bytes=
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -221,7 +224,17 @@ def bench_config(args, kind, B, world, cfg):
                       else "int64 ids in pinned host memory -> H2D"),
             "e2e": "H2D of the step's batch (prefetched one step ahead on a copy stream) + loss read back to the host, every step",
             "e2e_steps": args.steps,
-            "l2": "working set (activations + fp32 gradients + residual) exceeds the 126 MB L2 every step"}
+            "l2": "working set (activations + fp32 gradients + residual) exceeds the 50 MB L2 every step",
+            "cudnn": "deterministic algorithms chosen by heuristics (benchmark=False): same arguments, same outputs"}
+
+
+def reproducible_cudnn():
+    """Same arguments, same outputs: cuDNN may only use deterministic algorithms, and picks them by its heuristics
+    instead of by timing (``benchmark=True`` lets the fastest measured algorithm win, which changes from run to run and
+    changes the gradients in the last bits; the top-k selection then turns that into different selected sets)."""
+    import torch
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
 
 
 def synth_batches(kind, B, seq, gen):
@@ -264,6 +277,31 @@ def model_spec(args):
     raise ValueError(args.model)
 
 
+DUMP_SAMPLE = 2 << 20          # elements kept of a flattened output larger than this (8 MB in float32)
+
+
+def dump_outputs(out_dir, loss, model):
+    """What the last timed step handed back to its caller: the loss, the exchanged gradients and the parameters after
+    the optimizer step, each flattened in ``model.parameters()`` order.  Arrays longer than DUMP_SAMPLE are cut to a
+    fixed seeded sample of positions (saved as ``sample_index``), so two builds can be compared output for output."""
+    import numpy as np
+    import torch
+    params = [p for p in model.parameters()]
+    grad = torch.cat([(p.grad if p.grad is not None else torch.zeros_like(p)).detach().float().reshape(-1) for p in params])
+    weight = torch.cat([p.detach().float().reshape(-1) for p in params])
+    arrays = {"loss": loss.detach().float().reshape(1)}
+    if grad.numel() > DUMP_SAMPLE:
+        g = torch.Generator().manual_seed(2024)
+        idx = torch.randperm(grad.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+        arrays["sample_index"] = idx.double()
+        idx = idx.to(grad.device)
+        grad, weight = grad[idx], weight[idx]
+    arrays["grad"], arrays["params"] = grad, weight
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.cpu().numpy())
+
+
 def measure_dense_context(args, kind, B, world, pool, tgt):
     """Dense NCCL all-reduce data parallelism on the same box, same model / batch / optimizer (context row: on NVLink
     it is the strongest baseline; the compressed path is expected to match it, not beat it)."""
@@ -297,7 +335,7 @@ def run_ours(args, rank, world, local):
     from deepreduce_b200 import ops
     from deepreduce_b200.trainer import Trainer
     torch.manual_seed(1234)
-    torch.backends.cudnn.benchmark = True
+    reproducible_cudnn()
     model, kind, default_b, unit = model_spec(args)
     model = model.cuda()
     B = args.batch or default_b
@@ -312,9 +350,10 @@ def run_ours(args, rank, world, local):
                  overlap_grid=args.overlap_grid)
     dev_x = [tuple(t.cuda() for t in p) for p in pool]
     dev_y = [t.cuda() for t in tgt]
+    last = {}
 
     def step(i):
-        tr.step(*dev_x[i & 1], target=dev_y[i & 1])
+        last["loss"] = tr.step(*dev_x[i & 1], target=dev_y[i & 1])
 
     for i in range(args.warmup):
         step(i)
@@ -327,6 +366,8 @@ def run_ours(args, rank, world, local):
     launches = ops.launch_count() - l0
     clocks = sampler.stop() if rank == 0 else None
     tr.ddp.check()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], tr.model)
     value = world * B * args.steps / (ms / 1e3)
 
     e2e = None
@@ -354,9 +395,9 @@ def run_ours(args, rank, world, local):
                 e.step()
         for i in range(3):
             ex(i)
-        ms_ex, _ = timed(ex, 20, world)
+        ms_ex, _ = timed(ex, args.steps, world)
         stage2 = tr.ddp.stage2_bytes_per_step()
-        extra["exchange_ms_per_step"] = ms_ex / 20
+        extra["exchange_ms_per_step"] = ms_ex / args.steps
         extra["engine_grid"] = tr.ddp.engines[0].grid()
         extra["stage2_bytes_per_step_per_rank"] = int(stage2)
         extra["nvlink_bytes_out_per_step_per_rank"] = int((world - 1) * wire + stage2)
@@ -431,25 +472,18 @@ def run_reference(args, rank, world, local):
     imported on this path."""
     import numpy as np
     import torch
-    ref_file = os.path.join(ROOT, "baseline", "_ref", "deepreduce_ref", "deepreduce.py")
-    if not os.path.exists(ref_file):
-        sys.path.insert(0, os.path.join(ROOT, "baseline"))
-        try:
-            import install_reference
-            install_reference.install(verbose=False)
-        except Exception:
-            pass
-    if not os.path.exists(ref_file):
-        return {"impl": "reference", "unavailable": "reference not installable offline and /root/reference absent on this box"}
+    ref_file = os.path.join(ROOT, "oracle", "_ref", "deepreduce_ref", "deepreduce.py")
+    if not os.path.exists(ref_file):        # build() makes the copy; the benchmark never writes into the tree
+        return {"impl": "reference", "unavailable": "reference copy absent: build() found no checkout of the reference (DEEPREDUCE_REFERENCE, else BASELINE.json reference_path)"}
     sys.path.insert(0, os.path.join(ROOT, "baseline", "shims"))
-    sys.path.insert(0, os.path.join(ROOT, "baseline", "_ref"))
+    sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))
     if not hasattr(np, "RankWarning"):
         np.RankWarning = np.exceptions.RankWarning        # numpy>=2 moved it; the reference reads np.RankWarning
     from deepreduce_ref import deepreduce as R
     from grace_dl.dist.helper import grace_from_params
 
     torch.manual_seed(1234)
-    torch.backends.cudnn.benchmark = True
+    reproducible_cudnn()
     if args.model == "resnet50":
         import torchvision
         model, kind, default_b, unit = torchvision.models.resnet50(weights=None), "image224", 256, "images/s"
@@ -508,8 +542,10 @@ def run_reference(args, rank, world, local):
     dev_x = [tuple(t.cuda() for t in p) for p in pool]
     dev_y = [t.cuda() for t in tgt]
 
+    last = {}
+
     def step(i):
-        train(dev_x[i & 1], dev_y[i & 1])
+        last["loss"] = train(dev_x[i & 1], dev_y[i & 1])
 
     for i in range(args.warmup):
         step(i)
@@ -518,6 +554,8 @@ def run_reference(args, rank, world, local):
         sampler.start()
     ms, wall = timed(step, args.steps, world)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], model)     # p.grad holds what grc.step returned
     value = world * B * args.steps / (ms / 1e3)
     e2e = None
     if not args.no_e2e:

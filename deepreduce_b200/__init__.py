@@ -1,4 +1,4 @@
-"""deepreduce_b200 — a B200-native sparse-gradient communication framework with
+"""deepreduce_b200 — an H100-native (Hopper, sm_90a) sparse-gradient communication framework with
 the capabilities and API of hangxu0304/DeepReduce (see SURVEY.md, DESIGN.md).
 
 Front door (GRACE-compatible, reference README.md:30-48)::

@@ -43,7 +43,7 @@ def register(name: str, *aliases: str):
 
 
 def use_cuda(t) -> bool:
-    """True when the hand-written sm_100a kernels should handle ``t``."""
+    """True when the hand-written sm_90a kernels should handle ``t``."""
     if not getattr(t, "is_cuda", False):
         return False
     from .. import ops

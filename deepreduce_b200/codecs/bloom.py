@@ -13,7 +13,7 @@ Behavioural parity with reference pytorch/deepreduce.py:429-555 (``Bloomfilter``
 Differences by design (SURVEY §3.7): hashing is on-the-fly (``spec``), the filter
 is bit-packed ``int32`` words from birth, indices come back **ascending**, the
 ``random`` policy uses a seeded hash-rank (no global-RNG reseed), sizes are in
-whole 32-bit words.  On CUDA tensors every step runs in hand-written sm_100a
+whole 32-bit words.  On CUDA tensors every step runs in hand-written sm_90a
 kernels (``ops``); the functions named ``*_oracle`` are the plain-torch
 reference of the same ops used on CPU and in the numerics tests.
 """

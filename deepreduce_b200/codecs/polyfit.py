@@ -5,11 +5,11 @@ Parity with reference pytorch/deepreduce.py:306-425 (``PolyFit``) and :558-688
 ``get_segments`` table (:362-377), least-squares fit a degree-``poly_degree``
 polynomial per segment, ship coefficients + the permuted indices.
 
-B200-first changes (SURVEY §7.4 "Polyfit numerics"):
+GPU-first changes (SURVEY §7.4 "Polyfit numerics"):
 
 * the reference builds a monomial Vandermonde on x=1..n in fp64 and inverts the
-  6×6 normal matrix **on the CPU** per segment (:326-338).  B200 fp64 is
-  vestigial, so the fit uses the *Gram (discrete Chebyshev) polynomials*
+  6×6 normal matrix **on the CPU** per segment (:326-338).  fp64 is the slow
+  path on the GPU, so the fit uses the *Gram (discrete Chebyshev) polynomials*
   p_0..p_deg, which are **exactly orthogonal on the grid 0..n-1**::
 
       p_0 = 1,  p_1 = 1 - 2x/N,                       N = n-1

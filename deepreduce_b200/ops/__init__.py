@@ -1,4 +1,4 @@
-"""Native op loader + thin Python wrappers over the sm_100a kernels.
+"""Native op loader + thin Python wrappers over the sm_90a kernels.
 
 ``_dr_cuda.so`` / ``_dr_cpu.so`` are built in-tree by ``ops/build.py``
 (``__graft_entry__.build()``).  On a box with a GPU a missing CUDA extension is a
@@ -65,7 +65,7 @@ def require() -> bool:
     extension is not (never fall back silently on a GPU box)."""
     if _cuda_mod is None:
         raise RuntimeError(
-            "deepreduce_b200: CUDA tensor given but the sm_100a extension is not built/loadable "
+            "deepreduce_b200: CUDA tensor given but the sm_90a extension is not built/loadable "
             f"({_cuda_err!r}). Run `python -c 'import __graft_entry__ as g; g.build()'`.")
     return True
 
@@ -171,7 +171,7 @@ def polyfit_eval(coeffs, segments, degree, total):
 
 
 def dexp_fit(y_ascending):
-    """(a, b, p, q) float64[4] of the double-exponential fit of ascending |values| — one-CTA sm_100a kernel
+    """(a, b, p, q) float64[4] of the double-exponential fit of ascending |values| — one-CTA sm_90a kernel
     (scans + moment sums + both small solves); torch oracle: codecs.dexp.double_exponential_fit."""
     return cuda_module().dexp_fit(y_ascending.contiguous())
 

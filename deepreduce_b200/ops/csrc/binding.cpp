@@ -1,4 +1,4 @@
-// pybind11 / ATen bindings for the sm_100a kernels + the C++ runtime pieces
+// pybind11 / ATen bindings for the sm_90a kernels + the C++ runtime pieces
 // (bucket engine context, background launch thread, IPC arena).
 // The reference's native layer is TensorFlow CPU op glue (tensorflow/bloom_filter_compression.cc,
 // integer_compression.cc, logger.cc); its PyTorch path has no native code and runs strictly after backward with

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the DeepReduce-B200 kernels (sm_100a).
+// Shared device/host helpers for the DeepReduce-B200 kernels (sm_90a).
 // Hash family and bit layout are normative: see deepreduce_b200/spec.py.
 //
 // Parity: the reference looks hashes up in a precomputed MurmurHash3 table `hash_table[d_max, k_max]`
@@ -228,5 +228,8 @@ DR_D void gram_eval(float x, float N, int deg_eff, float (&p)[kDegP1]) {
 // launch accounting (bench.py's "gpu_launches")
 void count_launch(int n = 1);
 long long launch_count();
+
+// SMs of the current device, read once per device: grid-stride kernels size their grids as a few CTAs per SM
+int sm_count();
 
 }  // namespace dr

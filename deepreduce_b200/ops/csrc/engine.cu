@@ -1,4 +1,4 @@
-// DeepReduce-B200 fused bucket engine (sm_100a), v22.
+// DeepReduce-B200 fused bucket engine (sm_90a), v22.
 //
 // One persistent, cooperatively-launched kernel runs the whole per-bucket
 // gradient exchange:
@@ -40,6 +40,19 @@ namespace dr {
 static std::atomic<long long> g_launches{0};
 void count_launch(int n) { g_launches.fetch_add(n); }
 long long launch_count() { return g_launches.load(); }
+
+int sm_count() {
+  constexpr int kMaxDevices = 64;
+  static std::atomic<int> cached[kMaxDevices];
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev);
+  if (dev >= 0 && dev < kMaxDevices) n = cached[dev].load(std::memory_order_relaxed);
+  if (n > 0) return n;
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  if (n < 1) n = 1;
+  if (dev >= 0 && dev < kMaxDevices) cached[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
 
 namespace {
 
@@ -370,7 +383,7 @@ DR_D uint32_t round16(uint32_t bytes) { return (bytes + 15u) & ~15u; }
 //               thread); kTma = false: every THREAD copies its own float4 of g and r with cp.async (LDGSTS) into a
 //               private slot of the ring and reads it back itself — no mbarriers, no producer, warps never wait for
 //               each other between tensor boundaries.  Selected by EngineParams::use_tma; both are kept because which
-//               one feeds HBM better is a measured property (profiles/).
+//               one feeds HBM better is measured, not derived (scripts/engine_microbench.py).
 template <bool kTma>
 DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;

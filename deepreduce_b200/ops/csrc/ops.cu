@@ -1,4 +1,4 @@
-// Stand-alone sm_100a kernels behind the GRACE-compatible per-tensor codec API
+// Stand-alone sm_90a kernels behind the GRACE-compatible per-tensor codec API
 // (deepreduce_b200/codecs/*): bloom insert / universe query+select, QSGD,
 // bit packing, Gram-polynomial fit/eval, delta+bp128 integer coding.
 // Each has a plain-torch oracle in the codec module; tests compare them.
@@ -371,7 +371,8 @@ __global__ void rle_expand_kernel(const int64_t* __restrict__ ones_excl, const i
   }
 }
 
-inline int grid_for(int64_t n, int threads, int cap = 148 * 8) {
+inline int grid_for(int64_t n, int threads, int ctas_per_sm = 8) {   // grid-stride kernels: at most 8 CTAs per SM
+  const int64_t cap = (int64_t)ctas_per_sm * sm_count();
   int64_t g = (n + threads - 1) / threads;
   if (g < 1) g = 1;
   if (g > cap) g = cap;

@@ -108,7 +108,8 @@ void launch_u8_to_nhwc_norm(const uint8_t* in, void* out_bf16, int64_t n_pix, co
   count_launch();
   int64_t g = (n_pix / 4 + 255) / 256;
   if (g < 1) g = 1;
-  if (g > 148 * 16) g = 148 * 16;
+  const int64_t cap = 16LL * sm_count();           // grid-stride kernel: at most 16 CTAs per SM
+  if (g > cap) g = cap;
   u8_to_nhwc_norm_kernel<<<(int)g, 256, 0, st>>>(in, reinterpret_cast<__nv_bfloat16*>(out_bf16), n_pix, mean[0], mean[1],
                                                   mean[2], inv_std[0], inv_std[1], inv_std[2]);
 }

@@ -244,7 +244,7 @@ class DeepReduceDDP:
             else:
                 # the LAST bucket (or the only one): nothing is left to overlap with, so every microsecond until the
                 # kernel starts is exposed — launch inline on the current stream with the whole GPU instead of paying
-                # the thread hand-off + event round trip (measured: 54.30 -> 54.00 ms/step, profiles/overlap_sweep.md)
+                # the thread hand-off + event round trip
                 eng.ctx.set_grid_cap(0)
                 if self.sched is not None and len(self.buckets) > 1 and self.world > 1:
                     # cross-rank ordering: every rank must run its bucket kernels in the same order — a full-grid

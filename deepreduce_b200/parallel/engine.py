@@ -453,8 +453,8 @@ class BucketEngine:
         """Measure how fast every CTA of the persistent kernel gets through its share of the accumulate / insert / query /
         emit phases (``%globaltimer`` stamps, ``set_debug_times``) on synthetic gradients and re-cut the four tile
         partitions so that slow CTAs get less work.  Why: the two co-resident CTAs of an SM do not run the issue-bound
-        phases at the same speed (the per-CTA timeline shows the second-launched CTA of almost every SM 12 % slower in
-        accumulate and 20 % in query; profiles/README.md section 2), and every phase ends at a grid barrier, i.e. lasts
+        phases at the same speed (per-CTA timelines from scripts/cta_timeline.py show the second-launched CTA of an SM
+        slower in accumulate and query), and every phase ends at a grid barrier, i.e. lasts
         as long as its slowest CTA.  Collective at W > 1 (runs ``(rounds + 1) * (steps + 1)`` exchange steps).  Resets
         residual / select history / gradient afterwards; the step counter keeps running (flags are epoch-valued).
         Returns the per-round phase maxima / medians."""

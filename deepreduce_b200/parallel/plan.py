@@ -28,8 +28,9 @@ NUM_HIST = 3
 ALIGN_ELEMS = 32
 MAX_SEGMENTS = 22
 # (segment start, one-tile tensor) cost in tiles' worth for the four phase classes of the kernel's tile -> CTA partition
-# (accumulate, insert, query, emit): least-squares fit of the per-CTA phase durations of a ResNet-50 bucket
-# (profiles/round2/cta_timeline_v21.txt; scripts/cta_timeline.py)
+# (accumulate, insert, query, emit): least-squares fit of the per-CTA phase durations of a ResNet-50 bucket taken with
+# scripts/cta_timeline.py on the previous target GPU and not re-fitted on the H100; BucketEngine.calibrate_partition
+# measures the per-CTA speeds of the GPU it runs on and re-cuts the partition from them
 PART_WEIGHTS = ((5.0, 1.0), (2.0, 0.0), (5.5, 1.5), (3.0, 0.0))
 
 

@@ -1,5 +1,5 @@
 """Wire / hashing specification shared by the torch oracle, the C++ CPU ops and
-the sm_100a kernels.
+the sm_90a kernels.
 
 The reference keeps a precomputed ``hash_table[d_max, k_max]`` of MurmurHash3
 values on every GPU (reference pytorch/deepreduce.py:42-44, 461, 471) and

@@ -3,7 +3,7 @@
 The reference's TF half (tensorflow/deepreduce.py, 557 LoC, TF1 graph mode + Horovod)
 exposes whole-GRACE-TF compressors with ``compress(tensor, params)`` /
 ``decompress(tensors, ctx, params)`` static methods, a class-level residual store and the
-custom CPU ops.  TensorFlow/Horovod are not installable here, and a B200-first framework has
+custom CPU ops.  TensorFlow/Horovod are not installable here, and a GPU-first framework has
 one tensor runtime, so the same classes / parameter keys / wire formats are provided over
 torch tensors:
 

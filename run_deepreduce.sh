@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Launch recipes mirroring the reference's run_deepreduce.sh (OpenMPI/TCP, 1 GPU per host) on one 8xB200 box:
+# Launch recipes mirroring the reference's run_deepreduce.sh (OpenMPI/TCP, 1 GPU per host) on one 8-GPU H100 box:
 # one process per GPU via torchrun, NCCL bootstrap, fused P2P exchange.  Data is synthetic.
 N=${N:-8}
 RUN="python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1 --master-port ${PORT:-29400} -m deepreduce_b200.cli"

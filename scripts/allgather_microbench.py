@@ -4,9 +4,9 @@
     torchrun --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 scripts/allgather_microbench.py [iters]
 
 Prints one JSON line on rank 0: per-variant device time (CUDA events, max over ranks) and bus bandwidth
-(bytes a rank sends to its W-1 peers / time) against the 770 GB/s measured / 900 GB/s nominal NVLink figure.
+(bytes a rank sends to its W-1 peers / time) against the H100's 450 GB/s per direction NVLink 4 data-sheet figure.
 Variants: P2P stores (default arena), NVLS multicast (arena in symmetric memory), NCCL all_gather.
-Written in round 1 after the GPU budget was spent — first hardware run pending."""
+Not run on the H100."""
 import json
 import os
 import sys
@@ -71,7 +71,7 @@ def main():
     gathered = torch.empty(world * slot.numel(), dtype=torch.int32, device="cuda")
     ms = timed(lambda: dist.all_gather_into_tensor(gathered, slot), iters, world)
     out["variants"]["nccl_all_gather"] = {"ms": ms, "bus_gbs": sent / (ms * 1e-3) / 1e9 if world > 1 else 0.0}
-    out["nvlink_gbs_per_dir"] = {"measured": 770.0, "nominal": 900.0}
+    out["nvlink_gbs_per_dir"] = {"nominal": 450.0}
     if rank == 0:
         print(json.dumps(out), flush=True)
     dist.destroy_process_group()

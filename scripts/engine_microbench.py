@@ -75,7 +75,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)              # default: H100 SXM HBM3, data sheet
     d = plan.dense_bytes()
     # algorithmic HBM bytes: read g + read r + write r (accum), write dense out (decode); other passes re-read r (L2/HBM)
     min_bytes = 4 * d

@@ -53,11 +53,11 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)              # default: H100 SXM HBM3, data sheet
     d, wire, s2 = plan.dense_bytes(), plan.wire_bytes(), eng.stage2_bytes()
     nv = (world - 1) * wire + s2
     t_hbm = 4 * d / (hbm * 1e9) * 1e3
-    t_nv = nv / 770e9 * 1e3
+    t_nv = nv / 450e9 * 1e3                                  # H100 NVLink 4, data sheet, per direction
     if rank == 0:
         print(json.dumps({"kernel": "dr_engine_kernel (fused)", "world": world, "index": index, "value": value,
                           "fused_ms_median_max_over_ranks": med, "fused_ms_min": mn, "dense_bytes": d, "wire_bytes": wire,

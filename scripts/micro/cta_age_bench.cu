@@ -1,12 +1,12 @@
 // Microbenchmark: do two co-resident 512-thread CTAs of an SM run an issue-bound streaming phase at the same speed?
 // Work = the engine's accumulate phase in miniature (read g, read r, write r + g, write g = 0, candidate compaction by
 // ballot, digit-1 SMEM histogram, conditional digit-2 histogram), one contiguous tile range per (virtual) CTA.
-//   mode 0: 296 CTAs x 512 threads (2 per SM) — what the engine launches
-//   mode 1: 148 CTAs x 1024 threads, virtual CTA = warps 0-15 / 16-31
-//   mode 2: 148 CTAs x 1024 threads, virtual CTA = warps whose id has bit 2 clear / set (halves interleaved on every
+//   mode 0: 264 CTAs x 512 threads (2 per SM) — what the engine launches
+//   mode 1: 132 CTAs x 1024 threads, virtual CTA = warps 0-15 / 16-31
+//   mode 2: 132 CTAs x 1024 threads, virtual CTA = warps whose id has bit 2 clear / set (halves interleaved on every
 //           scheduler: warp w runs on sub-partition w % 4)
 // Prints the kernel time and the mean per-virtual-CTA duration of the first / second virtual CTA of every SM.
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o cta_age_bench cta_age_bench.cu
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o cta_age_bench cta_age_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -80,7 +80,7 @@ int main() {
   const size_t n = (size_t)n_tiles * kTile;
   float *g, *r, *flush, *src; uint2* cand; unsigned* cnt; unsigned long long* times; unsigned* smids;
   cudaMalloc(&g, n * 4); cudaMalloc(&r, n * 4); cudaMalloc(&src, n * 4); cudaMalloc(&flush, 256u << 20);
-  cudaMalloc(&cand, n * 8); cudaMalloc(&cnt, n_tiles * 16 * 4); cudaMalloc(&times, 296 * 8); cudaMalloc(&smids, 296 * 4);
+  cudaMalloc(&cand, n * 8); cudaMalloc(&cnt, n_tiles * 16 * 4); cudaMalloc(&times, 264 * 8); cudaMalloc(&smids, 264 * 4);
   float* h = (float*)malloc(n * 4);
   srand(1);
   for (size_t i = 0; i < n; ++i) h[i] = (float)rand() / RAND_MAX;
@@ -96,18 +96,18 @@ int main() {
       cudaMemsetAsync(r, 0, n * 4);
       cudaMemsetAsync(flush, 1, 256u << 20);
       cudaEventRecord(e0);
-      if (mode == 0) k<512><<<296, 512>>>(g, r, cand, cnt, n_tiles, thr, thr >> 20, mode, times, smids);
-      else k<1024><<<148, 1024>>>(g, r, cand, cnt, n_tiles, thr, thr >> 20, mode, times, smids);
+      if (mode == 0) k<512><<<264, 512>>>(g, r, cand, cnt, n_tiles, thr, thr >> 20, mode, times, smids);
+      else k<1024><<<132, 1024>>>(g, r, cand, cnt, n_tiles, thr, thr >> 20, mode, times, smids);
       cudaEventRecord(e1); cudaEventSynchronize(e1);
       float ms; cudaEventElapsedTime(&ms, e0, e1);
       if (it >= 2) {
         best = ms < best ? ms : best; sum += ms;
-        unsigned long long ht[296]; unsigned hs[296];
-        cudaMemcpy(ht, times, 296 * 8, cudaMemcpyDeviceToHost); cudaMemcpy(hs, smids, 296 * 4, cudaMemcpyDeviceToHost);
+        unsigned long long ht[264]; unsigned hs[264];
+        cudaMemcpy(ht, times, 264 * 8, cudaMemcpyDeviceToHost); cudaMemcpy(hs, smids, 264 * 4, cudaMemcpyDeviceToHost);
         // first / second virtual CTA of an SM: by index order among the virtual CTAs that report the same smid
         int seen[512]; memset(seen, 0, sizeof(seen));
         double f = 0, s = 0; int nf = 0, ns = 0; double m = 0;
-        for (int b = 0; b < 296; ++b) {
+        for (int b = 0; b < 264; ++b) {
           const double us = ht[b] / 1e3;
           if (us > m) m = us;
           if (seen[hs[b] & 511]++ == 0) { f += us; ++nf; } else { s += us; ++ns; }

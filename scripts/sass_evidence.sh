@@ -1,5 +1,5 @@
 #!/bin/bash
-# SASS evidence of the built extension (run on the CPU box): per engine-kernel variant the Blackwell / async mnemonics
+# SASS evidence of the built extension (needs no GPU): per engine-kernel variant the Hopper / async mnemonics
 SO=deepreduce_b200/ops/_dr_cuda.so
 cuobjdump -sass $SO > /tmp/_dr_cuda.sass
 python - <<'PY'

@@ -355,12 +355,12 @@ def test_phase_cuts_cover_all_tiles_and_follow_speeds():
 
 
 def test_partition_calibration_converges_on_a_two_speed_machine():
-    """The speed update behind BucketEngine.calibrate_partition, on a model of what was measured on B200: half of the
+    """The speed update behind BucketEngine.calibrate_partition, on a model of a GPU running two CTAs per SM: half of the
     CTAs (the second-launched one of every SM) run a phase 15 % slower.  With shares proportional to the calibrated
     speeds the systematic gap is removed within two rounds, and the noise of a single round does not blow up."""
     import numpy as np
     from deepreduce_b200.parallel.plan import update_cta_speeds
-    G = 296
+    G = 264                                  # 2 CTAs x 132 SMs (H100)
     true = np.ones(G); true[G // 2:] = 0.85
     speeds = np.ones(G)
     rng = np.random.default_rng(0)
@@ -384,7 +384,7 @@ def test_phase_cuts_property_any_speeds_any_plan():
     from deepreduce_b200.parallel import BucketPlan
 
     @settings(max_examples=40, deadline=None)
-    @given(st.lists(st.integers(1, 300000), min_size=1, max_size=12), st.sampled_from([2, 37, 148, 296]),
+    @given(st.lists(st.integers(1, 300000), min_size=1, max_size=12), st.sampled_from([2, 37, 132, 148, 264, 296]),
            st.integers(0, 2 ** 31 - 1))
     def check(numels, grid, seed):
         plan = BucketPlan(numels, compress_ratio=0.01)
