@@ -1,0 +1,120 @@
+"""Training BatchNorm fused with the ReLU and the residual add of ResNet-50, on channels_last bf16 activations.
+
+Forward runs the sm_90a kernels of ``ops/csrc/bn.cu``: torch's own channels-last statistics kernel, then one
+vectorised pass that applies BN, adds the skip branch and applies the ReLU.  The unfused graph writes and re-reads the
+BN output, the sum and the ReLU output instead.  Backward calls the ops autograd would run for the unfused graph
+(``threshold_backward``, then ``native_batch_norm_backward``), so gradients are the same ops on the same tensors.
+
+Every fused result is bitwise that of the unfused graph: same reductions, same fp32 expressions, same bf16 rounding
+points.  ``eligible()`` decides per call; anything it rejects (CPU, eval mode, fp32, another memory layout) runs the
+unfused modules unchanged.  ``DR_FUSED_BN=0`` selects the unfused graph everywhere, for A/B comparisons.
+"""
+from __future__ import annotations
+
+import os
+
+import torch
+import torch.nn as nn
+import torch.nn.functional as F
+
+
+def enabled() -> bool:
+    return os.environ.get("DR_FUSED_BN", "1") != "0"
+
+
+def _eligible_x(x: torch.Tensor) -> bool:
+    # the layout the native training path runs its channels-last kernels on (and that the fused kernels assume)
+    return (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.stride(1) == 1
+            and x.is_contiguous(memory_format=torch.channels_last) and x.size(1) % 8 == 0 and x.size(1) <= 8192
+            and x.numel() < 2 ** 31 - 1 and x.numel() // x.size(1) > 1)
+
+
+def _eligible_bn(bn: nn.BatchNorm2d) -> bool:
+    return (bn.training and bn.track_running_stats and bn.running_mean is not None and bn.momentum is not None
+            and bn.affine)
+
+
+def eligible(x: torch.Tensor, bn: nn.BatchNorm2d) -> bool:
+    return enabled() and _eligible_x(x) and _eligible_bn(bn)
+
+
+def _stats(x, bn):
+    """(save_mean, save_invstd) of a training step; updates the running stats and counter as nn.BatchNorm2d does."""
+    from .. import ops
+    bn.num_batches_tracked.add_(1)
+    return ops.cuda_module().bn_stats(x, bn.running_mean, bn.running_var, float(bn.momentum), float(bn.eps))
+
+
+def _bn_backward(g, x, weight, mean, invstd, eps):
+    return torch.ops.aten.native_batch_norm_backward(g, x, weight, None, None, mean, invstd, True, eps, [True, True, True])
+
+
+class _BNReLU(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, mean, invstd, eps):
+        from .. import ops
+        y = ops.cuda_module().bn_apply(0, x, [mean, invstd, weight, bias])
+        ctx.save_for_backward(x, weight, mean, invstd, y)
+        ctx.eps = eps
+        return y
+
+    @staticmethod
+    def backward(ctx, gy):
+        x, weight, mean, invstd, y = ctx.saved_tensors
+        g = torch.ops.aten.threshold_backward(gy, y, 0)
+        dx, dw, db = _bn_backward(g, x, weight, mean, invstd, ctx.eps)
+        return dx, dw, db, None, None, None
+
+
+class _BNAddReLU(torch.autograd.Function):
+    """relu(bn(x) + z) for an identity skip, relu(bn(x) + bn_z(z)) for a downsample skip (``pz`` given)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, mean, invstd, eps, z, wz, bz, mz, iz, eps_z):
+        from .. import ops
+        mod = ops.cuda_module()
+        if wz is None:
+            o = mod.bn_apply(1, x, [mean, invstd, weight, bias], z)
+            ctx.save_for_backward(x, weight, mean, invstd, o)
+        else:
+            o = mod.bn_apply(2, x, [mean, invstd, weight, bias], z, [mz, iz, wz, bz])
+            ctx.save_for_backward(x, weight, mean, invstd, o, z, wz, mz, iz)
+        ctx.eps, ctx.eps_z, ctx.has_bn_z = eps, eps_z, wz is not None
+        return o
+
+    @staticmethod
+    def backward(ctx, go):
+        saved = ctx.saved_tensors
+        x, weight, mean, invstd, o = saved[:5]
+        g = torch.ops.aten.threshold_backward(go, o, 0)
+        dx, dw, db = _bn_backward(g, x, weight, mean, invstd, ctx.eps)
+        if not ctx.has_bn_z:
+            return dx, dw, db, None, None, None, g, None, None, None, None, None
+        z, wz, mz, iz = saved[5:]
+        dz, dwz, dbz = _bn_backward(g, z, wz, mz, iz, ctx.eps_z)
+        return dx, dw, db, None, None, None, dz, dwz, dbz, None, None, None
+
+
+def bn_relu(x: torch.Tensor, bn: nn.BatchNorm2d) -> torch.Tensor:
+    """``F.relu(bn(x), inplace=True)``."""
+    if not eligible(x, bn):
+        return F.relu(bn(x), inplace=True)
+    mean, invstd = _stats(x, bn)
+    return _BNReLU.apply(x, bn.weight, bn.bias, mean, invstd, bn.eps)
+
+
+def bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, idt: torch.Tensor) -> torch.Tensor:
+    """``F.relu(bn(x) + idt, inplace=True)``."""
+    if not (eligible(x, bn) and idt.dtype == x.dtype and idt.shape == x.shape and idt.stride() == x.stride()):
+        return F.relu(bn(x) + idt, inplace=True)
+    mean, invstd = _stats(x, bn)
+    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, bn.eps, idt, None, None, None, None, None)
+
+
+def bn_bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, xd: torch.Tensor, bnd: nn.BatchNorm2d) -> torch.Tensor:
+    """``F.relu(bn(x) + bnd(xd), inplace=True)``: the tail of a bottleneck with a downsample branch."""
+    if not (eligible(x, bn) and eligible(xd, bnd) and xd.shape == x.shape and xd.stride() == x.stride()):
+        return F.relu(bn(x) + bnd(xd), inplace=True)
+    md, id_ = _stats(xd, bnd)
+    mean, invstd = _stats(x, bn)
+    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, bn.eps, xd, bnd.weight, bnd.bias, md, id_, bnd.eps)

@@ -9,6 +9,8 @@ from __future__ import annotations
 import torch.nn as nn
 import torch.nn.functional as F
 
+from .fused_bn import bn_add_relu, bn_bn_add_relu, bn_relu
+
 
 # ----------------------------------------------------------------------------
 # CIFAR ResNet (He et al. 2015, 6n+2 layers): resnet20 = n 3
@@ -77,11 +79,15 @@ class _Bottleneck(nn.Module):
             self.downsample = nn.Sequential(nn.Conv2d(inp, out, 1, stride, bias=False), nn.BatchNorm2d(out))
 
     def forward(self, x):
-        idt = x if self.downsample is None else self.downsample(x)
-        y = F.relu(self.bn1(self.conv1(x)), inplace=True)
-        y = F.relu(self.bn2(self.conv2(y)), inplace=True)
-        y = self.bn3(self.conv3(y))
-        return F.relu(y + idt, inplace=True)
+        # each helper is the unfused composite unless its input is a channels_last bf16 CUDA training tensor
+        # (models/fused_bn.py); either way the results are bitwise the same
+        xd = None if self.downsample is None else self.downsample[0](x)
+        y = bn_relu(self.conv1(x), self.bn1)
+        y = bn_relu(self.conv2(y), self.bn2)
+        y = self.conv3(y)
+        if xd is None:
+            return bn_add_relu(y, self.bn3, x)
+        return bn_bn_add_relu(y, self.bn3, xd, self.downsample[1])
 
 
 class ResNet(nn.Module):
@@ -103,7 +109,7 @@ class ResNet(nn.Module):
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
 
     def forward(self, x):
-        x = self.maxpool(F.relu(self.bn1(self.conv1(x)), inplace=True))
+        x = self.maxpool(bn_relu(self.conv1(x), self.bn1))
         x = self.layers(x)
         x = F.adaptive_avg_pool2d(x, 1).flatten(1)
         return self.fc(x)

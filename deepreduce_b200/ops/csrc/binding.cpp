@@ -243,6 +243,82 @@ static torch::Tensor u8_to_nhwc_norm(torch::Tensor in, std::vector<double> mean,
 }
 
 // ---------------------------------------------------------------------------
+// training BatchNorm (+ ReLU, + residual add) on channels_last bf16 (bn.cu)
+// ---------------------------------------------------------------------------
+// torch's own channels-last Welford statistics, the instantiation native_batch_norm runs for bf16 input (exported by
+// libtorch_cuda): mean and biased variance come out bitwise as in the unfused graph.
+namespace at::native {
+struct Var;
+template <typename scalar_t, typename VarTransform>
+void batch_norm_stats_channels_last_cuda_template(const at::Tensor& out_mean, const at::Tensor& out_invstd,
+                                                   const at::Tensor& input, double epsilon);
+}  // namespace at::native
+
+static void check_bn_input(const torch::Tensor& x) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kBFloat16 && x.dim() == 4 && x.stride(1) == 1 &&
+                  x.is_contiguous(at::MemoryFormat::ChannelsLast),
+              "bn: x must be a channels_last bf16 CUDA tensor");
+  TORCH_CHECK(x.size(1) % 8 == 0 && x.size(1) <= 8192, "bn: channels must be a multiple of 8, at most 8192");
+  TORCH_CHECK(x.numel() < std::numeric_limits<int32_t>::max(), "bn: tensor too large for 32-bit indexing");
+}
+
+static void check_chan(const torch::Tensor& t, int64_t C, const char* what) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kFloat32 && t.is_contiguous() && t.numel() == C, "bn: ", what,
+              " must be a contiguous float32 CUDA tensor of C elements");
+}
+
+// -> (save_mean, save_invstd); updates running_mean / running_var in place like native_batch_norm(training=True)
+static std::vector<torch::Tensor> bn_stats(torch::Tensor x, torch::Tensor running_mean, torch::Tensor running_var,
+                                           double momentum, double eps) {
+  check_bn_input(x);
+  const int64_t C = x.size(1);
+  check_chan(running_mean, C, "running_mean");
+  check_chan(running_var, C, "running_var");
+  const int64_t N = x.numel() / C;
+  TORCH_CHECK(N > 1, "bn: expected more than 1 value per channel when training");
+  c10::cuda::CUDAGuard g(x.device());
+  auto opts = x.options().dtype(torch::kFloat32);
+  auto mean = torch::empty({C}, opts), var = torch::empty({C}, opts);
+  at::native::batch_norm_stats_channels_last_cuda_template<c10::BFloat16, at::native::Var>(mean, var, x, eps);
+  const float bessel = static_cast<float>(static_cast<double>(N) / static_cast<double>(N - 1));
+  cudaError_t e = dr::launch_bn_update_stats(mean.data_ptr<float>(), var.data_ptr<float>(), running_mean.data_ptr<float>(),
+                                             running_var.data_ptr<float>(), (int)C, (float)momentum, bessel, (float)eps,
+                                             cur_stream());
+  TORCH_CHECK(e == cudaSuccess, "bn_stats: ", cudaGetErrorString(e));
+  return {mean, var};
+}
+
+static dr::BnParams bn_params(const std::vector<torch::Tensor>& p, int64_t C) {
+  TORCH_CHECK(p.size() == 4, "bn: expected (mean, invstd, weight, bias)");
+  const char* names[4] = {"mean", "invstd", "weight", "bias"};
+  for (int i = 0; i < 4; ++i) check_chan(p[i], C, names[i]);
+  return {p[0].data_ptr<float>(), p[1].data_ptr<float>(), p[2].data_ptr<float>(), p[3].data_ptr<float>()};
+}
+
+// mode 0: relu(bn(x)); 1: relu(bn(x) + z); 2: relu(bn(x) + bn_z(z)).  p / pz = (mean, invstd, weight, bias).
+static torch::Tensor bn_apply(int64_t mode, torch::Tensor x, std::vector<torch::Tensor> p, c10::optional<torch::Tensor> z,
+                              std::vector<torch::Tensor> pz) {
+  check_bn_input(x);
+  const int64_t C = x.size(1);
+  const dr::BnParams px = bn_params(p, C);
+  dr::BnParams pzz{};
+  const void* zp = nullptr;
+  if (mode != 0) {
+    TORCH_CHECK(z.has_value() && z->sizes() == x.sizes() && z->strides() == x.strides() &&
+                    z->scalar_type() == torch::kBFloat16 && z->device() == x.device(),
+                "bn: z must match x in shape, layout, dtype and device");
+    zp = z->data_ptr();
+    if (mode == 2) pzz = bn_params(pz, C);
+  }
+  c10::cuda::CUDAGuard g(x.device());
+  auto out = torch::empty_like(x);
+  cudaError_t e = dr::launch_bn_apply((int)mode, x.data_ptr(), px, zp, pzz, out.data_ptr(), x.numel() / C, (int)C,
+                                      cur_stream());
+  TORCH_CHECK(e == cudaSuccess, "bn_apply: ", cudaGetErrorString(e));
+  return out;
+}
+
+// ---------------------------------------------------------------------------
 // engine context
 // ---------------------------------------------------------------------------
 struct Engine {
@@ -473,6 +549,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("delta_bp128_encode", &delta_bp128_encode);
   m.def("delta_bp128_decode", &delta_bp128_decode);
   m.def("u8_to_nhwc_norm", &u8_to_nhwc_norm);
+  m.def("bn_stats", &bn_stats);
+  m.def("bn_apply", &bn_apply, py::arg("mode"), py::arg("x"), py::arg("p"), py::arg("z") = py::none(),
+        py::arg("pz") = std::vector<torch::Tensor>{});
   m.def("rle_runs", &rle_runs);
   m.def("rle_indices", &rle_indices);
   m.def("arena_alloc", &arena_alloc);

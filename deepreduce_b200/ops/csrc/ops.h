@@ -54,4 +54,12 @@ int arena_enable_peer_access(const int* devices, int n);   // peers = the listed
 void launch_u8_to_nhwc_norm(const uint8_t* in, void* out_bf16, int64_t n_pix, const float* mean, const float* inv_std,
                             cudaStream_t st);
 
+// bn.cu — training BatchNorm (+ ReLU, + residual add) on NHWC bf16, C % 8 == 0; per-channel fp32 parameters
+struct BnParams { const float* mean; const float* invstd; const float* weight; const float* bias; };
+cudaError_t launch_bn_update_stats(const float* mean, float* var_invstd, float* running_mean, float* running_var, int C,
+                                   float momentum, float bessel, float eps, cudaStream_t st);
+// mode 0: relu(bn(x)); 1: relu(bn(x) + z); 2: relu(bn(x) + bn_z(z))
+cudaError_t launch_bn_apply(int mode, const void* x, const BnParams& px, const void* z, const BnParams& pz, void* out,
+                            int64_t rows, int C, cudaStream_t st);
+
 }  // namespace dr

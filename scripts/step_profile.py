@@ -1,0 +1,163 @@
+#!/usr/bin/env python
+"""Per-kernel-class profile of the headline ResNet-50 step (bench.py's default configuration: batch 256, bf16 autocast,
+channels_last, top-k 1 % + bloom index, one 128 MB bucket, deterministic cuDNN by heuristics).
+
+    python scripts/step_profile.py [--steps 3] [--warmup 3] [--out script_out/step_profile]
+
+torch.profiler with CUDA activities, in a run of its own (tracing slows the host; take timings from bench.py).  Prints
+and writes ``<out>/profile_fused<0|1>.json`` and a markdown table: per kernel class the GPU time per step, and for the
+BatchNorm / ReLU / add classes the bytes per step computed from the activation shapes and the resulting GB/s.  The card
+name and power limit are read in the same run.  ``DR_FUSED_BN`` selects the path as it does for the model.
+"""
+from __future__ import annotations
+
+import argparse
+import collections
+import json
+import os
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+# (class, substrings of the kernel name); the first match wins
+CLASSES = [
+    ("exchange", ("dr_engine_kernel",)),
+    ("bn fused apply (own)", ("bn_apply_kernel",)),
+    ("bn running-stats update (own)", ("bn_update_stats_kernel",)),
+    ("bn stats", ("batch_norm_collect_statistics",)),
+    ("bn apply", ("batch_norm_transform_input",)),
+    ("bn bwd reduce", ("batch_norm_backward_reduce",)),
+    ("bn bwd elemt", ("batch_norm_backward_elemt",)),
+    ("relu", ("clamp_scalar", "clamp_min")),
+    ("max pool", ("max_pool",)),
+    ("threshold_backward", ("threshold",)),
+    ("add", ("AddFunctor", "CUDAFunctor_add", "add_kernel")),
+    ("optimizer", ("sgd", "Sgd", "multi_tensor")),
+    ("conv wgrad", ("wgrad",)),
+    ("conv dgrad", ("dgrad",)),
+    ("conv fprop", ("fprop", "implicit_gemm", "conv", "xmma", "cutlass", "cudnn")),
+]
+
+
+def classify(name: str) -> str:
+    for cls, keys in CLASSES:
+        if any(k in name for k in keys):
+            return cls
+    return "other"
+
+
+def card():
+    q = "name,power.limit,clocks.max.sm"
+    try:
+        return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", "0"],
+                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:  # noqa: BLE001
+        return f"nvidia-smi unavailable: {e}"
+
+
+def shape_bytes(model, run_step):
+    """Bytes of the bf16 BN inputs of one forward, by role: W = bn1/bn2/stem (BN + ReLU), T = bn3 (BN + add + ReLU),
+    D = downsample BN, I = block inputs (where backward sums the skip and conv1 gradients)."""
+    import torch.nn as nn
+    from deepreduce_b200.models.resnet import _Bottleneck
+    acc = collections.Counter()
+    hooks = []
+    for name, m in model.named_modules():
+        if isinstance(m, nn.Conv2d):
+            role = "D" if name.endswith("downsample.0") else ("T" if name.endswith("conv3") else "W")
+            hooks.append(m.register_forward_hook(lambda mod, i, o, r=role: acc.__setitem__(r, acc[r] + o.numel() * o.element_size())))
+        elif isinstance(m, _Bottleneck):
+            hooks.append(m.register_forward_hook(lambda mod, i, o: acc.__setitem__("I", acc["I"] + i[0].numel() * i[0].element_size())))
+    run_step()
+    for h in hooks:
+        h.remove()
+    return dict(acc)
+
+
+def pass_bytes(b, fused):
+    """Minimum bytes each memory-bound class moves per step (reads + writes over the tensors it touches)."""
+    W, T, D, I = b["W"], b["T"], b["D"], b["I"]
+    out = {"bn stats": W + T + D, "bn bwd reduce": 2 * (W + T + D), "bn bwd elemt": 3 * (W + T + D),
+           "threshold_backward": 3 * (W + T)}
+    if fused:      # bn_relu: read x, write y; tails: read x3 and idt (or xd), write o; backward adds stay
+        out.update({"bn fused apply (own)": 2 * W + 3 * T, "add": 3 * I})
+    else:          # apply: read x, write y; relu_ in place; forward add: 2 reads + 1 write; backward junction adds
+        out.update({"bn apply": 2 * (W + T + D), "relu": 2 * (W + T), "add": 3 * T + 3 * I})
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--out", default=os.path.join(ROOT, "script_out", "step_profile"))
+    args = ap.parse_args()
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    import bench
+    from deepreduce_b200.models import fused_bn, resnet50
+    from deepreduce_b200.trainer import Trainer
+    assert torch.cuda.is_available(), "needs a GPU"
+    torch.manual_seed(1234)
+    bench.reproducible_cudnn()
+    B = args.batch
+    tr = Trainer(resnet50().cuda(), dict(bench.CONFIGS["bloom"]), lr=0.05, amp_dtype=torch.bfloat16, channels_last=True,
+                 bucket_cap_mb=128.0, u8_input=True)
+    gen = torch.Generator().manual_seed(77)
+    x = torch.randint(0, 256, (B, 224, 224, 3), dtype=torch.uint8, generator=gen).cuda()
+    y = torch.randint(0, 1000, (B,), generator=gen).cuda()
+    step = lambda: tr.step(x, target=y)      # noqa: E731
+    for _ in range(args.warmup):
+        step()
+    sizes = shape_bytes(tr.model, step)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(args.steps):
+            step()
+        torch.cuda.synchronize()
+    tr.close()
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "trace.json")
+        prof.export_chrome_trace(path)
+        with open(path) as f:
+            trace = json.load(f)
+    per_cls, names = collections.Counter(), collections.defaultdict(collections.Counter)
+    for ev in trace.get("traceEvents", []):
+        if ev.get("cat") == "kernel" and "dur" in ev:
+            cls = classify(ev["name"])
+            per_cls[cls] += ev["dur"] / args.steps
+            names[cls][ev["name"][:140]] += ev["dur"] / args.steps
+    fused = fused_bn.enabled()
+    pb = pass_bytes(sizes, fused)
+    total = sum(per_cls.values())
+    rows = []
+    for cls, us in sorted(per_cls.items(), key=lambda kv: -kv[1]):
+        b = pb.get(cls)
+        rows.append({"class": cls, "ms_per_step": us / 1e3, "share": us / total, "bytes_per_step": b,
+                     "gbs": (b / (us * 1e-6) / 1e9) if b else None,
+                     "top_kernels": [[n, t / 1e3] for n, t in names[cls].most_common(3)]})
+    res = {"card": card(), "fused_bn": fused, "batch": B, "steps": args.steps, "kernel_ms_per_step": total / 1e3,
+           "bn_input_bytes": sizes, "classes": rows}
+    os.makedirs(args.out, exist_ok=True)
+    tag = f"fused{int(fused)}"
+    with open(os.path.join(args.out, f"profile_{tag}.json"), "w") as f:
+        json.dump(res, f, indent=1)
+    lines = [f"card: {res['card']}; DR_FUSED_BN={int(fused)}; batch {B}; GPU kernel time {total / 1e3:.2f} ms/step", "",
+             "| class | ms/step | share | GB/step (from shapes) | GB/s |", "|---|---|---|---|---|"]
+    for r in rows:
+        gb = f"{r['bytes_per_step'] / 1e9:.2f}" if r["bytes_per_step"] else ""
+        gbs = f"{r['gbs']:.0f}" if r["gbs"] else ""
+        lines.append(f"| {r['class']} | {r['ms_per_step']:.2f} | {100 * r['share']:.1f} % | {gb} | {gbs} |")
+    with open(os.path.join(args.out, f"profile_{tag}.md"), "w") as f:
+        f.write("\n".join(lines) + "\n")
+    print("\n".join(lines))
+    for r in rows:
+        print(r["class"], r["top_kernels"])
+
+
+if __name__ == "__main__":
+    main()
