@@ -1,9 +1,11 @@
 """Training BatchNorm fused with the ReLU and the residual add of ResNet-50, on channels_last bf16 activations.
 
 Forward runs the sm_90a kernels of ``ops/csrc/bn.cu``: torch's own channels-last statistics kernel, then one
-vectorised pass that applies BN, adds the skip branch and applies the ReLU.  The unfused graph writes and re-reads the
-BN output, the sum and the ReLU output instead.  Backward calls the ops autograd would run for the unfused graph
-(``threshold_backward``, then ``native_batch_norm_backward``), so gradients are the same ops on the same tensors.
+vectorised pass that applies BN, adds the skip branch and applies the ReLU, and saves a one-bit-per-element ReLU mask.
+The unfused graph writes and re-reads the BN output, the sum and the ReLU output instead.  Backward runs two more
+kernels of ``bn.cu`` on the output gradient and the mask: the per-channel sums in torch's reduction tree, then the
+elementwise input gradient(s).  They replace ``threshold_backward`` and ``native_batch_norm_backward``, which write and
+re-read a masked copy of the gradient.
 
 Every fused result is bitwise that of the unfused graph: same reductions, same fp32 expressions, same bf16 rounding
 points.  ``eligible()`` decides per call; anything it rejects (CPU, eval mode, fp32, another memory layout) runs the
@@ -45,54 +47,55 @@ def _stats(x, bn):
     return ops.cuda_module().bn_stats(x, bn.running_mean, bn.running_var, float(bn.momentum), float(bn.eps))
 
 
-def _bn_backward(g, x, weight, mean, invstd, eps):
-    return torch.ops.aten.native_batch_norm_backward(g, x, weight, None, None, mean, invstd, True, eps, [True, True, True])
+def _grad(go):
+    # the gradient reaching the fused op; the backward kernels read it in x's channels_last layout
+    return go.contiguous(memory_format=torch.channels_last)
 
 
 class _BNReLU(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, mean, invstd, eps):
+    def forward(ctx, x, weight, bias, mean, invstd):
         from .. import ops
-        y = ops.cuda_module().bn_apply(0, x, [mean, invstd, weight, bias])
-        ctx.save_for_backward(x, weight, mean, invstd, y)
-        ctx.eps = eps
+        y, mask = ops.cuda_module().bn_apply(0, x, [mean, invstd, weight, bias])
+        ctx.save_for_backward(x, weight, mean, invstd, mask)
         return y
 
     @staticmethod
     def backward(ctx, gy):
-        x, weight, mean, invstd, y = ctx.saved_tensors
-        g = torch.ops.aten.threshold_backward(gy, y, 0)
-        dx, dw, db = _bn_backward(g, x, weight, mean, invstd, ctx.eps)
-        return dx, dw, db, None, None, None
+        from .. import ops
+        x, weight, mean, invstd, mask = ctx.saved_tensors
+        dx, dw, db = ops.cuda_module().bn_backward(0, _grad(gy), mask, x, [mean, invstd, weight])
+        return dx, dw, db, None, None
 
 
 class _BNAddReLU(torch.autograd.Function):
-    """relu(bn(x) + z) for an identity skip, relu(bn(x) + bn_z(z)) for a downsample skip (``pz`` given)."""
+    """relu(bn(x) + z) for an identity skip, relu(bn(x) + bn_z(z)) for a downsample skip (``wz`` given)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, mean, invstd, eps, z, wz, bz, mz, iz, eps_z):
+    def forward(ctx, x, weight, bias, mean, invstd, z, wz, bz, mz, iz):
         from .. import ops
         mod = ops.cuda_module()
         if wz is None:
-            o = mod.bn_apply(1, x, [mean, invstd, weight, bias], z)
-            ctx.save_for_backward(x, weight, mean, invstd, o)
+            o, mask = mod.bn_apply(1, x, [mean, invstd, weight, bias], z)
+            ctx.save_for_backward(x, weight, mean, invstd, mask)
         else:
-            o = mod.bn_apply(2, x, [mean, invstd, weight, bias], z, [mz, iz, wz, bz])
-            ctx.save_for_backward(x, weight, mean, invstd, o, z, wz, mz, iz)
-        ctx.eps, ctx.eps_z, ctx.has_bn_z = eps, eps_z, wz is not None
+            o, mask = mod.bn_apply(2, x, [mean, invstd, weight, bias], z, [mz, iz, wz, bz])
+            ctx.save_for_backward(x, weight, mean, invstd, mask, z, wz, mz, iz)
+        ctx.has_bn_z = wz is not None
         return o
 
     @staticmethod
     def backward(ctx, go):
+        from .. import ops
+        mod = ops.cuda_module()
         saved = ctx.saved_tensors
-        x, weight, mean, invstd, o = saved[:5]
-        g = torch.ops.aten.threshold_backward(go, o, 0)
-        dx, dw, db = _bn_backward(g, x, weight, mean, invstd, ctx.eps)
+        x, weight, mean, invstd, mask = saved[:5]
         if not ctx.has_bn_z:
-            return dx, dw, db, None, None, None, g, None, None, None, None, None
+            dx, dw, db, g = mod.bn_backward(1, _grad(go), mask, x, [mean, invstd, weight])
+            return dx, dw, db, None, None, g, None, None, None, None
         z, wz, mz, iz = saved[5:]
-        dz, dwz, dbz = _bn_backward(g, z, wz, mz, iz, ctx.eps_z)
-        return dx, dw, db, None, None, None, dz, dwz, dbz, None, None, None
+        dx, dw, db, dz, dwz, dbz = mod.bn_backward(2, _grad(go), mask, x, [mean, invstd, weight], z, [mz, iz, wz])
+        return dx, dw, db, None, None, dz, dwz, dbz, None, None
 
 
 def bn_relu(x: torch.Tensor, bn: nn.BatchNorm2d) -> torch.Tensor:
@@ -100,7 +103,7 @@ def bn_relu(x: torch.Tensor, bn: nn.BatchNorm2d) -> torch.Tensor:
     if not eligible(x, bn):
         return F.relu(bn(x), inplace=True)
     mean, invstd = _stats(x, bn)
-    return _BNReLU.apply(x, bn.weight, bn.bias, mean, invstd, bn.eps)
+    return _BNReLU.apply(x, bn.weight, bn.bias, mean, invstd)
 
 
 def bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, idt: torch.Tensor) -> torch.Tensor:
@@ -108,7 +111,7 @@ def bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, idt: torch.Tensor) -> torch
     if not (eligible(x, bn) and idt.dtype == x.dtype and idt.shape == x.shape and idt.stride() == x.stride()):
         return F.relu(bn(x) + idt, inplace=True)
     mean, invstd = _stats(x, bn)
-    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, bn.eps, idt, None, None, None, None, None)
+    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, idt, None, None, None, None)
 
 
 def bn_bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, xd: torch.Tensor, bnd: nn.BatchNorm2d) -> torch.Tensor:
@@ -117,4 +120,4 @@ def bn_bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, xd: torch.Tensor, bnd: n
         return F.relu(bn(x) + bnd(xd), inplace=True)
     md, id_ = _stats(xd, bnd)
     mean, invstd = _stats(x, bn)
-    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, bn.eps, xd, bnd.weight, bnd.bias, md, id_, bnd.eps)
+    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, xd, bnd.weight, bnd.bias, md, id_)

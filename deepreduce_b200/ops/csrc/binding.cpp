@@ -295,27 +295,92 @@ static dr::BnParams bn_params(const std::vector<torch::Tensor>& p, int64_t C) {
   return {p[0].data_ptr<float>(), p[1].data_ptr<float>(), p[2].data_ptr<float>(), p[3].data_ptr<float>()};
 }
 
+static void check_like_x(const torch::Tensor& t, const torch::Tensor& x, const char* what) {
+  TORCH_CHECK(t.sizes() == x.sizes() && t.strides() == x.strides() && t.scalar_type() == torch::kBFloat16 &&
+                  t.device() == x.device(),
+              "bn: ", what, " must match x in shape, layout, dtype and device");
+}
+
 // mode 0: relu(bn(x)); 1: relu(bn(x) + z); 2: relu(bn(x) + bn_z(z)).  p / pz = (mean, invstd, weight, bias).
-static torch::Tensor bn_apply(int64_t mode, torch::Tensor x, std::vector<torch::Tensor> p, c10::optional<torch::Tensor> z,
-                              std::vector<torch::Tensor> pz) {
+// -> (out, mask): mask is uint8 [N*H*W, C/8], bit i of byte g set where out[..., 8g + i] is not <= 0.
+static std::vector<torch::Tensor> bn_apply(int64_t mode, torch::Tensor x, std::vector<torch::Tensor> p,
+                                           c10::optional<torch::Tensor> z, std::vector<torch::Tensor> pz) {
   check_bn_input(x);
   const int64_t C = x.size(1);
   const dr::BnParams px = bn_params(p, C);
   dr::BnParams pzz{};
   const void* zp = nullptr;
   if (mode != 0) {
-    TORCH_CHECK(z.has_value() && z->sizes() == x.sizes() && z->strides() == x.strides() &&
-                    z->scalar_type() == torch::kBFloat16 && z->device() == x.device(),
-                "bn: z must match x in shape, layout, dtype and device");
+    TORCH_CHECK(z.has_value(), "bn: mode ", mode, " needs z");
+    check_like_x(*z, x, "z");
     zp = z->data_ptr();
     if (mode == 2) pzz = bn_params(pz, C);
   }
   c10::cuda::CUDAGuard g(x.device());
+  const int64_t rows = x.numel() / C;
   auto out = torch::empty_like(x);
-  cudaError_t e = dr::launch_bn_apply((int)mode, x.data_ptr(), px, zp, pzz, out.data_ptr(), x.numel() / C, (int)C,
-                                      cur_stream());
+  auto mask = torch::empty({rows, C / 8}, x.options().dtype(torch::kUInt8));
+  cudaError_t e = dr::launch_bn_apply((int)mode, x.data_ptr(), px, zp, pzz, out.data_ptr(), mask.data_ptr(), rows,
+                                      (int)C, cur_stream());
   TORCH_CHECK(e == cudaSuccess, "bn_apply: ", cudaGetErrorString(e));
-  return out;
+  return {out, mask};
+}
+
+static dr::BnParams bn_bwd_params(const std::vector<torch::Tensor>& p, int64_t C) {
+  TORCH_CHECK(p.size() == 3, "bn_backward: expected (mean, invstd, weight)");
+  const char* names[3] = {"mean", "invstd", "weight"};
+  for (int i = 0; i < 3; ++i) check_chan(p[i], C, names[i]);
+  return {p[0].data_ptr<float>(), p[1].data_ptr<float>(), p[2].data_ptr<float>(), nullptr};
+}
+
+// Backward of bn_apply(mode) from the output gradient go and bn_apply's mask; p / pz = (mean, invstd, weight).
+// The gradient of the ReLU input is g = mask ? go : 0.  Returns
+//   mode 0: (dx, dw, db);  1: (dx, dw, db, g) (g is the gradient of z);  2: (dx, dw, db, dz, dw_z, db_z).
+// Bitwise native_batch_norm_backward(threshold_backward(go, out, 0), ...) of torch's channels-last kernels.
+static std::vector<torch::Tensor> bn_backward(int64_t mode, torch::Tensor go, torch::Tensor mask, torch::Tensor x,
+                                              std::vector<torch::Tensor> p, c10::optional<torch::Tensor> z,
+                                              std::vector<torch::Tensor> pz) {
+  TORCH_CHECK(mode >= 0 && mode <= 2, "bn_backward: mode must be 0, 1 or 2");
+  check_bn_input(x);
+  TORCH_CHECK(go.sizes() == x.sizes() && go.scalar_type() == torch::kBFloat16 && go.device() == x.device() &&
+                  go.is_contiguous(at::MemoryFormat::ChannelsLast),
+              "bn_backward: go must be a channels_last bf16 tensor of x's shape on x's device");
+  const int64_t C = x.size(1), rows = x.numel() / C;
+  TORCH_CHECK(mask.is_cuda() && mask.scalar_type() == torch::kUInt8 && mask.is_contiguous() &&
+                  mask.numel() == rows * (C / 8) && mask.device() == x.device(),
+              "bn_backward: mask must be bn_apply's mask for x");
+  c10::cuda::CUDAGuard guard(x.device());
+  int block_y = 0, grid_y = 0;
+  dr::bn_backward_tree(rows, (int)C, &block_y, &grid_y);
+  // every virtual thread of torch's tree owns at least one row, so no slot of its block tree is left unwritten
+  TORCH_CHECK((int64_t)block_y * grid_y <= rows, "bn_backward: reduction tree wider than the rows");
+  const int n_sums = mode == 2 ? 3 : 2;
+  auto f32 = x.options().dtype(torch::kFloat32);
+  auto sums = torch::empty({n_sums, C}, f32);
+  auto staging = grid_y > 1 ? torch::empty({n_sums, grid_y, C}, f32) : torch::Tensor();
+  auto dx = torch::empty_like(x), dw = torch::empty({C}, f32), db = torch::empty({C}, f32);
+  dr::BnBwd b{};
+  b.go = go.data_ptr(); b.mask = mask.data_ptr<uint8_t>(); b.x = x.data_ptr();
+  b.px = bn_bwd_params(p, C);
+  b.dx = dx.data_ptr(); b.sums = sums.data_ptr<float>(); b.staging = grid_y > 1 ? staging.data_ptr<float>() : nullptr;
+  b.dw = dw.data_ptr<float>(); b.db = db.data_ptr<float>();
+  std::vector<torch::Tensor> res{dx, dw, db};
+  if (mode == 1) {
+    auto g = torch::empty_like(x);
+    b.g = g.data_ptr();
+    res.push_back(g);
+  } else if (mode == 2) {
+    TORCH_CHECK(z.has_value(), "bn_backward: mode 2 needs z");
+    check_like_x(*z, x, "z");
+    b.z = z->data_ptr();
+    b.pz = bn_bwd_params(pz, C);
+    auto dz = torch::empty_like(x), dwz = torch::empty({C}, f32), dbz = torch::empty({C}, f32);
+    b.dz = dz.data_ptr(); b.dwz = dwz.data_ptr<float>(); b.dbz = dbz.data_ptr<float>();
+    res.insert(res.end(), {dz, dwz, dbz});
+  }
+  cudaError_t e = dr::launch_bn_backward((int)mode, b, rows, (int)C, cur_stream());
+  TORCH_CHECK(e == cudaSuccess, "bn_backward: ", cudaGetErrorString(e));
+  return res;
 }
 
 // ---------------------------------------------------------------------------
@@ -552,6 +617,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_stats", &bn_stats);
   m.def("bn_apply", &bn_apply, py::arg("mode"), py::arg("x"), py::arg("p"), py::arg("z") = py::none(),
         py::arg("pz") = std::vector<torch::Tensor>{});
+  m.def("bn_backward", &bn_backward, py::arg("mode"), py::arg("go"), py::arg("mask"), py::arg("x"), py::arg("p"),
+        py::arg("z") = py::none(), py::arg("pz") = std::vector<torch::Tensor>{});
   m.def("rle_runs", &rle_runs);
   m.def("rle_indices", &rle_indices);
   m.def("arena_alloc", &arena_alloc);

@@ -58,8 +58,19 @@ void launch_u8_to_nhwc_norm(const uint8_t* in, void* out_bf16, int64_t n_pix, co
 struct BnParams { const float* mean; const float* invstd; const float* weight; const float* bias; };
 cudaError_t launch_bn_update_stats(const float* mean, float* var_invstd, float* running_mean, float* running_var, int C,
                                    float momentum, float bessel, float eps, cudaStream_t st);
-// mode 0: relu(bn(x)); 1: relu(bn(x) + z); 2: relu(bn(x) + bn_z(z))
+// mode 0: relu(bn(x)); 1: relu(bn(x) + z); 2: relu(bn(x) + bn_z(z)).  Also writes the ReLU mask, uint8 [rows][C / 8].
 cudaError_t launch_bn_apply(int mode, const void* x, const BnParams& px, const void* z, const BnParams& pz, void* out,
-                            int64_t rows, int C, cudaStream_t st);
+                            void* mask, int64_t rows, int C, cudaStream_t st);
+// Backward of bn_apply's mode from the output gradient go and the mask.  bf16 tensors have x's shape; per-channel fp32
+// outputs have C elements; sums = [sum_dy, sum_dy_xmu(, sum_dy_xmu_z)] x C; staging = same x grid_y (bn_backward_tree)
+// when grid_y > 1.  Mode 1 also writes the masked gradient g; mode 2 reads z and writes dz, dwz, dbz.
+struct BnBwd {
+  const void* go; const uint8_t* mask; const void* x; const void* z;
+  BnParams px, pz;      // bias unused
+  void* dx; void* dz; void* g;
+  float* sums; float* staging; float* dw; float* db; float* dwz; float* dbz;
+};
+void bn_backward_tree(int64_t rows, int C, int* block_y, int* grid_y);
+cudaError_t launch_bn_backward(int mode, const BnBwd& b, int64_t rows, int C, cudaStream_t st);
 
 }  // namespace dr
