@@ -1,7 +1,8 @@
 """Training BatchNorm fused with the ReLU and the residual add of ResNet-50, on channels_last bf16 activations.
 
-Forward runs the sm_90a kernels of ``ops/csrc/bn.cu``: torch's own channels-last statistics kernel, then one
-vectorised pass that applies BN, adds the skip branch and applies the ReLU, and saves a one-bit-per-element ReLU mask.
+Forward runs the sm_90a kernels of ``ops/csrc/bn.cu``: a statistics pass that reproduces torch's channels-last Welford
+reduction tree and updates the running stats, then one vectorised pass that applies BN, adds the skip branch and applies
+the ReLU, and saves a one-bit-per-element ReLU mask.
 The unfused graph writes and re-reads the BN output, the sum and the ReLU output instead.  Backward runs two more
 kernels of ``bn.cu`` on the output gradient and the mask: the per-channel sums in torch's reduction tree, then the
 elementwise input gradient(s).  They replace ``threshold_backward`` and ``native_batch_norm_backward``, which write and

@@ -246,7 +246,7 @@ static torch::Tensor u8_to_nhwc_norm(torch::Tensor in, std::vector<double> mean,
 // training BatchNorm (+ ReLU, + residual add) on channels_last bf16 (bn.cu)
 // ---------------------------------------------------------------------------
 // torch's own channels-last Welford statistics, the instantiation native_batch_norm runs for bf16 input (exported by
-// libtorch_cuda): mean and biased variance come out bitwise as in the unfused graph.
+// libtorch_cuda).  bn_stats falls back to it where bn.cu's mirror of its tree does not apply.
 namespace at::native {
 struct Var;
 template <typename scalar_t, typename VarTransform>
@@ -267,9 +267,12 @@ static void check_chan(const torch::Tensor& t, int64_t C, const char* what) {
               " must be a contiguous float32 CUDA tensor of C elements");
 }
 
-// -> (save_mean, save_invstd); updates running_mean / running_var in place like native_batch_norm(training=True)
+// -> (save_mean, save_invstd); updates running_mean / running_var in place like native_batch_norm(training=True).
+// bn.cu's statistics pass reproduces torch's channels-last Welford tree, so the results are bitwise torch's.  torch's
+// kernel (+ bn.cu's running-stats update) runs instead with torch_kernel, for A/B comparisons, and for a tree with more
+// virtual threads than rows, which flexible_launch_configs does not produce but the mirror does not cover.
 static std::vector<torch::Tensor> bn_stats(torch::Tensor x, torch::Tensor running_mean, torch::Tensor running_var,
-                                           double momentum, double eps) {
+                                           double momentum, double eps, bool torch_kernel) {
   check_bn_input(x);
   const int64_t C = x.size(1);
   check_chan(running_mean, C, "running_mean");
@@ -278,14 +281,25 @@ static std::vector<torch::Tensor> bn_stats(torch::Tensor x, torch::Tensor runnin
   TORCH_CHECK(N > 1, "bn: expected more than 1 value per channel when training");
   c10::cuda::CUDAGuard g(x.device());
   auto opts = x.options().dtype(torch::kFloat32);
-  auto mean = torch::empty({C}, opts), var = torch::empty({C}, opts);
-  at::native::batch_norm_stats_channels_last_cuda_template<c10::BFloat16, at::native::Var>(mean, var, x, eps);
+  auto mean = torch::empty({C}, opts), invstd = torch::empty({C}, opts);
   const float bessel = static_cast<float>(static_cast<double>(N) / static_cast<double>(N - 1));
-  cudaError_t e = dr::launch_bn_update_stats(mean.data_ptr<float>(), var.data_ptr<float>(), running_mean.data_ptr<float>(),
-                                             running_var.data_ptr<float>(), (int)C, (float)momentum, bessel, (float)eps,
-                                             cur_stream());
+  int block_y = 0, grid_y = 0;
+  dr::bn_row_tree(N, (int)C, &block_y, &grid_y);
+  cudaError_t e;
+  if (!torch_kernel && (int64_t)block_y * grid_y <= N) {
+    auto staging = grid_y > 1 ? torch::empty({(2 * C + 1) * grid_y}, opts) : torch::Tensor();
+    const dr::BnStats s{x.data_ptr(), mean.data_ptr<float>(), invstd.data_ptr<float>(), running_mean.data_ptr<float>(),
+                        running_var.data_ptr<float>(), grid_y > 1 ? staging.data_ptr<float>() : nullptr,
+                        (float)momentum, bessel, (float)eps};
+    e = dr::launch_bn_stats(s, N, (int)C, cur_stream());
+  } else {
+    at::native::batch_norm_stats_channels_last_cuda_template<c10::BFloat16, at::native::Var>(mean, invstd, x, eps);
+    e = dr::launch_bn_update_stats(mean.data_ptr<float>(), invstd.data_ptr<float>(), running_mean.data_ptr<float>(),
+                                   running_var.data_ptr<float>(), (int)C, (float)momentum, bessel, (float)eps,
+                                   cur_stream());
+  }
   TORCH_CHECK(e == cudaSuccess, "bn_stats: ", cudaGetErrorString(e));
-  return {mean, var};
+  return {mean, invstd};
 }
 
 static dr::BnParams bn_params(const std::vector<torch::Tensor>& p, int64_t C) {
@@ -351,7 +365,7 @@ static std::vector<torch::Tensor> bn_backward(int64_t mode, torch::Tensor go, to
               "bn_backward: mask must be bn_apply's mask for x");
   c10::cuda::CUDAGuard guard(x.device());
   int block_y = 0, grid_y = 0;
-  dr::bn_backward_tree(rows, (int)C, &block_y, &grid_y);
+  dr::bn_row_tree(rows, (int)C, &block_y, &grid_y);
   // every virtual thread of torch's tree owns at least one row, so no slot of its block tree is left unwritten
   TORCH_CHECK((int64_t)block_y * grid_y <= rows, "bn_backward: reduction tree wider than the rows");
   const int n_sums = mode == 2 ? 3 : 2;
@@ -614,7 +628,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("delta_bp128_encode", &delta_bp128_encode);
   m.def("delta_bp128_decode", &delta_bp128_decode);
   m.def("u8_to_nhwc_norm", &u8_to_nhwc_norm);
-  m.def("bn_stats", &bn_stats);
+  m.def("bn_stats", &bn_stats, py::arg("x"), py::arg("running_mean"), py::arg("running_var"), py::arg("momentum"),
+        py::arg("eps"), py::arg("torch_kernel") = false);
   m.def("bn_apply", &bn_apply, py::arg("mode"), py::arg("x"), py::arg("p"), py::arg("z") = py::none(),
         py::arg("pz") = std::vector<torch::Tensor>{});
   m.def("bn_backward", &bn_backward, py::arg("mode"), py::arg("go"), py::arg("mask"), py::arg("x"), py::arg("p"),

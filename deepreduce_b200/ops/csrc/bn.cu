@@ -1,9 +1,8 @@
 // Training-mode BatchNorm for NHWC (channels_last) bf16 activations, fused with the ReLU and the residual add that
 // follow it in ResNet-50.  The results are bitwise those of the unfused graph (native_batch_norm -> relu_ -> add ->
 // relu_), because every expression and every bf16 rounding point is kept:
-//   * per-channel mean / biased var come from torch's own channels-last Welford kernel (binding.cpp), so the
-//     reduction order is torch's;
-//   * running stats and invstd: the expressions of torch's batch_norm_update_stats_and_invert;
+//   * per-channel mean / biased var: torch's channels-last Welford tree, operation for operation (bn_stats_kernel);
+//   * running stats and invstd: the expressions of torch's batch_norm_update_stats_and_invert, in the same pass;
 //   * apply: torch's channels-last transform w * (x - mean) * invstd + shift, which compiles to
 //     fma(w * (x - mean), invstd, shift) (checked in the sm_90 SASS of batch_norm_transform_input_channels_last_kernel),
 //     rounded to bf16;
@@ -15,7 +14,7 @@
 // The apply pass also writes the ReLU mask (one bit per element: !(out <= 0), threshold_backward's condition), and
 // backward runs on it instead of threshold_backward + native_batch_norm_backward:
 //   * reduce: per-channel sum(g) and sum(g * (x - mean)) with g = mask ? go : +0, in the reduction tree of torch's
-//     batch_norm_backward_reduce_channels_last_kernel (see BwdTree), so the sums are bitwise torch's;
+//     batch_norm_backward_reduce_channels_last_kernel (see RowTree), so the sums are bitwise torch's;
 //   * elementwise: torch's dx expression, pinned to the FMA placement of its sm_90 SASS.
 #include <cuda_bf16.h>
 
@@ -104,21 +103,217 @@ __global__ void __launch_bounds__(kApplyThreads) bn_apply_kernel(const __nv_bflo
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// backward
+// reduction trees
 // ---------------------------------------------------------------------------------------------------------------------
-// The reduction tree of torch's batch_norm_backward_reduce_channels_last_kernel<4> for `rows` x C (launch config from
-// flexible_launch_configs(rows, C, coop = true); block_x does not change a column's sums).  Virtual thread
-// v = block * block_y + y (of S = block_y * grid_y) keeps kBwdLoads accumulators; accumulator j sums rows
-// v + (i * kBwdLoads + j) * S for i = 0, 1, ... from 0.0f (rows past the end add g = 0, x = 0, as torch's loads do).  Then
-// ((a0 + a1) + a2) + a3, a pairwise tree over y inside each block (offsets block_y / 2 ... 1), and for grid_y > 1 the
-// same tree over y of 0.0f + s[y] + s[y + block_y] + ... of the block results s.  Nothing here is specific to the
-// backward sums: a statistics kernel that mirrors torch's Welford tree indexes rows the same way.
-struct BwdTree {
+// The row indexing of torch's channels-last reductions (batch_norm_collect_statistics_channels_last_kernel<4> and
+// batch_norm_backward_reduce_channels_last_kernel<4>) for `rows` x C, launch config from
+// flexible_launch_configs(rows, C, coop = true); block_x does not change a column's result.  Virtual thread
+// v = block * block_y + y (of S = block_y * grid_y) keeps kLoads accumulators; accumulator j takes rows
+// v + (i * kLoads + j) * S for i < loops(rows).  Then ((a0 . a1) . a2) . a3, a pairwise tree over y inside each block
+// (offsets block_y / 2 ... 1), and for grid_y > 1 the same tree over y of e . s[y] . s[y + block_y] . ... of the block
+// results s, from the identity e.  For the backward sums "." is + and e = 0.0f; for the statistics it is Welford's merge
+// and e = (count 0, mean 0, m2n 0).
+struct RowTree {
   int block_y, grid_y;
   __host__ __device__ int S() const { return block_y * grid_y; }
-  __host__ __device__ int loops(int rows) const { return 1 + (rows - 1) / (S() * kBwdLoads); }
-  static constexpr int kBwdLoads = 4;       // torch's ELEMENTS_PER_ITER
+  __host__ __device__ int loops(int rows) const { return 1 + (rows - 1) / (S() * kLoads); }
+  static constexpr int kLoads = 4;       // torch's ELEMENTS_PER_ITER
 };
+
+// ---------------------------------------------------------------------------------------------------------------------
+// forward statistics
+// ---------------------------------------------------------------------------------------------------------------------
+// Per-channel mean and biased variance, bitwise those of torch's batch_norm_collect_statistics_channels_last_kernel
+// <Var, BFloat16, float, 4>: the same RowTree and the same fp32 operations, each pinned to the placement of that
+// kernel's sm_90 SASS.  Only the thread layout differs: accumulator j of a virtual thread lives in a physical thread of
+// its own (4 per virtual thread, 8 channels each, one 16-byte load per row), and the four are merged in torch's order
+// through shared memory.
+constexpr int kStatsThreads = 256;    // at most; 78 registers per thread, 3 blocks per SM
+
+// Welford update of one element; inv = 1 / count (0 for a row past the end, with x = 0 and valid = 0: torch still runs
+// this arithmetic there, and a non-finite mean makes it NaN).  SASS: FADD d0 = x - mean; FFMA mean = d0 * inv + mean;
+// FADD d1 = x - mean; FMUL t = d0 * d1; FFMA m2n = t * valid + m2n.
+__device__ __forceinline__ void welford_update(float x, float inv, float valid, float& mean, float& m2n) {
+  const float d0 = __fsub_rn(x, mean);
+  mean = __fmaf_rn(d0, inv, mean);
+  const float d1 = __fsub_rn(x, mean);
+  m2n = __fmaf_rn(__fmul_rn(d0, d1), valid, m2n);
+}
+
+// torch's welford_merge_element of (n_new, mean_new, m2n_new) into (n, mean, m2n), kN channels that share the counts.
+// SASS: factor = 1.0f / max(1, n + n_new) (correctly rounded); FADD d = mean - mean_new;
+// FMUL u = d * d; FMUL u *= n_new; FMUL u *= n; FFMA u = u * factor + m2n_new; FADD m2n += u;
+// and mean = (mean_new * n_new + mean * n) * factor, whose contraction nvcc chose per inlined call site:
+//   kFuseNew (the merge of the 4 accumulators): FMUL t = mean * n; FFMA mean = mean_new * n_new + t;
+//   otherwise (the vertical tree, the cross-block merge): FMUL t = mean_new * n_new; FFMA mean = mean * n + t;
+// then FMUL mean *= factor.
+template <int kN, bool kFuseNew>
+__device__ __forceinline__ void welford_merge(int& n, float* mean, float* m2n, int n_new, const float* mean_new,
+                                              const float* m2n_new) {
+  const float fn = (float)n, fn_new = (float)n_new;
+  const float factor = __frcp_rn((float)max(1, n + n_new));
+#pragma unroll
+  for (int i = 0; i < kN; ++i) {
+    const float d = __fsub_rn(mean[i], mean_new[i]);
+    const float s = kFuseNew ? __fmaf_rn(mean_new[i], fn_new, __fmul_rn(mean[i], fn))
+                             : __fmaf_rn(mean[i], fn, __fmul_rn(mean_new[i], fn_new));
+    mean[i] = __fmul_rn(s, factor);
+    const float u = __fmul_rn(__fmul_rn(__fmul_rn(d, d), fn_new), fn);
+    m2n[i] = __fadd_rn(m2n[i], __fmaf_rn(u, factor, m2n_new[i]));
+  }
+  n += n_new;
+}
+
+// Shared-memory slots for a Welford merge across threads: mean[slots][kN], m2n[slots][kN], count[slots].
+template <int kN>
+struct WelfordSlots {
+  float* mean; float* m2n; int* count;
+  __device__ WelfordSlots(float* sh, int slots)
+      : mean(sh), m2n(sh + slots * kN), count(reinterpret_cast<int*>(sh + 2 * slots * kN)) {}
+  __device__ void put(int s, int n, const float* m, const float* q) const {
+#pragma unroll
+    for (int i = 0; i < kN; ++i) { mean[s * kN + i] = m[i]; m2n[s * kN + i] = q[i]; }
+    count[s] = n;
+  }
+  template <bool kFuseNew>
+  __device__ void merge_from(int s, int& n, float* m, float* q) const {
+    float mn[kN], qn[kN];
+#pragma unroll
+    for (int i = 0; i < kN; ++i) { mn[i] = mean[s * kN + i]; qn[i] = m2n[s * kN + i]; }
+    welford_merge<kN, kFuseNew>(n, m, q, count[s], mn, qn);
+  }
+  static size_t bytes(int slots) { return (size_t)slots * (2 * kN * sizeof(float) + sizeof(int)); }
+};
+
+// torch's welford_merge_block_vertical: pairwise tree over y (offsets block_y / 2 ... 1), result at y == 0.  Slot of y
+// is base + y * stride; threads with !part take part in the barriers only.
+template <int kN>
+__device__ __forceinline__ void welford_tree_over_y(const WelfordSlots<kN>& sl, bool part, int y, int block_y, int base,
+                                                    int stride, int& n, float* mean, float* m2n) {
+  for (int off = block_y / 2; off > 0; off >>= 1) {
+    if (part && y < 2 * off) sl.put(base + y * stride, n, mean, m2n);
+    __syncthreads();
+    if (part && y < off) sl.template merge_from<false>(base + (y + off) * stride, n, mean, m2n);
+    __syncthreads();
+  }
+}
+
+struct StatsOut {
+  float* mean; float* invstd; float* running_mean; float* running_var;
+  float* st_mean; float* st_m2n; int* st_count;     // [grid_y][C], [grid_y][C], [grid_y] when grid_y > 1
+  float momentum, bessel, eps;
+};
+
+// The end of torch's statistics kernel (var = m2n / count, Var transform) followed by the expressions of
+// batch_norm_update_stats_and_invert, as their SASS places them: FADD a = 1 - momentum; FMUL t = running * a;
+// FFMA running = new * momentum + t; the unbiased variance is FMUL var * bessel; invstd = rsqrtf(var + eps).
+__device__ __forceinline__ void stats_store(const StatsOut& o, int c, int n, float mean, float m2n) {
+  const float var = __fdiv_rn(m2n, (float)n);
+  const float keep = __fsub_rn(1.f, o.momentum);
+  o.mean[c] = mean;
+  o.invstd[c] = rsqrtf(__fadd_rn(var, o.eps));
+  o.running_mean[c] = __fmaf_rn(mean, o.momentum, __fmul_rn(o.running_mean[c], keep));
+  o.running_var[c] = __fmaf_rn(__fmul_rn(var, o.bessel), o.momentum, __fmul_rn(o.running_var[c], keep));
+}
+
+// Block = gpc channel groups x kLoads accumulators x block_y virtual threads of virtual block blockIdx.y; thread
+// (g, j, y) walks rows v + (i * kLoads + j) * S with the loads of the next kAhead iterations issued before the current
+// ones are used.  grid_y == 1: the block writes the final results; else its partial goes to staging.
+__global__ void __launch_bounds__(kStatsThreads) bn_stats_kernel(const __nv_bfloat16* __restrict__ x, StatsOut o,
+                                                                 RowTree t, int rows, int C) {
+  constexpr int L = RowTree::kLoads;
+  constexpr int kAhead = 4;
+  extern __shared__ float sh[];
+  const int gpc = blockDim.x / (L * t.block_y);
+  const int g = threadIdx.x % gpc, j = (threadIdx.x / gpc) % L, y = threadIdx.x / (gpc * L);
+  const int group = blockIdx.x * gpc + g;
+  const bool live = group * kVec < C;
+  const int c = live ? group * kVec : 0;
+  const int S = t.S();
+  const int n_loops = t.loops(rows);
+  const int r0 = blockIdx.y * t.block_y + y + j * S;      // row of iteration i: r0 + i * L * S
+  const int rstep = L * S;
+  float mean[kVec], m2n[kVec];
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) mean[i] = m2n[i] = 0.f;
+  int n = 0;
+  auto load = [&](uint4* b, int i0) {
+#pragma unroll
+    for (int u = 0; u < kAhead; ++u) {
+      const int r = r0 + (i0 + u) * rstep;
+      b[u] = live && i0 + u < n_loops && r < rows ? *reinterpret_cast<const uint4*>(x + (size_t)r * C + c) : uint4{};
+    }
+  };
+  uint4 cur[kAhead];
+  load(cur, 0);
+  for (int i0 = 0; i0 < n_loops; i0 += kAhead) {
+    uint4 nxt[kAhead];
+    load(nxt, i0 + kAhead);
+#pragma unroll
+    for (int u = 0; u < kAhead; ++u) {
+      const int i = i0 + u;
+      if (i >= n_loops) break;
+      // for a row in range, count = i + 1 in every accumulator, so 1 / count is one correctly rounded reciprocal
+      const bool valid = r0 + i * rstep < rows;
+      const float inv = valid ? __frcp_rn((float)(i + 1)) : 0.f;
+      const float fv = valid ? 1.f : 0.f;
+      n += valid;
+      const __nv_bfloat16* hx = reinterpret_cast<const __nv_bfloat16*>(&cur[u]);
+#pragma unroll
+      for (int k = 0; k < kVec; ++k) welford_update(__bfloat162float(hx[k]), inv, fv, mean[k], m2n[k]);
+    }
+#pragma unroll
+    for (int u = 0; u < kAhead; ++u) cur[u] = nxt[u];
+  }
+  // ((a0 . a1) . a2) . a3 in the thread of accumulator 0, then the tree over y
+  const WelfordSlots<kVec> sl(sh, blockDim.x);
+  sl.put(threadIdx.x, n, mean, m2n);
+  __syncthreads();
+  if (j == 0) {
+#pragma unroll
+    for (int a = 1; a < L; ++a) sl.merge_from<true>(threadIdx.x + a * gpc, n, mean, m2n);
+  }
+  __syncthreads();
+  welford_tree_over_y<kVec>(sl, j == 0, y, t.block_y, g, gpc * L, n, mean, m2n);
+  if (j != 0 || y != 0 || !live) return;
+  if (t.grid_y == 1) {
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) stats_store(o, c + i, n, mean[i], m2n[i]);
+    return;
+  }
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    o.st_mean[(size_t)blockIdx.y * C + c + i] = mean[i];
+    o.st_m2n[(size_t)blockIdx.y * C + c + i] = m2n[i];
+  }
+  if (group == 0) o.st_count[blockIdx.y] = n;
+}
+
+// grid_y > 1: the cross-block step of torch's kernel (its last block's code).  Block = cols channels x block_y; thread
+// (col, y) merges staging rows y, y + block_y, ... into (0, 0, 0), and the tree over y combines them.
+__global__ void bn_stats_finalize_kernel(StatsOut o, RowTree t, int C) {
+  extern __shared__ float sh[];
+  const int cols = blockDim.x / t.block_y;
+  const int col = threadIdx.x % cols, y = threadIdx.x / cols;
+  const int c = blockIdx.x * cols + col;
+  int n = 0;
+  float mean = 0.f, m2n = 0.f;
+  if (c < C)
+    for (int b = y; b < t.grid_y; b += t.block_y) {
+      const float mb = o.st_mean[(size_t)b * C + c], qb = o.st_m2n[(size_t)b * C + c];
+      welford_merge<1, false>(n, &mean, &m2n, o.st_count[b], &mb, &qb);
+    }
+  const WelfordSlots<1> sl(sh, blockDim.x);
+  welford_tree_over_y<1>(sl, true, y, t.block_y, col, cols, n, &mean, &m2n);
+  if (y == 0 && c < C) stats_store(o, c, n, mean, m2n);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// backward
+// ---------------------------------------------------------------------------------------------------------------------
+// The backward sums run on the same RowTree as the statistics: accumulator j sums rows v + (i * kLoads + j) * S from
+// 0.0f (rows past the end add g = 0, x = 0, as torch's loads do), then ((a0 + a1) + a2) + a3, the pairwise tree over y,
+// and for grid_y > 1 the tree over y of 0.0f + s[y] + s[y + block_y] + ...
 
 // Pairwise tree over y of kN columns per (y, column group) thread, as torch's merge_block_vertical_backward: the
 // result is at y == 0.  sh holds n * width floats; every thread of the block calls this.
@@ -171,9 +366,9 @@ __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __n
                                                                        const float* __restrict__ mean_z,
                                                                        const float* __restrict__ invstd_z,
                                                                        __nv_bfloat16* __restrict__ g_out, BwdOut o,
-                                                                       BwdTree t, int rows, int C) {
+                                                                       RowTree t, int rows, int C) {
   constexpr int kSums = kMode == 2 ? 3 : 2;
-  constexpr int L = BwdTree::kBwdLoads;
+  constexpr int L = RowTree::kLoads;
   extern __shared__ float sh[];                    // block_y x (gpc * kVec)
   const int gpc = blockDim.x / t.block_y;
   const int tg = threadIdx.x % gpc, y = threadIdx.x / gpc;
@@ -266,7 +461,7 @@ __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __n
 
 // grid_y > 1: the cross-block step of torch's tree.  Block = cols channels x block_y; thread (col, y) sums
 // 0.0f + s[y] + s[y + block_y] + ... and the tree over y combines them.
-__global__ void bn_bwd_finalize_kernel(BwdOut o, BwdTree t, int n_sums, int C, const float* __restrict__ invstd,
+__global__ void bn_bwd_finalize_kernel(BwdOut o, RowTree t, int n_sums, int C, const float* __restrict__ invstd,
                                        const float* __restrict__ invstd_z) {
   extern __shared__ float sh[];
   const int cols = blockDim.x / t.block_y;
@@ -407,7 +602,7 @@ int last_pow2(unsigned n) {       // torch's lastPow2 (ATen/native/cuda/LaunchUt
 
 // The vertical part of torch's flexible_launch_configs(rows, C, block, grid, coop = true): MAX_BLOCK_SIZE 512,
 // OPTIMAL_TILE_W 32, ELEMENTS_PER_THREAD 16, MAX_H_BLOCK 128.
-BwdTree bwd_tree(int rows, int C) {
+RowTree row_tree(int rows, int C) {
   const int block_x = std::min(last_pow2((unsigned)C), 32);
   const int block_y = std::min(last_pow2((unsigned)((rows + 15) / 16)), 512 / block_x);
   int grid_y = std::min((rows + block_y * 16 - 1) / (block_y * 16), 128);
@@ -416,7 +611,7 @@ BwdTree bwd_tree(int rows, int C) {
 }
 
 template <int kMode>
-cudaError_t launch_bwd_reduce(const BnBwd& b, const BwdTree& t, const BwdOut& o, int rows, int C, cudaStream_t st) {
+cudaError_t launch_bwd_reduce(const BnBwd& b, const RowTree& t, const BwdOut& o, int rows, int C, cudaStream_t st) {
   const int groups = C / kVec;
   const int gpc = std::min(groups, std::max(1, kReduceThreads / t.block_y));
   const dim3 grid((groups + gpc - 1) / gpc, t.grid_y);
@@ -446,7 +641,7 @@ cudaError_t launch_bwd_elemt(const BnBwd& b, const ElemtArgs& a, int64_t rows, i
 template <int kMode>
 cudaError_t launch_backward(const BnBwd& b, int64_t rows64, int C, cudaStream_t st) {
   const int rows = (int)rows64;
-  const BwdTree t = bwd_tree(rows, C);
+  const RowTree t = row_tree(rows, C);
   const BwdOut o{b.sums, b.dw, b.db, b.dwz, b.dbz, b.staging};
   cudaError_t e = launch_bwd_reduce<kMode>(b, t, o, rows, C, st);
   if (e != cudaSuccess) return e;
@@ -463,10 +658,31 @@ cudaError_t launch_backward(const BnBwd& b, int64_t rows64, int C, cudaStream_t 
   return launch_bwd_elemt<kMode>(b, a, rows64, C, st);
 }
 
+cudaError_t launch_stats(const BnStats& s, int rows, int C, cudaStream_t st) {
+  const RowTree t = row_tree(rows, C);
+  const int grid_y = t.grid_y;
+  const StatsOut o{s.mean, s.invstd, s.running_mean, s.running_var,
+                   s.staging, s.staging + (size_t)grid_y * C, reinterpret_cast<int*>(s.staging + 2 * (size_t)grid_y * C),
+                   s.momentum, s.bessel, s.eps};
+  const int groups = C / kVec;
+  const int gpc = std::min(groups, std::max(1, kStatsThreads / (RowTree::kLoads * t.block_y)));
+  const int threads = gpc * RowTree::kLoads * t.block_y;
+  count_launch();
+  bn_stats_kernel<<<dim3((groups + gpc - 1) / gpc, grid_y), threads, WelfordSlots<kVec>::bytes(threads), st>>>(
+      reinterpret_cast<const __nv_bfloat16*>(s.x), o, t, rows, C);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess || grid_y == 1) return e;
+  const int cols = std::max(1, 512 / t.block_y);
+  const int fthreads = cols * t.block_y;
+  count_launch();
+  bn_stats_finalize_kernel<<<(C + cols - 1) / cols, fthreads, WelfordSlots<1>::bytes(fthreads), st>>>(o, t, C);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
-void bn_backward_tree(int64_t rows, int C, int* block_y, int* grid_y) {
-  const BwdTree t = bwd_tree((int)rows, C);
+void bn_row_tree(int64_t rows, int C, int* block_y, int* grid_y) {
+  const RowTree t = row_tree((int)rows, C);
   *block_y = t.block_y;
   *grid_y = t.grid_y;
 }
@@ -479,6 +695,11 @@ cudaError_t launch_bn_backward(int mode, const BnBwd& b, int64_t rows, int C, cu
     case 2: return launch_backward<2>(b, rows, C, st);
     default: return cudaErrorInvalidValue;
   }
+}
+
+cudaError_t launch_bn_stats(const BnStats& s, int64_t rows, int C, cudaStream_t st) {
+  if (rows == 0) return cudaSuccess;
+  return launch_stats(s, (int)rows, C, st);
 }
 
 cudaError_t launch_bn_update_stats(const float* mean, float* var_invstd, float* running_mean, float* running_var, int C,

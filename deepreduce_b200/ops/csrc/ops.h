@@ -56,13 +56,26 @@ void launch_u8_to_nhwc_norm(const uint8_t* in, void* out_bf16, int64_t n_pix, co
 
 // bn.cu — training BatchNorm (+ ReLU, + residual add) on NHWC bf16, C % 8 == 0; per-channel fp32 parameters
 struct BnParams { const float* mean; const float* invstd; const float* weight; const float* bias; };
+// The (block_y, grid_y) of torch's channels-last reduction tree for rows x C (flexible_launch_configs, coop = true);
+// bn_stats and bn_backward reproduce it, and need block_y * grid_y <= rows.
+void bn_row_tree(int64_t rows, int C, int* block_y, int* grid_y);
+// Training statistics, bitwise torch's channels-last Welford kernel + batch_norm_update_stats_and_invert: writes mean
+// and invstd, updates running_mean / running_var.  staging: 2 * grid_y * C + grid_y floats when grid_y > 1.
+struct BnStats {
+  const void* x;
+  float* mean; float* invstd; float* running_mean; float* running_var;
+  float* staging;
+  float momentum, bessel, eps;
+};
+cudaError_t launch_bn_stats(const BnStats& s, int64_t rows, int C, cudaStream_t st);
+// torch's batch_norm_update_stats_and_invert on the (mean, var) of torch's statistics kernel; var becomes invstd.
 cudaError_t launch_bn_update_stats(const float* mean, float* var_invstd, float* running_mean, float* running_var, int C,
                                    float momentum, float bessel, float eps, cudaStream_t st);
 // mode 0: relu(bn(x)); 1: relu(bn(x) + z); 2: relu(bn(x) + bn_z(z)).  Also writes the ReLU mask, uint8 [rows][C / 8].
 cudaError_t launch_bn_apply(int mode, const void* x, const BnParams& px, const void* z, const BnParams& pz, void* out,
                             void* mask, int64_t rows, int C, cudaStream_t st);
 // Backward of bn_apply's mode from the output gradient go and the mask.  bf16 tensors have x's shape; per-channel fp32
-// outputs have C elements; sums = [sum_dy, sum_dy_xmu(, sum_dy_xmu_z)] x C; staging = same x grid_y (bn_backward_tree)
+// outputs have C elements; sums = [sum_dy, sum_dy_xmu(, sum_dy_xmu_z)] x C; staging = same x grid_y (bn_row_tree)
 // when grid_y > 1.  Mode 1 also writes the masked gradient g; mode 2 reads z and writes dz, dwz, dbz.
 struct BnBwd {
   const void* go; const uint8_t* mask; const void* x; const void* z;
@@ -70,7 +83,6 @@ struct BnBwd {
   void* dx; void* dz; void* g;
   float* sums; float* staging; float* dw; float* db; float* dwz; float* dbz;
 };
-void bn_backward_tree(int64_t rows, int C, int* block_y, int* grid_y);
 cudaError_t launch_bn_backward(int mode, const BnBwd& b, int64_t rows, int C, cudaStream_t st);
 
 }  // namespace dr

@@ -26,7 +26,7 @@ sys.path.insert(0, ROOT)
 CLASSES = [
     ("exchange", ("dr_engine_kernel",)),
     ("bn fused apply (own)", ("bn_apply_kernel",)),
-    ("bn running-stats update (own)", ("bn_update_stats_kernel",)),
+    ("bn stats (own)", ("bn_stats_kernel", "bn_stats_finalize_kernel")),
     ("bn bwd reduce (own)", ("bn_bwd_reduce_kernel", "bn_bwd_finalize_kernel")),
     ("bn bwd elemt (own)", ("bn_bwd_elemt_kernel",)),
     ("bn stats", ("batch_norm_collect_statistics",)),
@@ -82,18 +82,18 @@ def shape_bytes(model, run_step):
 def pass_bytes(b, fused):
     """Minimum bytes each memory-bound class moves per step (reads + writes over the tensors it touches)."""
     W, T, D, I = b["W"], b["T"], b["D"], b["I"]
-    out = {"bn stats": W + T + D}
+    out = {}
     if fused:
         # forward: bn_relu reads x, writes y; tails read x3 and idt (or xd), write o; each writes a 1/16-size ReLU mask.
         # backward, per BN + ReLU kind (Ti = identity tails, D = downsample tails, T = Ti + D):
         #   reduce: W and Ti read go, x, mask (Ti also writes g); D reads go, x, z, mask
         #   elemt:  W reads go, x, mask, writes dx; Ti reads g, x, writes dx; D reads go, x, z, mask, writes dx, dz
         Ti, M = T - D, (W + T) / 16
-        out.update({"bn fused apply (own)": 2 * W + 3 * T + M, "add": 3 * I,
+        out.update({"bn stats (own)": W + T + D, "bn fused apply (own)": 2 * W + 3 * T + M, "add": 3 * I,
                     "bn bwd reduce (own)": 2 * W + 3 * Ti + 3 * D + M,
                     "bn bwd elemt (own)": 3 * W + 3 * Ti + 5 * D + (W + D) / 16})
     else:          # apply: read x, write y; relu_ in place; forward add: 2 reads + 1 write; backward junction adds
-        out.update({"bn apply": 2 * (W + T + D), "relu": 2 * (W + T), "add": 3 * T + 3 * I,
+        out.update({"bn stats": W + T + D, "bn apply": 2 * (W + T + D), "relu": 2 * (W + T), "add": 3 * T + 3 * I,
                     "bn bwd reduce": 2 * (W + T + D), "bn bwd elemt": 3 * (W + T + D), "threshold_backward": 3 * (W + T)})
     return out
 
