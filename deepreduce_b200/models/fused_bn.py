@@ -7,6 +7,9 @@ The unfused graph writes and re-reads the BN output, the sum and the ReLU output
 kernels of ``bn.cu`` on the output gradient and the mask: the per-channel sums in torch's reduction tree, then the
 elementwise input gradient(s).  They replace ``threshold_backward`` and ``native_batch_norm_backward``, which write and
 re-read a masked copy of the gradient.
+The stem's BN + ReLU is fused with the max pool that follows it (``bn_relu_maxpool``): its forward writes the pooled
+output and a one-byte winner code per pooled element instead of the ReLU output and max pool's int64 indices, and its
+backward gathers the pooled gradient back through the codes, already masked, before the two backward kernels.
 
 Every fused result is bitwise that of the unfused graph: same reductions, same fp32 expressions, same bf16 rounding
 points.  ``eligible()`` decides per call; anything it rejects (CPU, eval mode, fp32, another memory layout) runs the
@@ -97,6 +100,43 @@ class _BNAddReLU(torch.autograd.Function):
         z, wz, mz, iz = saved[5:]
         dx, dw, db, dz, dwz, dbz = mod.bn_backward(2, _grad(go), mask, x, [mean, invstd, weight], z, [mz, iz, wz])
         return dx, dw, db, None, None, dz, dwz, dbz, None, None
+
+
+class _BNReLUMaxPool(torch.autograd.Function):
+    """maxpool(relu(bn(x))) for the stem's pool (kernel 3, stride 2, padding 1).  The ReLU output is never stored: the
+    forward pass writes the pooled output and one code byte per pooled element (winner slot + its ReLU mask), and
+    backward gathers the pooled gradient back onto x's positions from the codes."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, mean, invstd):
+        from .. import ops
+        out, codes = ops.cuda_module().bn_apply_pool(x, [mean, invstd, weight, bias])
+        ctx.save_for_backward(x, weight, mean, invstd, codes)
+        return out
+
+    @staticmethod
+    def backward(ctx, go):
+        from .. import ops
+        x, weight, mean, invstd, codes = ctx.saved_tensors
+        dx, dw, db = ops.cuda_module().bn_backward(3, _grad(go), codes, x, [mean, invstd, weight])
+        return dx, dw, db, None, None
+
+
+def _stem_pool(pool: nn.Module) -> bool:
+    # the only pool bn_apply_pool implements
+    if type(pool) is not nn.MaxPool2d:
+        return False
+    pair = lambda v: tuple(v) if isinstance(v, (tuple, list)) else (v, v)      # noqa: E731
+    return (pair(pool.kernel_size) == (3, 3) and pair(pool.stride) == (2, 2) and pair(pool.padding) == (1, 1)
+            and pair(pool.dilation) == (1, 1) and not pool.ceil_mode and not pool.return_indices)
+
+
+def bn_relu_maxpool(x: torch.Tensor, bn: nn.BatchNorm2d, pool: nn.MaxPool2d) -> torch.Tensor:
+    """``pool(F.relu(bn(x), inplace=True))``."""
+    if not (eligible(x, bn) and _stem_pool(pool)):
+        return pool(F.relu(bn(x), inplace=True))
+    mean, invstd = _stats(x, bn)
+    return _BNReLUMaxPool.apply(x, bn.weight, bn.bias, mean, invstd)
 
 
 def bn_relu(x: torch.Tensor, bn: nn.BatchNorm2d) -> torch.Tensor:

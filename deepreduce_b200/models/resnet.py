@@ -9,7 +9,7 @@ from __future__ import annotations
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .fused_bn import bn_add_relu, bn_bn_add_relu, bn_relu
+from .fused_bn import bn_add_relu, bn_bn_add_relu, bn_relu, bn_relu_maxpool
 
 
 # ----------------------------------------------------------------------------
@@ -109,7 +109,7 @@ class ResNet(nn.Module):
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
 
     def forward(self, x):
-        x = self.maxpool(bn_relu(self.conv1(x), self.bn1))
+        x = bn_relu_maxpool(self.conv1(x), self.bn1, self.maxpool)
         x = self.layers(x)
         x = F.adaptive_avg_pool2d(x, 1).flatten(1)
         return self.fc(x)

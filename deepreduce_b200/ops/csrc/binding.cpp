@@ -340,6 +340,27 @@ static std::vector<torch::Tensor> bn_apply(int64_t mode, torch::Tensor x, std::v
   return {out, mask};
 }
 
+// maxpool(relu(bn(x))) for the one pool this is specialised to: kernel 3, stride 2, padding 1, dilation 1, floor mode.
+// p = (mean, invstd, weight, bias).  -> (pooled, codes): pooled is channels_last (N, C, Ho, Wo) with
+// Ho = (H - 1) / 2 + 1, bitwise max_pool2d(relu(bn(x))); codes is uint8 [N*Ho*Wo, C], one byte per pooled element:
+// bits 0-6 the winner's slot in its 3x3 window, bit 7 the winner's ReLU mask.
+static std::vector<torch::Tensor> bn_apply_pool(torch::Tensor x, std::vector<torch::Tensor> p, int64_t kernel_size,
+                                                int64_t stride, int64_t padding, int64_t dilation, bool ceil_mode) {
+  TORCH_CHECK(kernel_size == 3 && stride == 2 && padding == 1 && dilation == 1 && !ceil_mode,
+              "bn_apply_pool: only kernel 3, stride 2, padding 1, dilation 1, floor mode");
+  check_bn_input(x);
+  const int64_t N = x.size(0), C = x.size(1), H = x.size(2), W = x.size(3);
+  const dr::BnParams px = bn_params(p, C);
+  c10::cuda::CUDAGuard g(x.device());
+  const dr::PoolGeom pg{(int)H, (int)W, (int)((H - 1) / 2 + 1), (int)((W - 1) / 2 + 1)};
+  auto out = torch::empty({N, C, pg.Ho, pg.Wo}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
+  auto codes = torch::empty({N * pg.Ho * pg.Wo, C}, x.options().dtype(torch::kUInt8));
+  cudaError_t e = dr::launch_bn_apply_pool(x.data_ptr(), px, out.data_ptr(), codes.data_ptr(), (int)N, pg, (int)C,
+                                           cur_stream());
+  TORCH_CHECK(e == cudaSuccess, "bn_apply_pool: ", cudaGetErrorString(e));
+  return {out, codes};
+}
+
 static dr::BnParams bn_bwd_params(const std::vector<torch::Tensor>& p, int64_t C) {
   TORCH_CHECK(p.size() == 3, "bn_backward: expected (mean, invstd, weight)");
   const char* names[3] = {"mean", "invstd", "weight"};
@@ -351,18 +372,25 @@ static dr::BnParams bn_bwd_params(const std::vector<torch::Tensor>& p, int64_t C
 // The gradient of the ReLU input is g = mask ? go : 0.  Returns
 //   mode 0: (dx, dw, db);  1: (dx, dw, db, g) (g is the gradient of z);  2: (dx, dw, db, dz, dw_z, db_z).
 // Bitwise native_batch_norm_backward(threshold_backward(go, out, 0), ...) of torch's channels-last kernels.
+// Mode 3 is the backward of bn_apply_pool: go is the pooled gradient (N, C, Ho, Wo) and mask the codes; go reaches
+// the ReLU output as max_pool2d_with_indices_backward gives it.  Returns (dx, dw, db).
 static std::vector<torch::Tensor> bn_backward(int64_t mode, torch::Tensor go, torch::Tensor mask, torch::Tensor x,
                                               std::vector<torch::Tensor> p, c10::optional<torch::Tensor> z,
                                               std::vector<torch::Tensor> pz) {
-  TORCH_CHECK(mode >= 0 && mode <= 2, "bn_backward: mode must be 0, 1 or 2");
+  TORCH_CHECK(mode >= 0 && mode <= 3, "bn_backward: mode must be 0, 1, 2 or 3");
   check_bn_input(x);
-  TORCH_CHECK(go.sizes() == x.sizes() && go.scalar_type() == torch::kBFloat16 && go.device() == x.device() &&
-                  go.is_contiguous(at::MemoryFormat::ChannelsLast),
-              "bn_backward: go must be a channels_last bf16 tensor of x's shape on x's device");
   const int64_t C = x.size(1), rows = x.numel() / C;
+  dr::PoolGeom pg{(int)x.size(2), (int)x.size(3), (int)((x.size(2) - 1) / 2 + 1), (int)((x.size(3) - 1) / 2 + 1)};
+  const std::vector<int64_t> go_shape =
+      mode == 3 ? std::vector<int64_t>{x.size(0), C, pg.Ho, pg.Wo} : x.sizes().vec();
+  TORCH_CHECK(go.sizes() == go_shape && go.scalar_type() == torch::kBFloat16 && go.device() == x.device() &&
+                  go.is_contiguous(at::MemoryFormat::ChannelsLast),
+              "bn_backward: go must be a channels_last bf16 tensor on x's device, of x's shape (mode 3: the pooled "
+              "shape)");
+  const int64_t mask_numel = mode == 3 ? go.numel() : rows * (C / 8);
   TORCH_CHECK(mask.is_cuda() && mask.scalar_type() == torch::kUInt8 && mask.is_contiguous() &&
-                  mask.numel() == rows * (C / 8) && mask.device() == x.device(),
-              "bn_backward: mask must be bn_apply's mask for x");
+                  mask.numel() == mask_numel && mask.device() == x.device(),
+              "bn_backward: mask must be bn_apply's mask (mode 3: bn_apply_pool's codes) for x");
   c10::cuda::CUDAGuard guard(x.device());
   int block_y = 0, grid_y = 0;
   dr::bn_row_tree(rows, (int)C, &block_y, &grid_y);
@@ -378,11 +406,13 @@ static std::vector<torch::Tensor> bn_backward(int64_t mode, torch::Tensor go, to
   b.px = bn_bwd_params(p, C);
   b.dx = dx.data_ptr(); b.sums = sums.data_ptr<float>(); b.staging = grid_y > 1 ? staging.data_ptr<float>() : nullptr;
   b.dw = dw.data_ptr<float>(); b.db = db.data_ptr<float>();
+  b.pool = pg;
   std::vector<torch::Tensor> res{dx, dw, db};
-  if (mode == 1) {
-    auto g = torch::empty_like(x);
+  torch::Tensor g;
+  if (mode == 1 || mode == 3) {
+    g = torch::empty_like(x);
     b.g = g.data_ptr();
-    res.push_back(g);
+    if (mode == 1) res.push_back(g);     // mode 3: the gathered, masked pooled gradient, read by both passes
   } else if (mode == 2) {
     TORCH_CHECK(z.has_value(), "bn_backward: mode 2 needs z");
     check_like_x(*z, x, "z");
@@ -632,6 +662,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("eps"), py::arg("torch_kernel") = false);
   m.def("bn_apply", &bn_apply, py::arg("mode"), py::arg("x"), py::arg("p"), py::arg("z") = py::none(),
         py::arg("pz") = std::vector<torch::Tensor>{});
+  m.def("bn_apply_pool", &bn_apply_pool, py::arg("x"), py::arg("p"), py::arg("kernel_size") = 3, py::arg("stride") = 2,
+        py::arg("padding") = 1, py::arg("dilation") = 1, py::arg("ceil_mode") = false);
   m.def("bn_backward", &bn_backward, py::arg("mode"), py::arg("go"), py::arg("mask"), py::arg("x"), py::arg("p"),
         py::arg("z") = py::none(), py::arg("pz") = std::vector<torch::Tensor>{});
   m.def("rle_runs", &rle_runs);

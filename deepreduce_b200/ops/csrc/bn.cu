@@ -16,6 +16,8 @@
 //   * reduce: per-channel sum(g) and sum(g * (x - mean)) with g = mask ? go : +0, in the reduction tree of torch's
 //     batch_norm_backward_reduce_channels_last_kernel (see RowTree), so the sums are bitwise torch's;
 //   * elementwise: torch's dx expression, pinned to the FMA placement of its sm_90 SASS.
+// The stem's relu(bn(x)) is pooled in the same pass (bn_apply_pool_kernel), which writes a winner code per pooled element
+// instead of the ReLU output; backward mode 3 gathers the pooled gradient through the codes.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -99,6 +101,173 @@ __global__ void __launch_bounds__(kApplyThreads) bn_apply_kernel(const __nv_bflo
     }
     *reinterpret_cast<uint4*>(out + off) = vo;
     mask[r * groups + c / kVec] = (uint8_t)bits;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// stem: relu(bn(x)) -> max pool (kernel 3, stride 2, padding 1, dilation 1, floor mode)
+// ---------------------------------------------------------------------------------------------------------------------
+// Input x is N x H x W x C, the pooled output N x Ho x Wo x C with Ho = (H - 1) / 2 + 1 (PoolGeom).  Window (oh, ow)
+// covers rows 2 oh - 1 .. 2 oh + 1 and columns 2 ow - 1 .. 2 ow + 1, clipped to the input.
+
+// One thread = one output position x 8 channels; each thread keeps its channel group and walks output positions.  The
+// window is scanned as torch's max_pool_forward_nhwc does (ih outer, iw inner, from -inf; the winner changes where
+// v > best || isnan(v)), so the first of equal maxima and the last NaN win, on the bf16 value relu(bn(x)) of mode 0.
+// codes[pos][c]: bits 0-6 the winner's slot (ih - (2 oh - 1)) * 3 + (iw - (2 ow - 1)) in the unclipped window, bit 7
+// its ReLU mask !(y <= 0).  Backward needs nothing else: a position that wins a window has the same y in all of them.
+__global__ void __launch_bounds__(kApplyThreads) bn_apply_pool_kernel(const __nv_bfloat16* __restrict__ x, BnParams px,
+                                                                      __nv_bfloat16* __restrict__ out,
+                                                                      uint8_t* __restrict__ codes, int64_t orows,
+                                                                      PoolGeom pg, int C) {
+  const int groups = C / kVec;
+  const int rows_per_cta = blockDim.x / groups;
+  const int rsub = threadIdx.x / groups;
+  if (rsub >= rows_per_cta) return;
+  const int c = (threadIdx.x % groups) * kVec;
+  ChanParams a;
+  load_params(px, c, a);
+  const int64_t step = (int64_t)gridDim.x * rows_per_cta;
+  for (int64_t r = (int64_t)blockIdx.x * rows_per_cta + rsub; r < orows; r += step) {
+    const int ow = (int)(r % pg.Wo);
+    const int64_t t = r / pg.Wo;
+    const int oh = (int)(t % pg.Ho);
+    const int64_t n = t / pg.Ho;
+    const int h0 = 2 * oh - 1, w0 = 2 * ow - 1;
+    uint4 v[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+      const int ih = h0 + k / 3, iw = w0 + k % 3;
+      v[k] = ih >= 0 && ih < pg.H && iw >= 0 && iw < pg.W
+                 ? *reinterpret_cast<const uint4*>(x + ((n * pg.H + ih) * pg.W + iw) * C + c)
+                 : uint4{};
+    }
+    __nv_bfloat16 best[kVec];
+    unsigned slot[kVec];
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) {
+      best[i] = __float2bfloat16_rn(-INFINITY);
+      slot[i] = 0;
+    }
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+      const int ih = h0 + k / 3, iw = w0 + k % 3;
+      if (ih < 0 || ih >= pg.H || iw < 0 || iw >= pg.W) continue;
+      const __nv_bfloat16* hx = reinterpret_cast<const __nv_bfloat16*>(&v[k]);
+#pragma unroll
+      for (int i = 0; i < kVec; ++i) {
+        const __nv_bfloat16 y = relu_bf16(__float2bfloat16_rn(bn_elem(__bfloat162float(hx[i]), a.m[i], a.inv[i], a.w[i], a.b[i])));
+        const float fy = __bfloat162float(y);
+        if (fy > __bfloat162float(best[i]) || isnan(fy)) {
+          best[i] = y;
+          slot[i] = k;
+        }
+      }
+    }
+    uint4 vo;
+    __nv_bfloat16* ho = reinterpret_cast<__nv_bfloat16*>(&vo);
+    uint2 vc;
+    uint8_t* hc = reinterpret_cast<uint8_t*>(&vc);
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) {
+      ho[i] = best[i];
+      hc[i] = (uint8_t)(slot[i] | (__bfloat162float(best[i]) <= 0.f ? 0u : 0x80u));
+    }
+    *reinterpret_cast<uint4*>(out + r * C + c) = vo;
+    *reinterpret_cast<uint2*>(codes + r * C + c) = vc;
+  }
+}
+
+// The pooled gradient of input position (n, h, w), 8 channels, as torch's max_pool_backward_nhwc gives it, from the
+// <= 2 x 2 windows that cover it (torch's p_start / p_end: windows h / 2 .. min((h + 1) / 2 + 1, Ho) - 1 along h):
+//   * covered by one window: its gradient where the position won it, copied as bf16 (a -0.0 stays), else +0;
+//   * covered by more: the fp32 sum from 0.0f, in (oh, ow) order, of the gradients of the windows it won, rounded to bf16.
+struct PoolGather {
+  uint4 g[4];
+  uint2 code[4];     // window (h / 2 + a, w / 2 + b) in entry 2 a + b
+  int off;           // element offset of window (h / 2, w / 2) in the pooled tensor, channel c
+  int nh, nw;        // windows along h and w (0 for a row past the end)
+  int sh, sw;        // h - (2 (h / 2) - 1), w - (2 (w / 2) - 1): the position's row / column in window (h / 2, w / 2)
+};
+
+__device__ __forceinline__ void pool_gather_codes(PoolGather& q, const uint8_t* __restrict__ codes, const PoolGeom& pg,
+                                                  int row, int C, int c, bool valid) {
+  const int w = row % pg.W, t = row / pg.W, h = t % pg.H, n = t / pg.H;
+  const int ph = h >> 1, pw = w >> 1;
+  q.nh = valid ? min((h + 1) / 2 + 1, pg.Ho) - ph : 0;
+  q.nw = valid ? min((w + 1) / 2 + 1, pg.Wo) - pw : 0;
+  q.sh = h - 2 * ph + 1;
+  q.sw = w - 2 * pw + 1;
+  q.off = ((n * pg.Ho + ph) * pg.Wo + pw) * C + c;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int a = k >> 1, b = k & 1;
+    q.code[k] = a < q.nh && b < q.nw ? *reinterpret_cast<const uint2*>(codes + q.off + (a * pg.Wo + b) * C) : uint2{};
+  }
+}
+
+__device__ __forceinline__ void pool_gather_grads(PoolGather& q, const __nv_bfloat16* __restrict__ gp,
+                                                  const PoolGeom& pg, int C) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int a = k >> 1, b = k & 1;
+    q.g[k] = a < q.nh && b < q.nw ? *reinterpret_cast<const uint4*>(gp + q.off + (a * pg.Wo + b) * C) : uint4{};
+  }
+}
+
+// -> g (8 bf16: the pooled gradient of the position) and bits (bit i: the ReLU mask of channel i where the position won
+// a window, else 0; g is +0 there anyway).
+__device__ __forceinline__ void pool_gather_resolve(const PoolGather& q, uint4& g, unsigned& bits) {
+  __nv_bfloat16* hg = reinterpret_cast<__nv_bfloat16*>(&g);
+  const bool single = q.nh == 1 && q.nw == 1;
+  bits = 0;
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) {
+    float s = 0.f;
+    __nv_bfloat16 one = __float2bfloat16_rn(0.f);
+    unsigned bit = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int a = k >> 1, b = k & 1;
+      const unsigned code = (reinterpret_cast<const uint8_t*>(&q.code[k]))[i];
+      if (a < q.nh && b < q.nw && (int)(code & 0x7fu) == (q.sh - 2 * a) * 3 + (q.sw - 2 * b)) {
+        const __nv_bfloat16 v = (reinterpret_cast<const __nv_bfloat16*>(&q.g[k]))[i];
+        s = __fadd_rn(s, __bfloat162float(v));
+        one = v;
+        bit = code >> 7;
+      }
+    }
+    hg[i] = single ? one : __float2bfloat16_rn(s);
+    bits |= bit << i;
+  }
+}
+
+// Backward of the stem, first pass: g = mask ? (pooled gradient gathered onto x's positions) : +0, bf16 in x's layout,
+// which is threshold_backward(max_pool2d_with_indices_backward(...)) of the unfused graph.  Mode 3 of the reduce and the
+// elementwise pass then read it as mode 1 reads the reduce's g.  Gathering inside the reduce instead left that
+// latency-bound pass (16 K threads at C = 64) at a fraction of its bandwidth.
+__global__ void __launch_bounds__(kApplyThreads) bn_pool_grad_kernel(const __nv_bfloat16* __restrict__ gp,
+                                                                     const uint8_t* __restrict__ codes,
+                                                                     __nv_bfloat16* __restrict__ g, PoolGeom pg,
+                                                                     int64_t rows, int C) {
+  const int groups = C / kVec;
+  const int rows_per_cta = blockDim.x / groups;
+  const int rsub = threadIdx.x / groups;
+  if (rsub >= rows_per_cta) return;
+  const int c = (threadIdx.x % groups) * kVec;
+  const int64_t step = (int64_t)gridDim.x * rows_per_cta;
+#pragma unroll 2
+  for (int64_t r = (int64_t)blockIdx.x * rows_per_cta + rsub; r < rows; r += step) {
+    PoolGather q;
+    pool_gather_codes(q, codes, pg, (int)r, C, c, true);
+    pool_gather_grads(q, gp, pg, C);
+    uint4 v;
+    unsigned bits;
+    pool_gather_resolve(q, v, bits);
+    __nv_bfloat16* hv = reinterpret_cast<__nv_bfloat16*>(&v);
+#pragma unroll
+    for (int i = 0; i < kVec; ++i)
+      if (!((bits >> i) & 1u)) hv[i] = __float2bfloat16_rn(0.f);
+    *reinterpret_cast<uint4*>(g + r * C + c) = v;
   }
 }
 
@@ -355,7 +524,8 @@ __device__ __forceinline__ void bwd_store(const BwdOut& o, int k, int c, int C, 
 __device__ __forceinline__ float masked(__nv_bfloat16 go, unsigned bit) { return bit ? __bfloat162float(go) : 0.f; }
 
 // One physical thread = 8 channels (16-byte loads, one mask byte) of one virtual thread.  Block = gpc channel groups x
-// block_y virtual threads of one virtual block (blockIdx.y).  kMode 0: sums of g; 1: also writes g; 2: also the z sums.
+// block_y virtual threads of one virtual block (blockIdx.y).  kMode 0: sums of g; 1: also writes g; 2: also the z sums;
+// 3: go is the masked gradient bn_pool_grad_kernel wrote (no mask).
 template <int kMode>
 __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ go,
                                                                        const uint8_t* __restrict__ mask,
@@ -407,7 +577,7 @@ __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __n
         b.g[j] = *reinterpret_cast<const uint4*>(go + off);
         b.x[j] = *reinterpret_cast<const uint4*>(x + off);
         if (kMode == 2) b.z[j] = *reinterpret_cast<const uint4*>(z + off);
-        b.m[j] = mask[rr * mgroups + group];
+        b.m[j] = kMode == 3 ? 0u : mask[rr * mgroups + group];      // mode 3's g is masked already
       } else {
         b.g[j] = uint4{}; b.x[j] = uint4{}; b.z[j] = uint4{}; b.m[j] = 0;
       }
@@ -429,7 +599,7 @@ __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __n
 #pragma unroll
       for (int i = 0; i < kVec; ++i) {
         const unsigned bit = (mb[j] >> i) & 1u;
-        const float g = masked(hg[i], bit);
+        const float g = kMode == 3 ? __bfloat162float(hg[i]) : masked(hg[i], bit);
         if (kMode == 1) ho[i] = bit ? hg[i] : __float2bfloat16_rn(0.f);      // threshold_backward's bits, NaN too
         // torch's sm_90 SASS: FADD d = x - mean; FADD acc += g; FFMA acc_xmu = d * g + acc_xmu
         acc[0][j][i] = __fadd_rn(acc[0][j][i], g);
@@ -478,7 +648,8 @@ __global__ void bn_bwd_finalize_kernel(BwdOut o, RowTree t, int n_sums, int C, c
 
 // Elementwise: torch's dx = (g - sum_dy * norm_fct - (x - mean) * f1) * f2 with f1 = ((invstd * invstd) * sum_dy_xmu)
 // * norm_fct and f2 = weight * invstd.  Its sm_90 SASS contracts it to fma(-f1, x - mean, fma(-sum_dy, norm_fct, g))
-// * f2, rounded to bf16 once.  kMode 1 reads the g the reduce wrote (gm = nullptr); 0 and 2 mask go; 2 also writes dz.
+// * f2, rounded to bf16 once.  kMode 1 reads the g the reduce wrote (gm = nullptr), 3 the g bn_pool_grad_kernel wrote;
+// 0 and 2 mask go; 2 also writes dz.
 struct ElemtChan {
   float m[kVec], f1[kVec], f2[kVec], sdy[kVec];
 };
@@ -530,10 +701,10 @@ __global__ void __launch_bounds__(kApplyThreads) bn_bwd_elemt_kernel(const __nv_
   for (int64_t r = (int64_t)blockIdx.x * rows_per_cta + rsub; r < rows; r += step) {
     const int64_t off = r * C + c;
     const uint4 vg = *reinterpret_cast<const uint4*>(g_in + off);
+    const unsigned mb = kMode == 1 || kMode == 3 ? 0xffu : mask[r * groups + c / kVec];
     const uint4 vx = *reinterpret_cast<const uint4*>(x + off);
     uint4 vz = make_uint4(0, 0, 0, 0);
     if (kMode == 2) vz = *reinterpret_cast<const uint4*>(z + off);
-    const unsigned mb = kMode == 1 ? 0xffu : mask[r * groups + c / kVec];
     const __nv_bfloat16* hg = reinterpret_cast<const __nv_bfloat16*>(&vg);
     const __nv_bfloat16* hx = reinterpret_cast<const __nv_bfloat16*>(&vx);
     const __nv_bfloat16* hz = reinterpret_cast<const __nv_bfloat16*>(&vz);
@@ -632,7 +803,7 @@ cudaError_t launch_bwd_elemt(const BnBwd& b, const ElemtArgs& a, int64_t rows, i
   const float norm = (float)(1.0 / (double)rows);      // torch: static_cast<accscalar_t>(1.0 / reduction_size)
   count_launch();
   bn_bwd_elemt_kernel<kMode><<<grid, threads, 0, st>>>(
-      reinterpret_cast<const __nv_bfloat16*>(kMode == 1 ? b.g : b.go), b.mask,
+      reinterpret_cast<const __nv_bfloat16*>(kMode == 1 || kMode == 3 ? b.g : b.go), b.mask,
       reinterpret_cast<const __nv_bfloat16*>(b.x), reinterpret_cast<const __nv_bfloat16*>(b.z), a,
       reinterpret_cast<__nv_bfloat16*>(b.dx), reinterpret_cast<__nv_bfloat16*>(b.dz), norm, rows, C);
   return cudaGetLastError();
@@ -643,7 +814,20 @@ cudaError_t launch_backward(const BnBwd& b, int64_t rows64, int C, cudaStream_t 
   const int rows = (int)rows64;
   const RowTree t = row_tree(rows, C);
   const BwdOut o{b.sums, b.dw, b.db, b.dwz, b.dbz, b.staging};
-  cudaError_t e = launch_bwd_reduce<kMode>(b, t, o, rows, C, st);
+  cudaError_t e;
+  if (kMode == 3) {
+    int grid = 0, threads = 0;
+    e = rows_grid(bn_pool_grad_kernel, rows64, C, grid, threads);
+    if (e != cudaSuccess) return e;
+    count_launch();
+    bn_pool_grad_kernel<<<grid, threads, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(b.go), b.mask,
+                                                  reinterpret_cast<__nv_bfloat16*>(b.g), b.pool, rows64, C);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  BnBwd bb = b;
+  if (kMode == 3) bb.go = b.g;           // the reduce reads the gathered, masked g
+  e = launch_bwd_reduce<kMode>(bb, t, o, rows, C, st);
   if (e != cudaSuccess) return e;
   if (t.grid_y > 1) {
     const int cols = std::max(1, 512 / t.block_y);
@@ -693,6 +877,7 @@ cudaError_t launch_bn_backward(int mode, const BnBwd& b, int64_t rows, int C, cu
     case 0: return launch_backward<0>(b, rows, C, st);
     case 1: return launch_backward<1>(b, rows, C, st);
     case 2: return launch_backward<2>(b, rows, C, st);
+    case 3: return launch_backward<3>(b, rows, C, st);
     default: return cudaErrorInvalidValue;
   }
 }
@@ -718,6 +903,20 @@ cudaError_t launch_bn_apply(int mode, const void* x, const BnParams& px, const v
     case 2: return launch_apply<2>(x, px, z, pz, out, mask, rows, C, st);
     default: return cudaErrorInvalidValue;
   }
+}
+
+cudaError_t launch_bn_apply_pool(const void* x, const BnParams& px, void* out, void* codes, int N, const PoolGeom& pg,
+                                 int C, cudaStream_t st) {
+  const int64_t orows = (int64_t)N * pg.Ho * pg.Wo;
+  if (orows == 0) return cudaSuccess;
+  int grid = 0, threads = 0;
+  cudaError_t e = rows_grid(bn_apply_pool_kernel, orows, C, grid, threads);
+  if (e != cudaSuccess) return e;
+  count_launch();
+  bn_apply_pool_kernel<<<grid, threads, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(x), px,
+                                                 reinterpret_cast<__nv_bfloat16*>(out),
+                                                 reinterpret_cast<uint8_t*>(codes), orows, pg, C);
+  return cudaGetLastError();
 }
 
 }  // namespace dr

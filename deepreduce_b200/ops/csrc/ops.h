@@ -74,14 +74,25 @@ cudaError_t launch_bn_update_stats(const float* mean, float* var_invstd, float* 
 // mode 0: relu(bn(x)); 1: relu(bn(x) + z); 2: relu(bn(x) + bn_z(z)).  Also writes the ReLU mask, uint8 [rows][C / 8].
 cudaError_t launch_bn_apply(int mode, const void* x, const BnParams& px, const void* z, const BnParams& pz, void* out,
                             void* mask, int64_t rows, int C, cudaStream_t st);
+// The stem's max pool (kernel 3, stride 2, padding 1, dilation 1, floor mode) on x of N x H x W x C: Ho = (H - 1) / 2 + 1,
+// Wo = (W - 1) / 2 + 1.
+struct PoolGeom { int H, W, Ho, Wo; };
+// maxpool(relu(bn(x))) (mode 0's relu(bn(x)), then torch's NHWC max pool): writes the pooled output, N x Ho x Wo x C,
+// and a code byte per pooled element, uint8 [N * Ho * Wo][C]: bits 0-6 the winner's slot (3 * row + column) in the
+// unclipped window, bit 7 the winner's ReLU mask.
+cudaError_t launch_bn_apply_pool(const void* x, const BnParams& px, void* out, void* codes, int N, const PoolGeom& pg,
+                                 int C, cudaStream_t st);
 // Backward of bn_apply's mode from the output gradient go and the mask.  bf16 tensors have x's shape; per-channel fp32
 // outputs have C elements; sums = [sum_dy, sum_dy_xmu(, sum_dy_xmu_z)] x C; staging = same x grid_y (bn_row_tree)
-// when grid_y > 1.  Mode 1 also writes the masked gradient g; mode 2 reads z and writes dz, dwz, dbz.
+// when grid_y > 1.  Mode 1 also writes the masked gradient g; mode 2 reads z and writes dz, dwz, dbz.  Mode 3 is the
+// backward of bn_apply_pool: go is the pooled gradient (N x Ho x Wo x C), mask its codes, pool the geometry, and g
+// (x's shape) receives the masked gradient of the ReLU output, which both passes then read.
 struct BnBwd {
   const void* go; const uint8_t* mask; const void* x; const void* z;
   BnParams px, pz;      // bias unused
   void* dx; void* dz; void* g;
   float* sums; float* staging; float* dw; float* db; float* dwz; float* dbz;
+  PoolGeom pool;        // mode 3
 };
 cudaError_t launch_bn_backward(int mode, const BnBwd& b, int64_t rows, int C, cudaStream_t st);
 

@@ -25,6 +25,8 @@ sys.path.insert(0, ROOT)
 # (class, substrings of the kernel name); the first match wins
 CLASSES = [
     ("exchange", ("dr_engine_kernel",)),
+    ("stem bn + max pool (own)", ("bn_apply_pool_kernel",)),
+    ("stem pool grad (own)", ("bn_pool_grad_kernel",)),
     ("bn fused apply (own)", ("bn_apply_kernel",)),
     ("bn stats (own)", ("bn_stats_kernel", "bn_stats_finalize_kernel")),
     ("bn bwd reduce (own)", ("bn_bwd_reduce_kernel", "bn_bwd_finalize_kernel")),
@@ -61,15 +63,16 @@ def card():
 
 
 def shape_bytes(model, run_step):
-    """Bytes of the bf16 BN inputs of one forward, by role: W = bn1/bn2/stem (BN + ReLU), T = bn3 (BN + add + ReLU),
-    D = downsample BN, I = block inputs (where backward sums the skip and conv1 gradients)."""
+    """Bytes of the bf16 BN inputs of one forward, by role: S = the stem (BN + ReLU + max pool), W = bn1/bn2 (BN + ReLU),
+    T = bn3 (BN + add + ReLU), D = downsample BN, I = block inputs (where backward sums the skip and conv1 gradients)."""
     import torch.nn as nn
     from deepreduce_b200.models.resnet import _Bottleneck
     acc = collections.Counter()
     hooks = []
     for name, m in model.named_modules():
         if isinstance(m, nn.Conv2d):
-            role = "D" if name.endswith("downsample.0") else ("T" if name.endswith("conv3") else "W")
+            role = ("S" if name == "conv1" else "D" if name.endswith("downsample.0")
+                    else "T" if name.endswith("conv3") else "W")
             hooks.append(m.register_forward_hook(lambda mod, i, o, r=role: acc.__setitem__(r, acc[r] + o.numel() * o.element_size())))
         elif isinstance(m, _Bottleneck):
             hooks.append(m.register_forward_hook(lambda mod, i, o: acc.__setitem__("I", acc["I"] + i[0].numel() * i[0].element_size())))
@@ -81,20 +84,30 @@ def shape_bytes(model, run_step):
 
 def pass_bytes(b, fused):
     """Minimum bytes each memory-bound class moves per step (reads + writes over the tensors it touches)."""
-    W, T, D, I = b["W"], b["T"], b["D"], b["I"]
+    S, W, T, D, I = b["S"], b["W"], b["T"], b["D"], b["I"]
+    P = S / 4                  # the pooled stem output (kernel 3, stride 2: a quarter of the positions)
     out = {}
     if fused:
         # forward: bn_relu reads x, writes y; tails read x3 and idt (or xd), write o; each writes a 1/16-size ReLU mask.
+        # The stem reads x and writes the pooled output and a code byte per pooled element (P / 2).
         # backward, per BN + ReLU kind (Ti = identity tails, D = downsample tails, T = Ti + D):
-        #   reduce: W and Ti read go, x, mask (Ti also writes g); D reads go, x, z, mask
-        #   elemt:  W reads go, x, mask, writes dx; Ti reads g, x, writes dx; D reads go, x, z, mask, writes dx, dz
+        #   stem pool grad: reads the pooled gradient and the codes, writes the masked g at x's size
+        #   reduce: W and Ti read go, x, mask (Ti also writes g); D reads go, x, z, mask; the stem reads g, x
+        #   elemt:  W reads go, x, mask, writes dx; Ti and the stem read g, x, write dx; D reads go, x, z, mask, writes
+        #           dx, dz
         Ti, M = T - D, (W + T) / 16
-        out.update({"bn stats (own)": W + T + D, "bn fused apply (own)": 2 * W + 3 * T + M, "add": 3 * I,
-                    "bn bwd reduce (own)": 2 * W + 3 * Ti + 3 * D + M,
-                    "bn bwd elemt (own)": 3 * W + 3 * Ti + 5 * D + (W + D) / 16})
+        out.update({"bn stats (own)": S + W + T + D, "stem bn + max pool (own)": S + 1.5 * P,
+                    "stem pool grad (own)": 1.5 * P + S,
+                    "bn fused apply (own)": 2 * W + 3 * T + M, "add": 3 * I,
+                    "bn bwd reduce (own)": 2 * S + 2 * W + 3 * Ti + 3 * D + M,
+                    "bn bwd elemt (own)": 3 * S + 3 * W + 3 * Ti + 5 * D + (W + D) / 16})
     else:          # apply: read x, write y; relu_ in place; forward add: 2 reads + 1 write; backward junction adds
+        W += S
+        # max pool: forward reads y, writes the output and int64 indices (4 P); backward zeroes dy, reads the gradient
+        # and the indices, writes dy
         out.update({"bn stats": W + T + D, "bn apply": 2 * (W + T + D), "relu": 2 * (W + T), "add": 3 * T + 3 * I,
-                    "bn bwd reduce": 2 * (W + T + D), "bn bwd elemt": 3 * (W + T + D), "threshold_backward": 3 * (W + T)})
+                    "bn bwd reduce": 2 * (W + T + D), "bn bwd elemt": 3 * (W + T + D), "threshold_backward": 3 * (W + T),
+                    "max pool": 3 * S + 10 * P})
     return out
 
 
