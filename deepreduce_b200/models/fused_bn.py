@@ -10,6 +10,10 @@ re-read a masked copy of the gradient.
 The stem's BN + ReLU is fused with the max pool that follows it (``bn_relu_maxpool``): its forward writes the pooled
 output and a one-byte winner code per pooled element instead of the ReLU output and max pool's int64 indices, and its
 backward gathers the pooled gradient back through the codes, already masked, before the two backward kernels.
+A block input of ResNet-50 feeds two consumers (conv1 and the skip path).  With ``fork=True`` its producer (the stem, or
+the previous block's tail) returns the output twice, as two autograd outputs sharing one storage, so backward receives
+the two gradients separately and the kernels add them as they load them, instead of autograd writing their sum with an
+elementwise add that the backward passes then read again.
 
 Every fused result is bitwise that of the unfused graph: same reductions, same fp32 expressions, same bf16 rounding
 points.  ``eligible()`` decides per call; anything it rejects (CPU, eval mode, fp32, another memory layout) runs the
@@ -56,6 +60,20 @@ def _grad(go):
     return go.contiguous(memory_format=torch.channels_last)
 
 
+def _fork(ctx, o, fork):
+    """o, or for a forked producer (o, alias of o): two autograd outputs, so their gradients reach backward apart."""
+    if not fork:
+        return o
+    ctx.set_materialize_grads(False)       # an unused output's gradient arrives as None, not as a zeros tensor
+    return o, o.detach()
+
+
+def _grads(grads):
+    """(go, go2) for bn_backward from the gradients of a producer's outputs: go2 is None unless both were used."""
+    gs = [_grad(g) for g in grads if g is not None]
+    return (gs + [None, None])[:2]
+
+
 class _BNReLU(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, mean, invstd):
@@ -76,7 +94,7 @@ class _BNAddReLU(torch.autograd.Function):
     """relu(bn(x) + z) for an identity skip, relu(bn(x) + bn_z(z)) for a downsample skip (``wz`` given)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, mean, invstd, z, wz, bz, mz, iz):
+    def forward(ctx, x, weight, bias, mean, invstd, z, wz, bz, mz, iz, fork):
         from .. import ops
         mod = ops.cuda_module()
         if wz is None:
@@ -86,20 +104,23 @@ class _BNAddReLU(torch.autograd.Function):
             o, mask = mod.bn_apply(2, x, [mean, invstd, weight, bias], z, [mz, iz, wz, bz])
             ctx.save_for_backward(x, weight, mean, invstd, mask, z, wz, mz, iz)
         ctx.has_bn_z = wz is not None
-        return o
+        return _fork(ctx, o, fork)
 
     @staticmethod
-    def backward(ctx, go):
+    def backward(ctx, *grads):
         from .. import ops
         mod = ops.cuda_module()
+        go, go2 = _grads(grads)
+        if go is None:
+            return (None,) * 11
         saved = ctx.saved_tensors
         x, weight, mean, invstd, mask = saved[:5]
         if not ctx.has_bn_z:
-            dx, dw, db, g = mod.bn_backward(1, _grad(go), mask, x, [mean, invstd, weight])
-            return dx, dw, db, None, None, g, None, None, None, None
+            dx, dw, db, g = mod.bn_backward(1, go, mask, x, [mean, invstd, weight], go2=go2)
+            return dx, dw, db, None, None, g, None, None, None, None, None
         z, wz, mz, iz = saved[5:]
-        dx, dw, db, dz, dwz, dbz = mod.bn_backward(2, _grad(go), mask, x, [mean, invstd, weight], z, [mz, iz, wz])
-        return dx, dw, db, None, None, dz, dwz, dbz, None, None
+        dx, dw, db, dz, dwz, dbz = mod.bn_backward(2, go, mask, x, [mean, invstd, weight], z, [mz, iz, wz], go2=go2)
+        return dx, dw, db, None, None, dz, dwz, dbz, None, None, None
 
 
 class _BNReLUMaxPool(torch.autograd.Function):
@@ -108,18 +129,21 @@ class _BNReLUMaxPool(torch.autograd.Function):
     backward gathers the pooled gradient back onto x's positions from the codes."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, mean, invstd):
+    def forward(ctx, x, weight, bias, mean, invstd, fork):
         from .. import ops
         out, codes = ops.cuda_module().bn_apply_pool(x, [mean, invstd, weight, bias])
         ctx.save_for_backward(x, weight, mean, invstd, codes)
-        return out
+        return _fork(ctx, out, fork)
 
     @staticmethod
-    def backward(ctx, go):
+    def backward(ctx, *grads):
         from .. import ops
+        go, go2 = _grads(grads)
+        if go is None:
+            return (None,) * 6
         x, weight, mean, invstd, codes = ctx.saved_tensors
-        dx, dw, db = ops.cuda_module().bn_backward(3, _grad(go), codes, x, [mean, invstd, weight])
-        return dx, dw, db, None, None
+        dx, dw, db = ops.cuda_module().bn_backward(3, go, codes, x, [mean, invstd, weight], go2=go2)
+        return dx, dw, db, None, None, None
 
 
 def _stem_pool(pool: nn.Module) -> bool:
@@ -131,12 +155,17 @@ def _stem_pool(pool: nn.Module) -> bool:
             and pair(pool.dilation) == (1, 1) and not pool.ceil_mode and not pool.return_indices)
 
 
-def bn_relu_maxpool(x: torch.Tensor, bn: nn.BatchNorm2d, pool: nn.MaxPool2d) -> torch.Tensor:
-    """``pool(F.relu(bn(x), inplace=True))``."""
+def _pair(o, fork):
+    # the unfused composite's output for fork=True: one tensor twice, whose gradients autograd adds
+    return (o, o) if fork else o
+
+
+def bn_relu_maxpool(x: torch.Tensor, bn: nn.BatchNorm2d, pool: nn.MaxPool2d, fork: bool = False):
+    """``pool(F.relu(bn(x), inplace=True))``; with ``fork`` a pair of it, one per consumer (module docstring)."""
     if not (eligible(x, bn) and _stem_pool(pool)):
-        return pool(F.relu(bn(x), inplace=True))
+        return _pair(pool(F.relu(bn(x), inplace=True)), fork)
     mean, invstd = _stats(x, bn)
-    return _BNReLUMaxPool.apply(x, bn.weight, bn.bias, mean, invstd)
+    return _BNReLUMaxPool.apply(x, bn.weight, bn.bias, mean, invstd, fork)
 
 
 def bn_relu(x: torch.Tensor, bn: nn.BatchNorm2d) -> torch.Tensor:
@@ -147,18 +176,19 @@ def bn_relu(x: torch.Tensor, bn: nn.BatchNorm2d) -> torch.Tensor:
     return _BNReLU.apply(x, bn.weight, bn.bias, mean, invstd)
 
 
-def bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, idt: torch.Tensor) -> torch.Tensor:
-    """``F.relu(bn(x) + idt, inplace=True)``."""
+def bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, idt: torch.Tensor, fork: bool = False):
+    """``F.relu(bn(x) + idt, inplace=True)``; with ``fork`` a pair of it, one per consumer (module docstring)."""
     if not (eligible(x, bn) and idt.dtype == x.dtype and idt.shape == x.shape and idt.stride() == x.stride()):
-        return F.relu(bn(x) + idt, inplace=True)
+        return _pair(F.relu(bn(x) + idt, inplace=True), fork)
     mean, invstd = _stats(x, bn)
-    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, idt, None, None, None, None)
+    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, idt, None, None, None, None, fork)
 
 
-def bn_bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, xd: torch.Tensor, bnd: nn.BatchNorm2d) -> torch.Tensor:
-    """``F.relu(bn(x) + bnd(xd), inplace=True)``: the tail of a bottleneck with a downsample branch."""
+def bn_bn_add_relu(x: torch.Tensor, bn: nn.BatchNorm2d, xd: torch.Tensor, bnd: nn.BatchNorm2d, fork: bool = False):
+    """``F.relu(bn(x) + bnd(xd), inplace=True)``: the tail of a bottleneck with a downsample branch; with ``fork`` a
+    pair of it, one per consumer (module docstring)."""
     if not (eligible(x, bn) and eligible(xd, bnd) and xd.shape == x.shape and xd.stride() == x.stride()):
-        return F.relu(bn(x) + bnd(xd), inplace=True)
+        return _pair(F.relu(bn(x) + bnd(xd), inplace=True), fork)
     md, id_ = _stats(xd, bnd)
     mean, invstd = _stats(x, bn)
-    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, xd, bnd.weight, bnd.bias, md, id_)
+    return _BNAddReLU.apply(x, bn.weight, bn.bias, mean, invstd, xd, bnd.weight, bnd.bias, md, id_, fork)

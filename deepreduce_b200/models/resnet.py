@@ -78,16 +78,21 @@ class _Bottleneck(nn.Module):
         if downsample:
             self.downsample = nn.Sequential(nn.Conv2d(inp, out, 1, stride, bias=False), nn.BatchNorm2d(out))
 
-    def forward(self, x):
+    def forward(self, x, skip=None, fork=False):
         # each helper is the unfused composite unless its input is a channels_last bf16 CUDA training tensor
-        # (models/fused_bn.py); either way the results are bitwise the same
-        xd = None if self.downsample is None else self.downsample[0](x)
+        # (models/fused_bn.py); either way the results are bitwise the same.  skip: the block input as the skip path
+        # reads it, when the producer returned it as a second output.  fork: return (output for the next conv1, output
+        # for the next skip path or None), so backward gets the two gradients apart.  Only the identity tail forks;
+        # for the downsample tail the second gradient did not pay (DESIGN.md §8a), and it returns (output, None).
+        skip = x if skip is None else skip
+        xd = None if self.downsample is None else self.downsample[0](skip)
         y = bn_relu(self.conv1(x), self.bn1)
         y = bn_relu(self.conv2(y), self.bn2)
         y = self.conv3(y)
         if xd is None:
-            return bn_add_relu(y, self.bn3, x)
-        return bn_bn_add_relu(y, self.bn3, xd, self.downsample[1])
+            return bn_add_relu(y, self.bn3, skip, fork=fork)
+        o = bn_bn_add_relu(y, self.bn3, xd, self.downsample[1])
+        return (o, None) if fork else o
 
 
 class ResNet(nn.Module):
@@ -109,8 +114,11 @@ class ResNet(nn.Module):
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
 
     def forward(self, x):
-        x = bn_relu_maxpool(self.conv1(x), self.bn1, self.maxpool)
-        x = self.layers(x)
+        # every block input feeds conv1 and the skip path; an identity tail returns it once per consumer (fork), so
+        # its backward adds the two gradients itself.  The stem stays on one output (DESIGN.md §8a).
+        x, skip = bn_relu_maxpool(self.conv1(x), self.bn1, self.maxpool), None
+        for blk in self.layers:
+            x, skip = blk(x, skip, fork=True)
         x = F.adaptive_avg_pool2d(x, 1).flatten(1)
         return self.fc(x)
 

@@ -374,19 +374,23 @@ static dr::BnParams bn_bwd_params(const std::vector<torch::Tensor>& p, int64_t C
 // Bitwise native_batch_norm_backward(threshold_backward(go, out, 0), ...) of torch's channels-last kernels.
 // Mode 3 is the backward of bn_apply_pool: go is the pooled gradient (N, C, Ho, Wo) and mask the codes; go reaches
 // the ReLU output as max_pool2d_with_indices_backward gives it.  Returns (dx, dw, db).
+// go2 (modes 1-3): a second gradient of the output, checked like go.  The output then feeds two consumers, and the
+// kernels use the bf16 sum go + go2 (fp32 sum, rounded once: autograd's add) wherever they would use go.
 static std::vector<torch::Tensor> bn_backward(int64_t mode, torch::Tensor go, torch::Tensor mask, torch::Tensor x,
                                               std::vector<torch::Tensor> p, c10::optional<torch::Tensor> z,
-                                              std::vector<torch::Tensor> pz) {
+                                              std::vector<torch::Tensor> pz, c10::optional<torch::Tensor> go2) {
   TORCH_CHECK(mode >= 0 && mode <= 3, "bn_backward: mode must be 0, 1, 2 or 3");
+  TORCH_CHECK(!go2.has_value() || mode != 0, "bn_backward: mode 0 takes no go2");
   check_bn_input(x);
   const int64_t C = x.size(1), rows = x.numel() / C;
   dr::PoolGeom pg{(int)x.size(2), (int)x.size(3), (int)((x.size(2) - 1) / 2 + 1), (int)((x.size(3) - 1) / 2 + 1)};
   const std::vector<int64_t> go_shape =
       mode == 3 ? std::vector<int64_t>{x.size(0), C, pg.Ho, pg.Wo} : x.sizes().vec();
-  TORCH_CHECK(go.sizes() == go_shape && go.scalar_type() == torch::kBFloat16 && go.device() == x.device() &&
-                  go.is_contiguous(at::MemoryFormat::ChannelsLast),
-              "bn_backward: go must be a channels_last bf16 tensor on x's device, of x's shape (mode 3: the pooled "
-              "shape)");
+  for (const torch::Tensor* t : {&go, go2.has_value() ? &*go2 : &go})
+    TORCH_CHECK(t->sizes() == go_shape && t->scalar_type() == torch::kBFloat16 && t->device() == x.device() &&
+                    t->is_contiguous(at::MemoryFormat::ChannelsLast),
+                "bn_backward: go and go2 must be channels_last bf16 tensors on x's device, of x's shape (mode 3: the "
+                "pooled shape)");
   const int64_t mask_numel = mode == 3 ? go.numel() : rows * (C / 8);
   TORCH_CHECK(mask.is_cuda() && mask.scalar_type() == torch::kUInt8 && mask.is_contiguous() &&
                   mask.numel() == mask_numel && mask.device() == x.device(),
@@ -402,7 +406,7 @@ static std::vector<torch::Tensor> bn_backward(int64_t mode, torch::Tensor go, to
   auto staging = grid_y > 1 ? torch::empty({n_sums, grid_y, C}, f32) : torch::Tensor();
   auto dx = torch::empty_like(x), dw = torch::empty({C}, f32), db = torch::empty({C}, f32);
   dr::BnBwd b{};
-  b.go = go.data_ptr(); b.mask = mask.data_ptr<uint8_t>(); b.x = x.data_ptr();
+  b.go = go.data_ptr(); b.go2 = go2.has_value() ? go2->data_ptr() : nullptr; b.mask = mask.data_ptr<uint8_t>(); b.x = x.data_ptr();
   b.px = bn_bwd_params(p, C);
   b.dx = dx.data_ptr(); b.sums = sums.data_ptr<float>(); b.staging = grid_y > 1 ? staging.data_ptr<float>() : nullptr;
   b.dw = dw.data_ptr<float>(); b.db = db.data_ptr<float>();
@@ -665,7 +669,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_apply_pool", &bn_apply_pool, py::arg("x"), py::arg("p"), py::arg("kernel_size") = 3, py::arg("stride") = 2,
         py::arg("padding") = 1, py::arg("dilation") = 1, py::arg("ceil_mode") = false);
   m.def("bn_backward", &bn_backward, py::arg("mode"), py::arg("go"), py::arg("mask"), py::arg("x"), py::arg("p"),
-        py::arg("z") = py::none(), py::arg("pz") = std::vector<torch::Tensor>{});
+        py::arg("z") = py::none(), py::arg("pz") = std::vector<torch::Tensor>{}, py::arg("go2") = py::none());
   m.def("rle_runs", &rle_runs);
   m.def("rle_indices", &rle_indices);
   m.def("arena_alloc", &arena_alloc);

@@ -59,6 +59,18 @@ __device__ __forceinline__ __nv_bfloat16 relu_bf16(__nv_bfloat16 v) {
   return __bfloat162float(v) <= 0.f ? __float2bfloat16_rn(0.f) : v;
 }
 
+// The two gradients of a block input (conv1's and the skip path's), summed as autograd's bf16 add does: fp32 sum of the
+// bf16 values, rounded once.  The operands commute, so the order autograd would have added them in does not matter.
+__device__ __forceinline__ uint4 add_bf16x8(const uint4& a, const uint4& b) {
+  uint4 s;
+  const __nv_bfloat16* ha = reinterpret_cast<const __nv_bfloat16*>(&a);
+  const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&b);
+  __nv_bfloat16* hs = reinterpret_cast<__nv_bfloat16*>(&s);
+#pragma unroll
+  for (int i = 0; i < kVec; ++i) hs[i] = __float2bfloat16_rn(__fadd_rn(__bfloat162float(ha[i]), __bfloat162float(hb[i])));
+  return s;
+}
+
 // kMode 0: relu(bn(x));  1: relu(bn(x) + z);  2: relu(bn(x) + bn_z(z)).
 // Each thread owns one group of 8 channels for the whole launch (its parameters stay in registers) and walks rows.
 // mask[row][C / 8]: bit i of a byte is channel 8 * group + i, set where !(out <= 0) (so a NaN output passes gradient).
@@ -205,12 +217,18 @@ __device__ __forceinline__ void pool_gather_codes(PoolGather& q, const uint8_t* 
   }
 }
 
+// kTwo: the pooled output is a block input with two consumers; its gradient is the bf16 sum of gp and gp2, formed per
+// pooled element before the gather.
+template <bool kTwo>
 __device__ __forceinline__ void pool_gather_grads(PoolGather& q, const __nv_bfloat16* __restrict__ gp,
-                                                  const PoolGeom& pg, int C) {
+                                                  const __nv_bfloat16* __restrict__ gp2, const PoolGeom& pg, int C) {
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const int a = k >> 1, b = k & 1;
-    q.g[k] = a < q.nh && b < q.nw ? *reinterpret_cast<const uint4*>(gp + q.off + (a * pg.Wo + b) * C) : uint4{};
+    const bool in = a < q.nh && b < q.nw;
+    const int off = q.off + (a * pg.Wo + b) * C;
+    q.g[k] = in ? *reinterpret_cast<const uint4*>(gp + off) : uint4{};
+    if (kTwo && in) q.g[k] = add_bf16x8(q.g[k], *reinterpret_cast<const uint4*>(gp2 + off));
   }
 }
 
@@ -244,8 +262,10 @@ __device__ __forceinline__ void pool_gather_resolve(const PoolGather& q, uint4& 
 // Backward of the stem, first pass: g = mask ? (pooled gradient gathered onto x's positions) : +0, bf16 in x's layout,
 // which is threshold_backward(max_pool2d_with_indices_backward(...)) of the unfused graph.  Mode 3 of the reduce and the
 // elementwise pass then read it as mode 1 reads the reduce's g.  Gathering inside the reduce instead left that
-// latency-bound pass (16 K threads at C = 64) at a fraction of its bandwidth.
+// latency-bound pass (16 K threads at C = 64) at a fraction of its bandwidth.  kTwo: the pooled gradient is gp + gp2.
+template <bool kTwo>
 __global__ void __launch_bounds__(kApplyThreads) bn_pool_grad_kernel(const __nv_bfloat16* __restrict__ gp,
+                                                                     const __nv_bfloat16* __restrict__ gp2,
                                                                      const uint8_t* __restrict__ codes,
                                                                      __nv_bfloat16* __restrict__ g, PoolGeom pg,
                                                                      int64_t rows, int C) {
@@ -259,7 +279,7 @@ __global__ void __launch_bounds__(kApplyThreads) bn_pool_grad_kernel(const __nv_
   for (int64_t r = (int64_t)blockIdx.x * rows_per_cta + rsub; r < rows; r += step) {
     PoolGather q;
     pool_gather_codes(q, codes, pg, (int)r, C, c, true);
-    pool_gather_grads(q, gp, pg, C);
+    pool_gather_grads<kTwo>(q, gp, gp2, pg, C);
     uint4 v;
     unsigned bits;
     pool_gather_resolve(q, v, bits);
@@ -525,9 +545,11 @@ __device__ __forceinline__ float masked(__nv_bfloat16 go, unsigned bit) { return
 
 // One physical thread = 8 channels (16-byte loads, one mask byte) of one virtual thread.  Block = gpc channel groups x
 // block_y virtual threads of one virtual block (blockIdx.y).  kMode 0: sums of g; 1: also writes g; 2: also the z sums;
-// 3: go is the masked gradient bn_pool_grad_kernel wrote (no mask).
-template <int kMode>
+// 3: go is the masked gradient bn_pool_grad_kernel wrote (no mask).  kTwo (modes 1, 2): the output is a block input and
+// its gradient is the bf16 sum of go and go2 (add_bf16x8), formed before the mask.
+template <int kMode, bool kTwo>
 __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ go,
+                                                                       const __nv_bfloat16* __restrict__ go2,
                                                                        const uint8_t* __restrict__ mask,
                                                                        const __nv_bfloat16* __restrict__ x,
                                                                        const float* __restrict__ mean,
@@ -564,8 +586,12 @@ __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __n
   const int n_loops = t.loops(rows);
   // The tree fixes the thread count (S * C / kVec; 16 K threads for C = 64), so each thread keeps two iterations of loads
   // in flight: the next one is issued before the current one is summed.  Rows past the end load nothing and give 0.
+  // With two gradients the current batch's pair is summed before the next loads are issued, so only the next batch
+  // holds a second gradient.  Mode 2 with two gradients has no room for a second batch (249 registers without it) and
+  // runs at 64 K-262 K threads (C >= 256), so it loads at the top of each iteration instead.
+  constexpr bool kAhead = !(kTwo && kMode == 2);
   struct Batch {
-    uint4 g[L], x[L], z[L];
+    uint4 g[L], g2[L], x[L], z[L];
     unsigned m[L];
   };
   auto load = [&](Batch& b, int r0) {
@@ -575,19 +601,25 @@ __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __n
       if (live && rr < rows) {
         const int off = rr * C + c;
         b.g[j] = *reinterpret_cast<const uint4*>(go + off);
+        if (kTwo) b.g2[j] = *reinterpret_cast<const uint4*>(go2 + off);
         b.x[j] = *reinterpret_cast<const uint4*>(x + off);
         if (kMode == 2) b.z[j] = *reinterpret_cast<const uint4*>(z + off);
         b.m[j] = kMode == 3 ? 0u : mask[rr * mgroups + group];      // mode 3's g is masked already
       } else {
-        b.g[j] = uint4{}; b.x[j] = uint4{}; b.z[j] = uint4{}; b.m[j] = 0;
+        b.g[j] = uint4{}; b.g2[j] = uint4{}; b.x[j] = uint4{}; b.z[j] = uint4{}; b.m[j] = 0;
       }
     }
   };
   Batch cur;
-  load(cur, r);
+  if (kAhead) load(cur, r);
   for (int it = 0; it < n_loops; ++it) {
+    if (!kAhead) load(cur, r);
+    if (kTwo) {
+#pragma unroll
+      for (int j = 0; j < L; ++j) cur.g[j] = add_bf16x8(cur.g[j], cur.g2[j]);
+    }
     Batch nxt;
-    load(nxt, r + L * S);
+    if (kAhead) load(nxt, r + L * S);
     const unsigned* mb = cur.m;
 #pragma unroll
     for (int j = 0; j < L; ++j) {
@@ -608,7 +640,7 @@ __global__ void __launch_bounds__(kReduceThreads) bn_bwd_reduce_kernel(const __n
       }
       if (kMode == 1 && live && r + j * S < rows) *reinterpret_cast<uint4*>(g_out + (r + j * S) * C + c) = vo;
     }
-    cur = nxt;
+    if (kAhead) cur = nxt;
     r += L * S;
   }
 #pragma unroll
@@ -679,8 +711,10 @@ struct ElemtArgs {
   const float *mean_z, *invstd_z, *weight_z;
 };
 
-template <int kMode>
+// kTwo (mode 2): the gradient is the bf16 sum of g_in and g2_in, as in the reduce.
+template <int kMode, bool kTwo>
 __global__ void __launch_bounds__(kApplyThreads) bn_bwd_elemt_kernel(const __nv_bfloat16* __restrict__ g_in,
+                                                                     const __nv_bfloat16* __restrict__ g2_in,
                                                                      const uint8_t* __restrict__ mask,
                                                                      const __nv_bfloat16* __restrict__ x,
                                                                      const __nv_bfloat16* __restrict__ z, ElemtArgs a,
@@ -700,7 +734,8 @@ __global__ void __launch_bounds__(kApplyThreads) bn_bwd_elemt_kernel(const __nv_
 #pragma unroll 2
   for (int64_t r = (int64_t)blockIdx.x * rows_per_cta + rsub; r < rows; r += step) {
     const int64_t off = r * C + c;
-    const uint4 vg = *reinterpret_cast<const uint4*>(g_in + off);
+    uint4 vg = *reinterpret_cast<const uint4*>(g_in + off);
+    if (kTwo) vg = add_bf16x8(vg, *reinterpret_cast<const uint4*>(g2_in + off));
     const unsigned mb = kMode == 1 || kMode == 3 ? 0xffu : mask[r * groups + c / kVec];
     const uint4 vx = *reinterpret_cast<const uint4*>(x + off);
     uint4 vz = make_uint4(0, 0, 0, 0);
@@ -781,35 +816,38 @@ RowTree row_tree(int rows, int C) {
   return {block_y, grid_y};
 }
 
-template <int kMode>
+template <int kMode, bool kTwo>
 cudaError_t launch_bwd_reduce(const BnBwd& b, const RowTree& t, const BwdOut& o, int rows, int C, cudaStream_t st) {
   const int groups = C / kVec;
   const int gpc = std::min(groups, std::max(1, kReduceThreads / t.block_y));
   const dim3 grid((groups + gpc - 1) / gpc, t.grid_y);
   const int threads = gpc * t.block_y;
   count_launch();
-  bn_bwd_reduce_kernel<kMode><<<grid, threads, threads * kVec * sizeof(float), st>>>(
-      reinterpret_cast<const __nv_bfloat16*>(b.go), b.mask, reinterpret_cast<const __nv_bfloat16*>(b.x), b.px.mean,
-      b.px.invstd, reinterpret_cast<const __nv_bfloat16*>(b.z), b.pz.mean, b.pz.invstd,
-      reinterpret_cast<__nv_bfloat16*>(b.g), o, t, rows, C);
+  bn_bwd_reduce_kernel<kMode, kTwo><<<grid, threads, threads * kVec * sizeof(float), st>>>(
+      reinterpret_cast<const __nv_bfloat16*>(b.go), reinterpret_cast<const __nv_bfloat16*>(b.go2), b.mask,
+      reinterpret_cast<const __nv_bfloat16*>(b.x), b.px.mean, b.px.invstd, reinterpret_cast<const __nv_bfloat16*>(b.z),
+      b.pz.mean, b.pz.invstd, reinterpret_cast<__nv_bfloat16*>(b.g), o, t, rows, C);
   return cudaGetLastError();
 }
 
-template <int kMode>
+template <int kMode, bool kTwo>
 cudaError_t launch_bwd_elemt(const BnBwd& b, const ElemtArgs& a, int64_t rows, int C, cudaStream_t st) {
   int grid = 0, threads = 0;
-  cudaError_t e = rows_grid(bn_bwd_elemt_kernel<kMode>, rows, C, grid, threads);
+  cudaError_t e = rows_grid(bn_bwd_elemt_kernel<kMode, kTwo>, rows, C, grid, threads);
   if (e != cudaSuccess) return e;
   const float norm = (float)(1.0 / (double)rows);      // torch: static_cast<accscalar_t>(1.0 / reduction_size)
   count_launch();
-  bn_bwd_elemt_kernel<kMode><<<grid, threads, 0, st>>>(
-      reinterpret_cast<const __nv_bfloat16*>(kMode == 1 || kMode == 3 ? b.g : b.go), b.mask,
-      reinterpret_cast<const __nv_bfloat16*>(b.x), reinterpret_cast<const __nv_bfloat16*>(b.z), a,
-      reinterpret_cast<__nv_bfloat16*>(b.dx), reinterpret_cast<__nv_bfloat16*>(b.dz), norm, rows, C);
+  bn_bwd_elemt_kernel<kMode, kTwo><<<grid, threads, 0, st>>>(
+      reinterpret_cast<const __nv_bfloat16*>(kMode == 1 || kMode == 3 ? b.g : b.go),
+      reinterpret_cast<const __nv_bfloat16*>(b.go2), b.mask, reinterpret_cast<const __nv_bfloat16*>(b.x),
+      reinterpret_cast<const __nv_bfloat16*>(b.z), a, reinterpret_cast<__nv_bfloat16*>(b.dx),
+      reinterpret_cast<__nv_bfloat16*>(b.dz), norm, rows, C);
   return cudaGetLastError();
 }
 
-template <int kMode>
+// kTwo: b.go2 is set.  Mode 1 folds it in the reduce, which writes the summed, masked g for the elementwise pass; mode 2
+// folds it in both passes; mode 3 in bn_pool_grad_kernel, whose g both passes read.
+template <int kMode, bool kTwo>
 cudaError_t launch_backward(const BnBwd& b, int64_t rows64, int C, cudaStream_t st) {
   const int rows = (int)rows64;
   const RowTree t = row_tree(rows, C);
@@ -817,17 +855,18 @@ cudaError_t launch_backward(const BnBwd& b, int64_t rows64, int C, cudaStream_t 
   cudaError_t e;
   if (kMode == 3) {
     int grid = 0, threads = 0;
-    e = rows_grid(bn_pool_grad_kernel, rows64, C, grid, threads);
+    e = rows_grid(bn_pool_grad_kernel<kTwo>, rows64, C, grid, threads);
     if (e != cudaSuccess) return e;
     count_launch();
-    bn_pool_grad_kernel<<<grid, threads, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(b.go), b.mask,
-                                                  reinterpret_cast<__nv_bfloat16*>(b.g), b.pool, rows64, C);
+    bn_pool_grad_kernel<kTwo><<<grid, threads, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(b.go),
+                                                        reinterpret_cast<const __nv_bfloat16*>(b.go2), b.mask,
+                                                        reinterpret_cast<__nv_bfloat16*>(b.g), b.pool, rows64, C);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }
   BnBwd bb = b;
   if (kMode == 3) bb.go = b.g;           // the reduce reads the gathered, masked g
-  e = launch_bwd_reduce<kMode>(bb, t, o, rows, C, st);
+  e = launch_bwd_reduce<kMode, kTwo && kMode != 3>(bb, t, o, rows, C, st);
   if (e != cudaSuccess) return e;
   if (t.grid_y > 1) {
     const int cols = std::max(1, 512 / t.block_y);
@@ -839,7 +878,7 @@ cudaError_t launch_backward(const BnBwd& b, int64_t rows64, int C, cudaStream_t 
     if (e != cudaSuccess) return e;
   }
   const ElemtArgs a{b.px.mean, b.px.invstd, b.px.weight, b.sums, b.pz.mean, b.pz.invstd, b.pz.weight};
-  return launch_bwd_elemt<kMode>(b, a, rows64, C, st);
+  return launch_bwd_elemt<kMode, kTwo && kMode == 2>(b, a, rows64, C, st);
 }
 
 cudaError_t launch_stats(const BnStats& s, int rows, int C, cudaStream_t st) {
@@ -873,11 +912,12 @@ void bn_row_tree(int64_t rows, int C, int* block_y, int* grid_y) {
 
 cudaError_t launch_bn_backward(int mode, const BnBwd& b, int64_t rows, int C, cudaStream_t st) {
   if (rows == 0) return cudaSuccess;
+  const bool two = b.go2 != nullptr;
   switch (mode) {
-    case 0: return launch_backward<0>(b, rows, C, st);
-    case 1: return launch_backward<1>(b, rows, C, st);
-    case 2: return launch_backward<2>(b, rows, C, st);
-    case 3: return launch_backward<3>(b, rows, C, st);
+    case 0: return two ? cudaErrorInvalidValue : launch_backward<0, false>(b, rows, C, st);
+    case 1: return two ? launch_backward<1, true>(b, rows, C, st) : launch_backward<1, false>(b, rows, C, st);
+    case 2: return two ? launch_backward<2, true>(b, rows, C, st) : launch_backward<2, false>(b, rows, C, st);
+    case 3: return two ? launch_backward<3, true>(b, rows, C, st) : launch_backward<3, false>(b, rows, C, st);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -86,9 +86,11 @@ cudaError_t launch_bn_apply_pool(const void* x, const BnParams& px, void* out, v
 // outputs have C elements; sums = [sum_dy, sum_dy_xmu(, sum_dy_xmu_z)] x C; staging = same x grid_y (bn_row_tree)
 // when grid_y > 1.  Mode 1 also writes the masked gradient g; mode 2 reads z and writes dz, dwz, dbz.  Mode 3 is the
 // backward of bn_apply_pool: go is the pooled gradient (N x Ho x Wo x C), mask its codes, pool the geometry, and g
-// (x's shape) receives the masked gradient of the ReLU output, which both passes then read.
+// (x's shape) receives the masked gradient of the ReLU output, which both passes then read.  go2 (modes 1-3, may be
+// null): a second gradient of go's shape; the output gradient is then the bf16 sum go + go2, autograd's sum at a block
+// input with two consumers, formed as the kernels load it.
 struct BnBwd {
-  const void* go; const uint8_t* mask; const void* x; const void* z;
+  const void* go; const void* go2; const uint8_t* mask; const void* x; const void* z;
   BnParams px, pz;      // bias unused
   void* dx; void* dz; void* g;
   float* sums; float* staging; float* dw; float* db; float* dwz; float* dbz;

@@ -64,18 +64,30 @@ def card():
 
 def shape_bytes(model, run_step):
     """Bytes of the bf16 BN inputs of one forward, by role: S = the stem (BN + ReLU + max pool), W = bn1/bn2 (BN + ReLU),
-    T = bn3 (BN + add + ReLU), D = downsample BN, I = block inputs (where backward sums the skip and conv1 gradients)."""
+    T = bn3 (BN + add + ReLU), D = downsample BN, I = block inputs (where backward sums the skip and conv1 gradients),
+    split by the producer of the block input: IS the stem, IT a tail with an identity skip, ID a tail with a downsample
+    BN (I = IS + IT + ID)."""
     import torch.nn as nn
     from deepreduce_b200.models.resnet import _Bottleneck
     acc = collections.Counter()
     hooks = []
+    add = lambda key, t: acc.__setitem__(key, acc[key] + t.numel() * t.element_size())      # noqa: E731
     for name, m in model.named_modules():
         if isinstance(m, nn.Conv2d):
             role = ("S" if name == "conv1" else "D" if name.endswith("downsample.0")
                     else "T" if name.endswith("conv3") else "W")
-            hooks.append(m.register_forward_hook(lambda mod, i, o, r=role: acc.__setitem__(r, acc[r] + o.numel() * o.element_size())))
-        elif isinstance(m, _Bottleneck):
-            hooks.append(m.register_forward_hook(lambda mod, i, o: acc.__setitem__("I", acc["I"] + i[0].numel() * i[0].element_size())))
+            hooks.append(m.register_forward_hook(lambda mod, i, o, r=role: add(r, o)))
+
+    def block_input(mod, i, o, src):
+        add("I", i[0])
+        add(src, i[0])
+
+    prev = None
+    for m in model.modules():
+        if isinstance(m, _Bottleneck):
+            src = "IS" if prev is None else "IT" if prev.downsample is None else "ID"
+            hooks.append(m.register_forward_hook(lambda mod, i, o, r=src: block_input(mod, i, o, r)))
+            prev = m
     run_step()
     for h in hooks:
         h.remove()
@@ -95,11 +107,14 @@ def pass_bytes(b, fused):
         #   reduce: W and Ti read go, x, mask (Ti also writes g); D reads go, x, z, mask; the stem reads g, x
         #   elemt:  W reads go, x, mask, writes dx; Ti and the stem read g, x, write dx; D reads go, x, z, mask, writes
         #           dx, dz
+        # A block input made by an identity tail is not summed by an add: the tail's reduce reads its two gradients.
+        # The inputs made by the stem and by downsample tails are still summed by autograd's add (read, read, write).
         Ti, M = T - D, (W + T) / 16
+        IS, IT, ID = b.get("IS", 0), b.get("IT", 0), b.get("ID", 0)
         out.update({"bn stats (own)": S + W + T + D, "stem bn + max pool (own)": S + 1.5 * P,
                     "stem pool grad (own)": 1.5 * P + S,
-                    "bn fused apply (own)": 2 * W + 3 * T + M, "add": 3 * I,
-                    "bn bwd reduce (own)": 2 * S + 2 * W + 3 * Ti + 3 * D + M,
+                    "bn fused apply (own)": 2 * W + 3 * T + M, "add": 3 * (IS + ID),
+                    "bn bwd reduce (own)": 2 * S + 2 * W + 3 * Ti + 3 * D + M + IT,
                     "bn bwd elemt (own)": 3 * S + 3 * W + 3 * Ti + 5 * D + (W + D) / 16})
     else:          # apply: read x, write y; relu_ in place; forward add: 2 reads + 1 write; backward junction adds
         W += S
