@@ -234,6 +234,10 @@ static torch::Tensor u8_to_nhwc_norm(torch::Tensor in, std::vector<double> mean,
   CHECK_CUDA_T(in);
   TORCH_CHECK(in.scalar_type() == torch::kUInt8 && in.size(-1) == 3, "expect uint8 [...,3] NHWC");
   c10::cuda::CUDAGuard g(in.device());
+  in = in.contiguous();
+  // the kernel reads 4 pixels as three 32-bit words: a batch slice of images with an odd byte count (x[1:] of
+  // 225x225x3 images) starts off a 4-byte boundary, so such an input goes through a fresh (aligned) copy first
+  if (reinterpret_cast<uintptr_t>(in.data_ptr()) % 4 != 0) in = in.clone(at::MemoryFormat::Contiguous);
   auto out = torch::empty(in.sizes(), in.options().dtype(torch::kBFloat16));
   float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]};
   float s[3] = {(float)(1.0 / stdv[0]), (float)(1.0 / stdv[1]), (float)(1.0 / stdv[2])};
