@@ -412,9 +412,13 @@ class BucketEngine:
             self.ctx.set_peer_timeout_ms(int(peer_timeout_ms))
             self.ctx.set_fault(int(fault))
             # DR_DETERMINISTIC=1: rank-ordered decode sums (bit-reproducible run to run); default: independent
-            # (sender, tile) work items with RED.ADD.F32 (every rank still ends with identical bits: owner computes)
+            # (sender, tile) work items with RED.ADD.F32.  Sharded, every rank still ends with identical bits: the owner
+            # of a slice computes it and the others receive its bits.  Unsharded (DR_SHARD=0, and always with the NCCL
+            # transport) every rank sums every tile itself, and at W > 2 the RED.ADD order would let the ranks' bits
+            # drift apart, so those engines always take the rank-ordered sums (at W = 2, 0 + a + b is order-free).
             self.deterministic = os.environ.get("DR_DETERMINISTIC", "0") == "1"
-            self.ctx.set_deterministic(int(self.deterministic))
+            self.rank_ordered = self.deterministic or (not self.shard and self.world > 2)
+            self.ctx.set_deterministic(int(self.rank_ordered))
             scale = (1.0 / self.world) if average else 1.0
             if filter_smem_bytes is None:      # <1>: 128 regs, 1 CTA/SM; <2>: 64 regs, 2 CTAs/SM
                 filter_smem_bytes = 160 * 1024 if blocks_per_sm < 2 else 80 * 1024
