@@ -56,7 +56,7 @@ int sm_count() {
 
 namespace {
 
-constexpr uint32_t kErrPeerWait = 2u, kErrResolve = 3u, kErrS2Overflow = 6u;
+constexpr uint32_t kErrPeerWait = 2u, kErrResolve = 3u, kErrS2Overflow = 6u, kErrDisagree = 7u;
 constexpr uint32_t kNoTensor = 0xFFFFFFFFu;
 constexpr uint32_t kFullMask = 0xFFFFFFFFu;
 constexpr uint32_t kGroupsPerTile = kTile / 32;       // 128 mask words per tile
@@ -287,6 +287,9 @@ DR_D void tile_range(const EngineParams& P, int part, uint32_t& t_begin, uint32_
 // ===========================================================================
 constexpr uint32_t kUnsafe = 0xFFFFFFFFu;   // sel.bin1 marker: history bound hid the threshold -> fallback phase
 
+// kModeShared select key of the in-tensor index i (plan.h "Selection rule"): the smallest hash gets the largest key
+DR_D uint32_t shared_key(uint32_t i, uint32_t seed) { return (0xFFFFFFFFu - policy_hash(i, seed)) >> 1; }
+
 DR_D void write_digit1(const EngineParams& P, Smem& sm, uint32_t t) {
   if (threadIdx.x == 0) {
     P.sel[t].bin1 = sm.s.res[0]; P.sel[t].krem1 = sm.s.res[1]; P.sel[t].done_epoch = 0;
@@ -384,7 +387,7 @@ DR_D uint32_t round16(uint32_t bytes) { return (bytes + 15u) & ~15u; }
 //               private slot of the ring and reads it back itself — no mbarriers, no producer, warps never wait for
 //               each other between tensor boundaries.  Selected by EngineParams::use_tma; both are kept because which
 //               one feeds HBM better is measured, not derived (scripts/engine_microbench.py).
-template <bool kTma>
+template <bool kTma, bool kFull>
 DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t parity_slot = P.epoch & 1u;
@@ -466,8 +469,13 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
     const uint32_t cur = ti.tensor;
     const TensorDesc* tdp = P.tensors + cur;
     const uint32_t mode = __ldg(&tdp->mode), fixed = __ldg(&tdp->fixed_thr);
+    // 'randomk' (full kernel only): the keys are hashes of the element index (CTA-uniform per tensor), the candidate
+    // bound is static
+    const bool shared = kFull && (mode == (uint32_t)kModeShared);
+    const uint32_t hseed = shared ? policy_seed(P.epoch, __ldg(&tdp->salt)) : 0u;
     uint32_t lower;
     if (fixed) lower = fixed;
+    else if (shared) lower = __ldg(&tdp->shared_lb);
     else {
       const uint32_t prev = P.use_history ? __ldcg(&P.sel[cur].prev_thr) : 0u;
       lower = (prev > (1u << 23)) ? prev - (1u << P.hist_shift) : 0u;      // a fraction of last step's threshold
@@ -522,8 +530,12 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
             }
             *reinterpret_cast<float4*>(r_t + off) = a;
             *reinterpret_cast<float4*>(g_t + off) = zero4;                // the dense output starts from zero
-            const uint32_t kv[4] = {__float_as_uint(a.x) & 0x7FFFFFFFu, __float_as_uint(a.y) & 0x7FFFFFFFu,
-                                    __float_as_uint(a.z) & 0x7FFFFFFFu, __float_as_uint(a.w) & 0x7FFFFFFFu};
+            uint32_t kv[4] = {__float_as_uint(a.x) & 0x7FFFFFFFu, __float_as_uint(a.y) & 0x7FFFFFFFu,
+                              __float_as_uint(a.z) & 0x7FFFFFFFu, __float_as_uint(a.w) & 0x7FFFFFFFu};
+            if (shared) {
+#pragma unroll
+              for (int j = 0; j < 4; ++j) kv[j] = shared_key(ti.local0 + e0 + (uint32_t)j, hseed);
+            }
             if (whole) {
 #pragma unroll
               for (int j = 0; j < 4; ++j) { key4[j] = kv[j]; if (kv[j] >= lower) m |= 1u << j; }
@@ -586,6 +598,7 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
 // phase 1 (rare): the history bound hid the threshold of some tensor (fewer than K candidates): redo digit 1 over
 // all of its keys and rebuild its candidate lists in full, so the later phases stay candidate-only.
 // ===========================================================================
+template <bool kFull>
 DR_D void phase_fallback(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   clear_hist(sm);
@@ -599,6 +612,9 @@ DR_D void phase_fallback(const EngineParams& P, Smem& sm) {
     const bool active = (__ldcg(&P.sel[cur].bin1) == kUnsafe) && (__ldcg(&P.sel[cur].done_epoch) != P.epoch) &&
                         (__ldg(&tdp->fixed_thr) == 0u);
     if (!active) { tile = seg_end; continue; }
+    // 'randomk': the keys are the index hashes of phase 0, not the residual's bit patterns
+    const bool shared = kFull && (__ldg(&tdp->mode) == (uint32_t)kModeShared);
+    const uint32_t hseed = shared ? policy_seed(P.epoch, __ldg(&tdp->salt)) : 0u;
     uint32_t keys[8];
     for (uint32_t tl = tile; tl < seg_end; ++tl) {
       const Tile ti = load_tile(P, tl);
@@ -610,8 +626,14 @@ DR_D void phase_fallback(const EngineParams& P, Smem& sm) {
         uint32_t key4[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
         uint32_t m = 0;
         if (e0 < ti.n) {
-          const uint4 q = __ldcg(reinterpret_cast<const uint4*>(P.resid + ti.base + e0));
-          const uint32_t kv[4] = {q.x & 0x7FFFFFFFu, q.y & 0x7FFFFFFFu, q.z & 0x7FFFFFFFu, q.w & 0x7FFFFFFFu};
+          uint32_t kv[4];
+          if (shared) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) kv[j] = shared_key(ti.local0 + e0 + (uint32_t)j, hseed);
+          } else {
+            const uint4 q = __ldcg(reinterpret_cast<const uint4*>(P.resid + ti.base + e0));
+            kv[0] = q.x & 0x7FFFFFFFu; kv[1] = q.y & 0x7FFFFFFFu; kv[2] = q.z & 0x7FFFFFFFu; kv[3] = q.w & 0x7FFFFFFFu;
+          }
 #pragma unroll
           for (int j = 0; j < 4; ++j) if (e0 + j < ti.n) { key4[j] = kv[j]; m |= 1u << j; }
         }
@@ -1221,7 +1243,8 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
         __syncwarp();
       }
       if (lane == 0) {
-        if (mode == (uint32_t)kModeBloom) my_slot[off_prefix + tile_local] = min(excl, limit);
+        // bloom: shipped prefix table; shared: sender-local scratch that the decode reads back from the own slot
+        if (mode == (uint32_t)kModeBloom || (kFull && mode == (uint32_t)kModeShared)) my_slot[off_prefix + tile_local] = min(excl, limit);
         else if (kFull && mode == (uint32_t)kModeRle)
           reinterpret_cast<uint16_t*>(my_slot + off_prefix)[tile_local] =
               (uint16_t)(excl >= limit ? 0u : min(total, limit - excl));
@@ -1738,7 +1761,51 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
     }
     load_tensor(P, t, sm);
     const uint32_t seg_end = min(t_last, sm.td.tile_begin + sm.td.n_tiles);
-    if (kFull && sm.td.mode == (uint32_t)kModeRle) {
+    if (kFull && sm.td.mode == (uint32_t)kModeShared) {
+      // 'randomk': every rank holds the same selection, so my own positive mask and my own per-tile prefix place every
+      // sender's p-th value.  A sender whose header words differ from mine drew a different set: status 7, not added.
+      const uint32_t* own = slot_ptr(arena, P, parity, P.rank);
+      const DynHeader* od = reinterpret_cast<const DynHeader*>(own + kSlotHeaderWords) + t;
+      const uint32_t o_sel = __ldcg(&od->n_sel), o_cut = __ldcg(&od->cutoff), o_thr = __ldcg(&od->thr_bits);
+      uint16_t* list = reinterpret_cast<uint16_t*>(g_filter_smem);          // in-tile offset of the rank-th positive
+      for (; tile < seg_end; ++tile) {
+        const Tile ti = load_tile(P, tile);
+        const uint32_t pre = __ldcg(own + sm.td.off_prefix + (tile - sm.td.tile_begin));
+        __syncthreads();
+        for (int j = tid; j < kTile; j += kThreads) sm.u.acc[j] = 0.0f;
+        if (warp == 0) {
+          uint32_t mm[4];
+          load_masks(P.pos_mask, tile, 0xFu, ti.n, lane, mm);
+          const uint32_t c = (uint32_t)(__popc(mm[0]) + __popc(mm[1]) + __popc(mm[2]) + __popc(mm[3]));
+          const uint32_t incl = warp_incl_scan(c, lane);
+          uint32_t lr = incl - c;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            for (uint32_t w = mm[j]; w; w &= w - 1u)
+              list[lr++] = (uint16_t)((4u * lane + (uint32_t)j) * 32u + (uint32_t)(__ffs((int)w) - 1));
+          }
+          if (lane == 31u) sm.s.lb = incl;
+        }
+        __syncthreads();
+        const uint32_t n_take = pre < o_sel ? min(sm.s.lb, o_sel - pre) : 0u;
+        for (int r = 0; r < P.world; ++r) {
+          const uint32_t* slot = slot_ptr(arena, P, parity, r);
+          const DynHeader* dyn = reinterpret_cast<const DynHeader*>(slot + kSlotHeaderWords) + t;
+          if (__ldcg(&dyn->n_sel) != o_sel || __ldcg(&dyn->cutoff) != o_cut || __ldcg(&dyn->thr_bits) != o_thr) {
+            if (tid == 0) { atomicExch(P.status, kErrDisagree); atomicExch(P.status + 1, (uint32_t)r); }
+            continue;                                                      // CTA-uniform
+          }
+          const float* vals = reinterpret_cast<const float*>(slot + sm.td.off_vals);
+          const float* fitted = P.expand_buf + (size_t)r * P.poly_total + sm.td.poly_off;
+          for (uint32_t j = tid; j < n_take; j += kThreads) {
+            const uint32_t e = list[j];                                    // distinct per sender: no atomics
+            sm.u.acc[e] = sm.u.acc[e] + __fmul_rn(coded_value<kFull>(slot, sm.td, vals, fitted, pre + j), P.scale);
+          }
+          __syncthreads();                                                 // senders are added in rank order
+        }
+        for (uint32_t e = tid; e < ti.n; e += kThreads) P.grad[ti.base + e] = sm.u.acc[e];
+      }
+    } else if (kFull && sm.td.mode == (uint32_t)kModeRle) {
       // running entry prefix of every sender at my first tile of this tensor = sum of the earlier tiles' counts
       __syncthreads();
       if (tid < 16) sm.s.rle_pre[tid] = 0u;
@@ -2094,8 +2161,8 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
       }
     }
     switch (ph) {
-      case kPhAccum: if (P.use_tma) phase_accum<true>(P, sm); else phase_accum<false>(P, sm); break;
-      case kPhFallback: phase_fallback(P, sm); break;
+      case kPhAccum: if (P.use_tma) phase_accum<true, kFull>(P, sm); else phase_accum<false, kFull>(P, sm); break;
+      case kPhFallback: phase_fallback<kFull>(P, sm); break;
       case kPhHist2: phase_hist2(P, sm); break;
       case kPhInsert: phase_insert(P, sm); break;
       case kPhQuery: phase_query(P, sm); break;
@@ -2133,7 +2200,8 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
 // filter staging; <2> = 64 regs, two CTAs per SM, up to 88 KB each.
 static bool g_attr_set = false;
 
-// ... x two feature sets: <.., false> index-only (plain pairs / bloom), <.., true> + value codecs and run-length index
+// ... x two feature sets: <.., false> index-only (plain pairs / bloom), <.., true> + value codecs, run-length index and
+// the shared 'randomk' index
 static const void* kernel_for(int blocks_per_sm, bool full) {
   if (blocks_per_sm >= 2) return full ? (const void*)dr_engine_kernel<2, true> : (const void*)dr_engine_kernel<2, false>;
   return full ? (const void*)dr_engine_kernel<1, true> : (const void*)dr_engine_kernel<1, false>;
@@ -2171,7 +2239,7 @@ cudaError_t engine_launch(const EngineParams& P, int grid, int blocks_per_sm, in
   if (e != cudaSuccess) return e;
   void* args[] = {const_cast<EngineParams*>(&P)};
   count_launch(1);
-  const bool full = P.n_poly != 0 || P.n_poly_tasks != 0 || P.has_rle != 0;
+  const bool full = P.n_poly != 0 || P.n_poly_tasks != 0 || P.has_rle != 0 || P.has_shared != 0;
   return cudaLaunchCooperativeKernel(kernel_for(blocks_per_sm, full), dim3(grid), dim3(kThreads), args,
                                      (size_t)dyn_smem_bytes, stream);
 }

@@ -24,6 +24,8 @@ enum TensorMode : uint32_t {
   kModeBloom = 1,   // bloom-filter index codec, fp32 values
   kModeRle = 2,     // lossless tile-local run coding: u16 count per 4096-element tile (off_prefix) + the cumulative
                     // zero-run offset of every selected element inside its tile, 12 bits each, LSB-first (off_idx)
+  kModeShared = 3,  // 'randomk': the index set is a seeded draw every rank computes itself (selection rule below), so
+                    // only the values travel; off_prefix is sender-local scratch (per-tile exclusive prefix)
 };
 
 enum Policy : int { kPolicyLeftmost = 0, kPolicyRandom = 1, kPolicyP0 = 2 };
@@ -58,7 +60,8 @@ struct TensorDesc {
   uint32_t poly_off;     // offset of this tensor's values in the engine's per-value scratch arrays
   uint32_t poly_ord;     // ordinal among the vmode==1 tensors (selects its bin table)
   uint32_t fixed_thr;    // != 0: 'threshold' sparsifier — select key >= fixed_thr (31-bit |x| pattern), no radix select, variable K
-  uint32_t reserved[6];
+  uint32_t shared_lb;    // kModeShared: static candidate bound on the hash key (multiple of 512; replaces the history bound)
+  uint32_t reserved[5];
 };
 static_assert(sizeof(TensorDesc) == 128, "TensorDesc must be 32 words");
 constexpr int kDescWords = 32;
@@ -104,6 +107,11 @@ constexpr uint32_t kArenaHdrWords = 128;
 //   selected  <=>  (key >> 9) >= max(T22, 1)
 // i.e. the threshold is resolved to 22 bits (8 exponent + 14 mantissa): at least K elements are
 // selected, plus the few that share the threshold's 22-bit prefix; exact zeros are never selected.
+//
+// kModeShared ('randomk', mirrored by parallel/engine.py::select_randomk_oracle): the key of the in-tensor index i is
+//   key(i) = (0xFFFFFFFF - policy_hash(i, policy_seed(epoch, salt))) >> 1      (smallest hash -> largest key)
+// and the same 22-bit rule applies to it: a superset of the K smallest hashes, plus ~numel / 2^22 elements sharing the
+// threshold's prefix.  The set depends on (numel, K, epoch, salt) only, so every rank computes the same one.
 enum Phase : int {
   kPhAccum = 0,      // r = beta*r + gamma*g ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
   kPhFallback = 1,   // (only if some bound was unsafe) digit 1 redone without the bound, candidate lists rebuilt in full
@@ -199,6 +207,7 @@ struct EngineParams {
   int fault;                     // fault injection (tests): 1 = this rank never releases its stage-1 flags
   uint32_t* mc_arena;            // NVLS multicast mapping of the symmetric arena (nullptr: per-peer P2P stores)
   int has_rle;                   // some tensor uses kModeRle (its bit stream is OR-ed, so it is zeroed every step)
+  int has_shared;                // some tensor uses kModeShared ('randomk': only the <.., true> kernel carries that path)
   int shard;                     // 1: sharded decode + stage-2 exchange (when world > 1)
   uint32_t s2_words;             // words per stage-2 slot: [count, epoch, 0, 0][idx x cap][val x cap]
   uint32_t s2_cap;               // entries per stage-2 slot

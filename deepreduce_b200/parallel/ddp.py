@@ -9,6 +9,7 @@ background thread that launches the fused exchange kernel on a high-priority
 side stream; ``finish()`` makes the optimizer's stream wait on the done events.
 
 CUDA + ('topk' [+ 'index': 'bloom' | plain])  -> fused engine (one kernel/bucket)
+CUDA + 'randomk' [+ QSGD values]              -> fused engine, values only on the wire (shared-seed index)
 CUDA + 'none'/'allreduce'                     -> dense NCCL all-reduce of the flat bucket
 anything else (CPU/gloo, other codecs)        -> GRACE-compatible per-tensor path
 """
@@ -40,11 +41,12 @@ def _is_dense(p: torch.Tensor) -> bool:
 
 
 def _fused_supported(params: dict) -> bool:
-    """Which ``params`` dicts the fused bucket engine serves (everything else takes the GRACE-compatible per-tensor
-    path).  Covers every recipe of the reference's launch script (run_deepreduce.sh:35-107): top-k or threshold
-    sparsifier x {no codec, index (bloom leftmost / random / p0, run-length), value (polyfit, QSGD int8/int16), both}.
+    """Which top-k / threshold ``params`` dicts the fused bucket engine serves with a per-rank index (everything else
+    takes the GRACE-compatible per-tensor path, unless ``_fused_randomk_supported`` takes it).  Covers every recipe of
+    the reference's launch script (run_deepreduce.sh:35-107): top-k or threshold sparsifier x {no codec, index (bloom
+    leftmost / random / p0, run-length), value (polyfit, QSGD int8/int16), both}.
     Not fused: bloom policy 'conflict_sets' (per-tensor GPU kernel), host codecs (Huffman, Deflate, dexp, the integer
-    family), 'randomk', non-512 QSGD buckets."""
+    family), non-512 QSGD buckets."""
     if params.get('compressor') not in ('topk', 'threshold') or params.get('communicator', 'allgather') != 'allgather':
         return False
     dr = params.get('deepreduce', None)
@@ -66,6 +68,24 @@ def _fused_supported(params: dict) -> bool:
     return False
 
 
+def _fused_randomk_supported(params: dict) -> bool:
+    """Which 'randomk' ``params`` dicts the fused engine serves in its shared-index mode (``kModeShared``): every rank
+    draws the same index set from (step, tensor), so only values travel and the allgather and allreduce communicators
+    give the same aggregate.  With no codec, or with QSGD values (``'deepreduce': 'value', 'value': 'qsgd'``, bucket
+    512).  Not fused: 'randomk' with an index codec, 'both', or polyfit values."""
+    if params.get('compressor') != 'randomk' or params.get('communicator', 'allgather') not in ('allgather', 'allreduce'):
+        return False
+    dr = params.get('deepreduce', None)
+    return dr is None or (dr == 'value' and params.get('value', 'polyfit') == 'qsgd'
+                          and 1 <= int(params.get('quantum_num', 127)) <= 32767
+                          and int(params.get('bucket_size', 512)) == 512)
+
+
+def fused_path(params: dict) -> bool:
+    """True if ``DeepReduceDDP`` on CUDA runs ``params`` through the fused bucket engine."""
+    return _fused_supported(params) or _fused_randomk_supported(params)
+
+
 def plan_kwargs_from_params(params: dict) -> dict:
     """``params`` dict (the reference's ``--grace_config``) -> BucketPlan keyword arguments."""
     from ..codecs.bloom import canonical_policy
@@ -82,6 +102,8 @@ def plan_kwargs_from_params(params: dict) -> dict:
     if params.get('compressor') == 'threshold':
         kw.update(sparsifier='threshold', threshold=float(params.get('threshold', 0.0)),
                   capacity_ratio=params.get('threshold_capacity', None))
+    elif params.get('compressor') == 'randomk':
+        kw.update(sparsifier='randomk')
     return kw
 
 
@@ -98,7 +120,7 @@ class DeepReduceDDP:
         self.device = self.named[0][1].device
         self.is_cuda = self.device.type == "cuda"
         self.dense = self.params.get('compressor', 'none') in ('none', None)
-        self.fused = self.is_cuda and not self.dense and _fused_supported(self.params)
+        self.fused = self.is_cuda and not self.dense and fused_path(self.params)
         self.overlap = overlap and self.is_cuda
         self.step_count = 0
         self.engines: List[BucketEngine] = []

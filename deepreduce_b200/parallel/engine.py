@@ -33,7 +33,7 @@ import torch.distributed as dist
 from .. import spec
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle
 from .plan import update_cta_speeds
-from .plan import (ARENA_HDR_WORDS, DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, NUM_HIST, POLICY_ID,
+from .plan import (ARENA_HDR_WORDS, DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID,
                    SLOT_HEADER_WORDS, BucketPlan, rle_stream_words)
 
 (PH_ACCUM, PH_FALLBACK, PH_HIST2, PH_INSERT, PH_QUERY, PH_EMIT, PH_RANK_HIST, PH_RANK_SCAN, PH_RANK_SCATTER,
@@ -41,7 +41,8 @@ from .plan import (ARENA_HDR_WORDS, DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, 
  PH_SCATTER, PH_END) = range(21)
 MAGIC = 0xD33B2000
 STATUS_NAMES = {0: "ok", 1: "(unused)", 2: "peer flag watchdog", 3: "select resolve failed", 4: "grid barrier watchdog", 5: "TMA mbarrier watchdog",
-                6: "stage-2 slot overflow (sharded decode)"}
+                6: "stage-2 slot overflow (sharded decode)",
+                7: "ranks disagree on the 'randomk' draw (a sender's header differs from the receiver's)"}
 
 
 # ---------------------------------------------------------------------------
@@ -89,6 +90,18 @@ def select_threshold_oracle(acc: torch.Tensor, fixed_thr: int):
     return torch.nonzero(_abs_keys(acc) >= fixed_thr).flatten(), int(fixed_thr)
 
 
+def select_randomk_oracle(numel: int, k: int, epoch: int, salt: int):
+    """'randomk' selection rule of the fused engine (normative, see ops/csrc/plan.h): with
+    key(i) = (0xFFFFFFFF - policy_hash(i, policy_seed(epoch, salt))) >> 1, the top-k rule on the keys.  A superset of
+    the K smallest hashes plus the few sharing the threshold's 22-bit prefix; it depends on (numel, K, epoch, salt)
+    only, so every rank computes the same set.  Returns (ascending indices, threshold key lower bound)."""
+    h = spec.policy_hash(torch.arange(int(numel), dtype=torch.int64), spec.policy_seed(int(epoch), int(salt)))
+    keys = (0xFFFFFFFF - h) >> 1
+    kth = int(torch.topk(keys, int(k), sorted=True).values[-1].item())
+    T22 = max(kth >> 9, 1)
+    return torch.nonzero((keys >> 9) >= T22).flatten(), T22 << 9
+
+
 def random_policy_filter(pos: torch.Tensor, n_ins: int, limit: int, epoch: int, salt: int, T: Optional[int] = None):
     """'random' policy of the fused engine: keep the positives x with policy_hash(x, policy_seed(step, tensor)) <= T,
     T = floor(2^32 * min(n_ins, limit) / n_pos) (0xFFFFFFFF = keep all when nothing has to go).  Sender: T from the
@@ -103,8 +116,12 @@ def random_policy_filter(pos: torch.Tensor, n_ins: int, limit: int, epoch: int, 
 
 def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, policy: str, seed: int, epoch: int = 1):
     """Encode one tensor into `slot` (uint32 numpy view); returns new residual."""
-    sel_topk, T = (select_threshold_oracle(acc, tp.fixed_thr) if getattr(tp, "fixed_thr", 0)
-                   else select_topk_oracle(acc, tp.k))
+    if tp.mode == MODE_SHARED:
+        sel_topk, T = select_randomk_oracle(tp.numel, tp.k, epoch, tp.salt)
+    elif getattr(tp, "fixed_thr", 0):
+        sel_topk, T = select_threshold_oracle(acc, tp.fixed_thr)
+    else:
+        sel_topk, T = select_topk_oracle(acc, tp.k)
     dyn = SLOT_HEADER_WORDS + DYN_WORDS * t_index
     resid = acc.clone()
     if tp.mode == MODE_BLOOM:
@@ -144,6 +161,12 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
         cnt[:tp.n_tiles] = np.bincount(s_np // spec.TILE, minlength=tp.n_tiles).astype(np.uint16)
         slot[tp.off_prefix:tp.off_prefix + (tp.n_tiles + 1) // 2] = cnt.view(np.uint32)
         slot[tp.off_idx:tp.off_idx + rle_stream_words(tp.val_cap)] = rle_pack12(s_np % spec.TILE, tp.val_cap)
+        cutoff = int(sel[-1].item()) if n_pos >= limit else 0xFFFFFFFF
+    elif tp.mode == MODE_SHARED:
+        # no index on the wire: every receiver draws the same set (the per-tile prefix is sender-local scratch)
+        n_pos = int(sel_topk.numel())
+        limit = tp.val_cap
+        sel = sel_topk[:limit]
         cutoff = int(sel[-1].item()) if n_pos >= limit else 0xFFFFFFFF
     else:
         n_pos = int(sel_topk.numel())
@@ -266,6 +289,14 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
             assert int(cnt.sum()) == n_sel, t.name
             local = rle_unpack12(a[t.off_idx:t.off_idx + rle_stream_words(t.val_cap)], n_sel)
             idx = torch.from_numpy(np.repeat(np.arange(t.n_tiles, dtype=np.int64), cnt) * spec.TILE + local)
+        elif t.mode == MODE_SHARED:
+            # the index set is drawn again from the plan and the epoch in slot word 1; the sender's threshold must match
+            pos, thr = select_randomk_oracle(t.numel, t.k, int(a[1]), t.salt)
+            assert thr == int(a[d0 + 2]), (t.name, thr, int(a[d0 + 2]))
+            if cutoff != 0xFFFFFFFF:
+                pos = pos[pos <= cutoff]
+            idx = pos[:n_sel]
+            assert int(idx.numel()) == n_sel, t.name
         else:
             idx = torch.from_numpy(a[t.off_idx:t.off_idx + n_sel].astype(np.int64))
         n = int(idx.numel())
@@ -320,6 +351,8 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
         elif t.mode == MODE_RLE:
             ibytes = 4 * ((t.n_tiles + 1) // 2 + rle_stream_words(t.val_cap))
             false_pos = 0
+        elif t.mode == MODE_SHARED:
+            ibytes, false_pos = 0, 0                         # every rank draws the index set itself
         else:
             ibytes, false_pos = 4 * t.val_cap, 0
         row = {"name": t.name, "numel": t.numel, "k": t.k, "n_sel": n_sel, "n_pos": n_pos, "false_pos": false_pos,
@@ -328,6 +361,8 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
         if plan.policy == "random" and t.mode == MODE_BLOOM:   # header word 2 is the policy's acceptance threshold here
             row["threshold"] = None
             row["accept_rate"] = 1.0 if thr_bits == 0xFFFFFFFF else thr_bits / 2.0 ** 32
+        if t.mode == MODE_SHARED:                            # header word 2 is a hash-key threshold, not a magnitude
+            row["threshold"] = None
         per.append(row)
         for key in tot:
             tot[key] += row[key]
@@ -428,6 +463,7 @@ class BucketEngine:
             if getattr(self, "multicast_ptr", 0):
                 self.ctx.set_multicast(self.multicast_ptr)
             self.ctx.set_has_rle(int(any(t.mode == MODE_RLE for t in plan.tensors)))
+            self.ctx.set_has_shared(int(any(t.mode == MODE_SHARED for t in plan.tensors)))
             ids, n_poly, tasks, n_tasks = plan.poly_tables()
             self.poly_ids, self.poly_tasks = ids.to(dev), tasks.to(dev)
             from .plan import RANK_BINS

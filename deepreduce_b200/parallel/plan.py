@@ -18,7 +18,8 @@ import torch
 
 from .. import spec
 
-MODE_RAW, MODE_BLOOM, MODE_RLE = 0, 1, 2
+MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED = 0, 1, 2, 3
+KEY_SPAN = 1 << 31                    # select keys are 31-bit
 POLICY_ID = {"leftmost": 0, "random": 1, "p0": 2}
 SLOT_HEADER_WORDS = 8
 DYN_WORDS = 4
@@ -55,6 +56,23 @@ def rle_stream_words(k: int) -> int:
 
 def _align(x: int, a: int) -> int:
     return (x + a - 1) // a * a
+
+
+def randomk_capacity(d: int, k: int) -> int:
+    """Slot capacity of a 'randomk' tensor: K plus room for the elements that share the threshold's 22-bit key prefix
+    (about d / 2^22 expected; more than the slack are cut left-most, consistently on every rank)."""
+    return min(d, k + 16 + (d >> 20))
+
+
+def randomk_bound(d: int, k: int) -> int:
+    """Static candidate bound of a 'randomk' tensor: the hash key above which K + 8 sqrt(K) + 16 of its d uniformly
+    distributed keys are expected, rounded down to a 22-bit prefix boundary (so it never splits the threshold's bin).
+    The K-th largest key falls below it only if the count above it is some 8 standard deviations short; then the
+    kernel's fallback phase redoes the select over every key."""
+    m = k + int(math.ceil(8.0 * math.sqrt(k))) + 16
+    if m >= d:
+        return 0
+    return (KEY_SPAN * (d - m) // d) & ~511
 
 
 def split_large(numels, names, shapes, split_numel: Optional[int]):
@@ -130,13 +148,14 @@ class TensorPlan:
     poly_off: int = 0
     poly_ord: int = 0
     fixed_thr: int = 0        # 'threshold' sparsifier: select |x| bit pattern >= fixed_thr (0: top-k radix select)
+    shared_lb: int = 0        # MODE_SHARED: static candidate bound on the hash key (randomk_bound)
 
     def words(self) -> List[int]:
         return [self.elem_off, self.numel, self.k, self.tile_begin, self.n_tiles, self.mode, self.m_bits,
                 self.n_hash, self.off_vals, self.off_filter, self.off_prefix, self.off_idx, self.val_cap,
                 self.salt, self.n_filter_words, self.off_hint, self.vmode, self.off_coef, self.off_rankmap,
                 self.off_selidx, self.off_sorted, self.poly_degree, self.rank_u32, self.poly_off, self.poly_ord,
-                self.fixed_thr, 0, 0, 0, 0, 0, 0]
+                self.fixed_thr, self.shared_lb, 0, 0, 0, 0, 0]
 
 
 @dataclass
@@ -157,6 +176,7 @@ class BucketPlan:
     poly_degree: int = 5
     poly_min_k: int = 512                 # tensors shipping fewer values keep them as fp32 (the fit header would be larger)
     sparsifier: str = "topk"              # 'topk' (radix select of the K largest) | 'threshold' (|x| > threshold, variable K)
+                                          # | 'randomk' (seeded index draw every rank repeats: only values are shipped)
     threshold: float = 0.0
     capacity_ratio: Optional[float] = None   # 'threshold': slot capacity as a fraction of d (default 1.0 = lossless)
     raw_slack: int = 0                    # plain-pair tensors: room for this many coordinates beyond K (the select keeps
@@ -170,8 +190,14 @@ class BucketPlan:
             raise NotImplementedError("value codecs are fused with the bloom index or plain indices, not with 'rle'")
         if self.value not in (None, "polyfit", "qsgd"):
             raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd'; got {self.value!r}")
-        if self.sparsifier not in ("topk", "threshold"):
-            raise ValueError(f"fused engine sparsifiers: 'topk', 'threshold'; got {self.sparsifier!r}")
+        if self.sparsifier not in ("topk", "threshold", "randomk"):
+            raise ValueError(f"fused engine sparsifiers: 'topk', 'threshold', 'randomk'; got {self.sparsifier!r}")
+        shared = self.sparsifier == "randomk"
+        if shared and self.index is not None:
+            raise ValueError("'randomk' ships no index (every rank draws the same set): pass index=None")
+        if shared and self.value == "polyfit":
+            # rank_bin centres the value bins on the selection threshold, which here is a hash, not a magnitude
+            raise NotImplementedError("'randomk' is fused with fp32 or QSGD values, not with 'polyfit'")
         if self.value == "qsgd" and not (1 <= int(self.quantum_num) <= 32767):
             raise ValueError("quantum_num must be in [1, 32767]")
         fixed_thr = 0
@@ -202,7 +228,18 @@ class BucketPlan:
             tp = TensorPlan(name=names[i], numel=d, shape=tuple(shapes[i]), elem_off=elem, k=k, tile_begin=tile,
                             n_tiles=n_tiles, mode=MODE_RAW, salt=i, poly_degree=int(self.poly_degree),
                             fixed_thr=fixed_thr)
-            if self.index == "bloom" and d > self.min_numel:
+            if shared:
+                # values only (+ the dyn header); the per-tile prefix is sender-local scratch the decode reads back
+                tp.mode = MODE_SHARED
+                tp.val_cap = randomk_capacity(d, k)
+                tp.shared_lb = randomk_bound(d, k)
+                if d > self.min_numel:
+                    word = self._value_region(tp, word, scratch)
+                else:
+                    tp.off_vals = word
+                    word = _align(word + tp.val_cap, 4)
+                scratch.append((tp, "off_prefix", n_tiles))
+            elif self.index == "bloom" and d > self.min_numel:
                 n_hash, m_bits, n_words = spec.bloom_layout(k, d, self.fpr, self.max_hash)
                 tp.mode = MODE_BLOOM
                 tp.m_bits, tp.n_hash, tp.n_filter_words = m_bits, n_hash, n_words

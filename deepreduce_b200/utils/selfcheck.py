@@ -21,18 +21,19 @@ import torch.distributed as dist
 
 from .. import spec
 from ..codecs.bloom import bloom_query_oracle
-from ..parallel.plan import DYN_WORDS, MODE_BLOOM, MODE_RAW, SLOT_HEADER_WORDS
+from ..parallel.plan import DYN_WORDS, MODE_BLOOM, MODE_RAW, MODE_SHARED, SLOT_HEADER_WORDS
 
 
 def decode_slot_torch(plan, slot: torch.Tensor, seed: int = spec.DEFAULT_SEED):
     """One sender's dense contribution (flat fp32, unscaled) rebuilt from the words of its slot with torch ops on the
-    slot's device.  Supports the fp32-value modes (bloom index with/without hint, plain pairs); returns None if the
-    plan uses a mode this decoder does not cover (value codecs, run-length) — callers then skip check 3."""
+    slot's device.  Supports the fp32-value modes (bloom index with/without hint, plain pairs, the shared 'randomk'
+    index); returns None if the plan uses a mode this decoder does not cover (value codecs, run-length) — callers then
+    skip check 3."""
     dev = slot.device
     hdr = slot[:SLOT_HEADER_WORDS + DYN_WORDS * len(plan.tensors)].to(torch.int64).cpu() & 0xFFFFFFFF
     out = torch.zeros(plan.total_elems, dtype=torch.float32, device=dev)
     for ti, t in enumerate(plan.tensors):
-        if t.vmode != 0 or t.mode not in (MODE_BLOOM, MODE_RAW):
+        if t.vmode != 0 or t.mode not in (MODE_BLOOM, MODE_RAW, MODE_SHARED):
             return None
         d0 = SLOT_HEADER_WORDS + DYN_WORDS * ti
         n_sel, cutoff = int(hdr[d0]), int(hdr[d0 + 1])
@@ -49,6 +50,12 @@ def decode_slot_torch(plan, slot: torch.Tensor, seed: int = spec.DEFAULT_SEED):
                 T = int(hdr[d0 + 2])
                 if T != 0xFFFFFFFF:
                     pos = pos[(spec.policy_hash(pos, spec.policy_seed(int(hdr[1]), t.salt)) <= T).to(pos.device)]
+            if cutoff != 0xFFFFFFFF:
+                pos = pos[pos <= cutoff]
+            idx = pos[:n_sel]
+        elif t.mode == MODE_SHARED:                        # no index on the wire: draw the set from the plan + the step
+            from ..parallel.engine import select_randomk_oracle
+            pos = select_randomk_oracle(t.numel, t.k, int(hdr[1]), t.salt)[0].to(dev)
             if cutoff != 0xFFFFFFFF:
                 pos = pos[pos <= cutoff]
             idx = pos[:n_sel]
