@@ -509,6 +509,15 @@ struct Engine {
     P.shard = shard; P.s2_words = (uint32_t)s2_words; P.s2_cap = (uint32_t)s2_cap;
   }
 
+  // bf16 bucket: the bf16 dense gradient (in and out; the constructor's grad is then unused) and the fp32 apply
+  // accumulator of acc_tiles tiles (every tile this rank decodes, or 0 when no tensor is applied through it)
+  void set_bf16(int64_t grad_bf16, int64_t acc32, int64_t acc_tiles) {
+    TORCH_CHECK(grad_bf16 != 0, "set_bf16: null gradient");
+    TORCH_CHECK(acc_tiles == 0 || acc32 != 0, "set_bf16: null accumulator");
+    P.grad_bf16 = reinterpret_cast<uint16_t*>(grad_bf16); P.acc32 = reinterpret_cast<float*>(acc32);
+    P.acc_tiles = (uint32_t)acc_tiles; P.bf16 = 1;
+  }
+
   void set_buffers(int64_t grad, int64_t resid) {
     P.grad = reinterpret_cast<float*>(grad); P.resid = reinterpret_cast<float*>(resid);
   }
@@ -522,6 +531,12 @@ struct Engine {
     EngineParams Q = P;
     Q.epoch = epoch; Q.phase_begin = phase_begin; Q.phase_end = phase_end;
     TORCH_CHECK(P.pos_mask && P.cand, "Engine: set_scratch() was not called");
+    if (P.bf16 && P.acc_tiles) {                 // one acc32 row per tile of the span engine.cu decode_span gives this rank
+      const uint32_t span = (P.shard && P.world > 1)
+          ? (uint32_t)(((uint64_t)P.n_tiles * (P.rank + 1)) / P.world - ((uint64_t)P.n_tiles * P.rank) / P.world)
+          : P.n_tiles;
+      TORCH_CHECK(P.acc_tiles >= span, "Engine: the bf16 accumulator covers ", P.acc_tiles, " tiles, the decode span ", span);
+    }
     int g = get_grid();
     if (grid_cap > 0 && grid_cap < g) g = grid_cap;
     cudaError_t e = dr::engine_launch(Q, g, blocks_per_sm, dyn_smem, st);
@@ -696,6 +711,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                     int64_t, int64_t, int64_t, std::vector<int64_t>, int, int>())
       .def("configure", &Engine::configure)
       .def("set_buffers", &Engine::set_buffers)
+      .def("set_bf16", &Engine::set_bf16)
       .def("set_poly", &Engine::set_poly)
       .def("set_shard", &Engine::set_shard)
       .def("set_has_rle", &Engine::set_has_rle)

@@ -32,6 +32,8 @@
 #include "common.cuh"
 #include "plan.h"
 
+#include <cuda_bf16.h>
+
 #include <atomic>
 #include <cstdio>
 
@@ -122,6 +124,25 @@ DR_D void decode_range(const EngineParams& P, uint32_t& tile, uint32_t& t_end) {
   const uint32_t span = s_end - s_begin;
   tile = s_begin + (uint32_t)(((uint64_t)span * blockIdx.x) / gridDim.x);
   t_end = s_begin + (uint32_t)(((uint64_t)span * (blockIdx.x + 1)) / gridDim.x);
+}
+
+// final value of dense output element i: fp32 as is, bf16 rounded once to nearest-even
+template <bool kB>
+DR_D void put_out(const EngineParams& P, size_t i, float v) {
+  if constexpr (kB) P.grad_bf16[i] = __bfloat16_as_ushort(__float2bfloat16_rn(v));
+  else P.grad[i] = v;
+}
+
+// four consecutive bf16 (8 bytes, element 0 in the low half of x) widened to fp32 — exact
+DR_D float4 widen_bf16x4(uint2 h) {
+  return make_float4(__uint_as_float(h.x << 16), __uint_as_float(h.x & 0xFFFF0000u), __uint_as_float(h.y << 16),
+                     __uint_as_float(h.y & 0xFFFF0000u));
+}
+
+// bf16 buckets whose bloom tensor is applied by phase_compact (every sender added into acc32, then rounded): all of them
+// except where emit already scattered the rank's own values (W == 1, fp32 values)
+DR_D bool bloom_applied(const EngineParams& P, uint32_t mode, uint32_t vmode) {
+  return mode == (uint32_t)kModeBloom && !(P.world == 1 && vmode == 0u);
 }
 
 struct Tile { uint32_t tensor, base, n, local0, single; };   // `single`: the tensor has exactly one tile
@@ -387,7 +408,10 @@ DR_D uint32_t round16(uint32_t bytes) { return (bytes + 15u) & ~15u; }
 //               private slot of the ring and reads it back itself — no mbarriers, no producer, warps never wait for
 //               each other between tensor boundaries.  Selected by EngineParams::use_tma; both are kept because which
 //               one feeds HBM better is measured, not derived (scripts/engine_microbench.py).
-template <bool kTma, bool kFull>
+// kB = true    : bf16 bucket.  The g half of a stage holds the bf16 half-tile (4 KB, the rest of its 8 KB unused, so the
+//               ring arithmetic is the same), each thread widens its 8 bytes in registers and zero-fills its 8 bytes of
+//               the bf16 output; the rows of acc32 that the apply of this step adds into are zeroed here too.
+template <bool kTma, bool kFull, bool kB>
 DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t parity_slot = P.epoch & 1u;
@@ -406,6 +430,8 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   for (int j = tid; j < 2 * kHistBins; j += kThreads) sm.u.hist[j] = 0;
   __syncthreads();
   const bool has_resid = (P.beta != 0.0f);
+  uint32_t acc_begin = 0, acc_end = 0;         // bf16: the tiles this rank decodes own the rows of acc32
+  if constexpr (kB) decode_span(P, P.rank, acc_begin, acc_end);
   uint32_t t0, t_end;
   tile_range(P, kPartAccum, t0, t_end);
   if (t0 >= t_end) return;
@@ -437,13 +463,20 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
         uint8_t* dst = ring + (size_t)p_stage * kStageBytes;
         if (kTma) {
           const uint32_t bytes = round16(min(t.n - off, kHalf) * 4u);
-          mbar_expect_tx(&full[p_stage], has_resid ? 2u * bytes : bytes);
-          bulk_g2s(dst, P.grad + t.base + off, bytes, &full[p_stage]);
+          if constexpr (kB) {                           // tensors start at 32-element boundaries: 16-byte aligned source
+            const uint32_t gbytes = round16(min(t.n - off, kHalf) * 2u);
+            mbar_expect_tx(&full[p_stage], has_resid ? gbytes + bytes : gbytes);
+            bulk_g2s(dst, P.grad_bf16 + t.base + off, gbytes, &full[p_stage]);
+          } else {
+            mbar_expect_tx(&full[p_stage], has_resid ? 2u * bytes : bytes);
+            bulk_g2s(dst, P.grad + t.base + off, bytes, &full[p_stage]);
+          }
           if (has_resid) bulk_g2s(dst + kHalf * 4u, P.resid + t.base + off, bytes, &full[p_stage]);
-        } else {                                        // this thread's own 16 bytes of g and of r
+        } else {                                        // this thread's own 16 bytes of g and of r (bf16: 8 bytes of g)
           const uint32_t e0 = off + tid * 4u;
           if (e0 < t.n) {
-            cp_async_16(dst + tid * 16u, P.grad + t.base + e0);
+            if constexpr (kB) cp_async_8(dst + tid * 8u, P.grad_bf16 + t.base + e0);
+            else cp_async_16(dst + tid * 16u, P.grad + t.base + e0);
             if (has_resid) cp_async_16(dst + kHalf * 4u + tid * 16u, P.resid + t.base + e0);
           }
           cp_async_commit();
@@ -469,6 +502,8 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
     const uint32_t cur = ti.tensor;
     const TensorDesc* tdp = P.tensors + cur;
     const uint32_t mode = __ldg(&tdp->mode), fixed = __ldg(&tdp->fixed_thr);
+    bool zero_acc = false;                                                 // bf16: this tensor's rows of acc32 start from 0
+    if constexpr (kB) zero_acc = bloom_applied(P, mode, __ldg(&tdp->vmode));
     // 'randomk' (full kernel only): the keys are hashes of the element index (CTA-uniform per tensor), the candidate
     // bound is static
     const bool shared = kFull && (mode == (uint32_t)kModeShared);
@@ -519,7 +554,9 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
           uint32_t m = 0;
           const bool whole = (ti.n - off) >= kHalf;                        // CTA-uniform fast path: no bounds checks
           if (whole || e0 < ti.n) {
-            const float4 g = sg[tid];
+            float4 g;
+            if constexpr (kB) g = widen_bf16x4(reinterpret_cast<const uint2*>(sg)[tid]);
+            else g = sg[tid];
             float4 a;
             if (has_resid) {
               const float4 r = sr[tid];
@@ -529,7 +566,13 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
               a.x = gamma * g.x; a.y = gamma * g.y; a.z = gamma * g.z; a.w = gamma * g.w;
             }
             *reinterpret_cast<float4*>(r_t + off) = a;
-            *reinterpret_cast<float4*>(g_t + off) = zero4;                // the dense output starts from zero
+            if constexpr (kB) {
+              *reinterpret_cast<uint2*>(P.grad_bf16 + ti.base + e0) = make_uint2(0u, 0u);
+              if (zero_acc && tile >= acc_begin && tile < acc_end)
+                *reinterpret_cast<float4*>(P.acc32 + (size_t)(tile - acc_begin) * kTile + e0) = zero4;
+            } else {
+              *reinterpret_cast<float4*>(g_t + off) = zero4;              // the dense output starts from zero
+            }
             uint32_t kv[4] = {__float_as_uint(a.x) & 0x7FFFFFFFu, __float_as_uint(a.y) & 0x7FFFFFFFu,
                               __float_as_uint(a.z) & 0x7FFFFFFFu, __float_as_uint(a.w) & 0x7FFFFFFFu};
             if (shared) {
@@ -1121,7 +1164,7 @@ DR_D void policy_filter(const EngineParams& P, Smem& sm) {
   }
 }
 
-template <bool kFull>
+template <bool kFull, bool kB>
 DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t parity = P.epoch & 1u;
@@ -1231,7 +1274,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
             const uint32_t rp = excl + base + q;
             vals[rp] = v;
             P.resid[gi] = 0.0f;                                            // residual is exactly 0 on the shipped set
-            if (scatter) P.grad[gi] = v * P.scale;
+            if (scatter) put_out<kB>(P, gi, v * P.scale);
             if (mode == (uint32_t)kModeRaw) idxs[rp] = ti.local0 + e;
             else if (kFull && mode == (uint32_t)kModeRle) rle_put(idxs, rp, e);
             if (kFull && vmode) my_slot[off_selidx + rp] = (uint32_t)gi;
@@ -1610,6 +1653,7 @@ DR_D void phase_push(const EngineParams& P, Smem& sm) {
 // wait is bounded by WALL TIME (peer_timeout_ms — a rank can legitimately be seconds late: checkpoint, dataloader
 // stall, first-step autotune), and on expiry the status word is set, the output is poisoned with NaN and the CTA
 // leaves the kernel without decoding slots the peer may still be writing.  Returns false (CTA-uniform) on timeout.
+template <bool kB>
 DR_D bool wait_flags(const EngineParams& P, uint32_t base, uint32_t aux_base) {
   const int p = threadIdx.x;
   int bad = 0;
@@ -1631,7 +1675,10 @@ DR_D bool wait_flags(const EngineParams& P, uint32_t base, uint32_t aux_base) {
   if (any_bad && threadIdx.x == 0) {                     // poison: the aggregate of this step does not exist
     uint32_t tile, t_end;
     decode_range(P, tile, t_end);
-    if (tile < t_end) P.grad[load_tile(P, tile).base] = __uint_as_float(0x7FC00000u);
+    if (tile < t_end) {
+      if constexpr (kB) P.grad_bf16[load_tile(P, tile).base] = 0x7FC0u;
+      else P.grad[load_tile(P, tile).base] = __uint_as_float(0x7FC00000u);
+    }
   }
   return !any_bad;
 }
@@ -1739,7 +1786,7 @@ DR_D void dbg_stamp(const EngineParams& P, int slot, int which) {
   if (P.debug_times && threadIdx.x == 0) P.debug_times[((size_t)slot * gridDim.x + blockIdx.x) * 2 + which] = globaltimer_ns();
 }
 
-template <bool kFull>
+template <bool kFull, bool kB>
 DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t parity = P.epoch & 1u;
@@ -1803,7 +1850,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           }
           __syncthreads();                                                 // senders are added in rank order
         }
-        for (uint32_t e = tid; e < ti.n; e += kThreads) P.grad[ti.base + e] = sm.u.acc[e];
+        for (uint32_t e = tid; e < ti.n; e += kThreads) put_out<kB>(P, ti.base + e, sm.u.acc[e]);
       }
     } else if (kFull && sm.td.mode == (uint32_t)kModeRle) {
       // running entry prefix of every sender at my first tile of this tensor = sum of the earlier tiles' counts
@@ -1836,7 +1883,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           __syncthreads();                                  // senders are added in rank order: deterministic sums
           if (tid == 0) sm.s.rle_pre[r] = pre + c;
         }
-        for (uint32_t e = tid; e < ti.n; e += kThreads) P.grad[ti.base + e] = sm.u.acc[e];
+        for (uint32_t e = tid; e < ti.n; e += kThreads) put_out<kB>(P, ti.base + e, sm.u.acc[e]);
       }
     } else {
       for (; tile < seg_end; ++tile) {
@@ -1866,7 +1913,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           }
           __syncthreads();                                  // rank-major: one sender at a time
         }
-        for (uint32_t e = tid; e < ti.n; e += kThreads) P.grad[ti.base + e] = sm.u.acc[e];
+        for (uint32_t e = tid; e < ti.n; e += kThreads) put_out<kB>(P, ti.base + e, sm.u.acc[e]);
       }
     }
   }
@@ -1970,8 +2017,11 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
         fill_list(list, mm, incl - c, base, lane);
         __syncwarp();
         const uint32_t n_here = min(kListCap, n_take - base);
-        for (uint32_t q = lane; q < n_here; q += 32u)
-          atomicAdd(P.grad + ti.base + list[q], coded_value<kFull>(slot, td, vals, fitted, pre + base + q) * P.scale);
+        for (uint32_t q = lane; q < n_here; q += 32u) {
+          const float v = coded_value<kFull>(slot, td, vals, fitted, pre + base + q) * P.scale;
+          if constexpr (kB) atomicAdd(P.acc32 + (size_t)(tl - s_begin) * kTile + list[q], v);   // the tile's acc32 row
+          else atomicAdd(P.grad + ti.base + list[q], v);
+        }
         __syncwarp();
       }
     }
@@ -2014,15 +2064,35 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           const uint32_t n_here = min(kListCap, n_take - base);
           for (uint32_t q = lane; q < n_here; q += 32u) {
             const uint32_t e = list[q];
-            float* o = P.grad + ti.base + e;
+            float* o;                                                      // bf16: the tile's acc32 row
+            if constexpr (kB) o = P.acc32 + (size_t)(tl - s_begin) * kTile + e;
+            else o = P.grad + ti.base + e;
             *o = *o + coded_value<kFull>(slot, td, vals, fitted, pre + base + q) * P.scale;
           }
           __syncwarp();
         }
       }
     }
+    if constexpr (kB) {
+      // every sender of the tile is in its acc32 row: round once into the bf16 output (the row was zeroed in phase 0 up
+      // to the tile's element count rounded up to 4, so the 4-wide pass below reads only zeroed words)
+      if (bloom_applied(P, td.mode, td.vmode)) {
+        __syncwarp();
+        const float4* row = reinterpret_cast<const float4*>(P.acc32 + (size_t)(tl - s_begin) * kTile);
+        const uint32_t n4 = (ti.n + 3u) >> 2;
+        for (uint32_t i = lane; i < n4; i += 32u) {
+          const float4 a = __ldcg(row + i);
+          const uint32_t lo = (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(a.x)) |
+                              ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(a.y)) << 16);
+          const uint32_t hi = (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(a.z)) |
+                              ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(a.w)) << 16);
+          reinterpret_cast<uint2*>(P.grad_bf16 + ti.base)[i] = make_uint2(lo, hi);
+        }
+      }
+    }
     if (stage2) {
-      // the tile is final (every sender added, or written by part (1)): its non-zeros go to the peers
+      // the tile is final (every sender added, or written by part (1)): its non-zeros go to the peers (bf16: the rounded
+      // values, shipped as their exact fp32 widening)
       __syncwarp();
       const float4* src4 = reinterpret_cast<const float4*>(P.grad + ti.base);
       const uint32_t n4 = (ti.n + 3u) >> 2;                                  // tensors are padded to 32 floats
@@ -2031,7 +2101,9 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const uint32_t i = i0 + (uint32_t)u * 32u + lane;
-          v4[u] = i < n4 ? __ldcg(src4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+          if constexpr (kB) v4[u] = i < n4 ? widen_bf16x4(__ldcg(reinterpret_cast<const uint2*>(P.grad_bf16 + ti.base) + i))
+                                           : make_float4(0.f, 0.f, 0.f, 0.f);
+          else v4[u] = i < n4 ? __ldcg(src4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
@@ -2039,7 +2111,11 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           const float vv[4] = {v4[u].x, v4[u].y, v4[u].z, v4[u].w};
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const bool nz = vv[j] != 0.f && (i * 4u + (uint32_t)j) < ti.n;
+            // bf16: a rounded -0 (an fp32 aggregate never is -0: every sum starts from +0) travels like any value, so
+            // the receivers' bits stay the owner's; only +0 is the zero fill every rank already holds
+            bool nz;
+            if constexpr (kB) nz = __float_as_uint(vv[j]) != 0u && (i * 4u + (uint32_t)j) < ti.n;
+            else nz = vv[j] != 0.f && (i * 4u + (uint32_t)j) < ti.n;
             const uint32_t bal = __ballot_sync(kFullMask, nz);
             if (nz) {
               const uint32_t pos = n_st + (uint32_t)__popc(bal & lt);
@@ -2100,6 +2176,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   }
 }
 
+template <bool kB>
 DR_D void phase_scatter(const EngineParams& P) {
   const uint32_t parity = P.epoch & 1u;
   const uint32_t gtid = blockIdx.x * kThreads + threadIdx.x, gsz = gridDim.x * kThreads;
@@ -2108,7 +2185,7 @@ DR_D void phase_scatter(const EngineParams& P) {
     const uint32_t* s2 = s2_ptr(P.arena[P.rank], P, parity, r);
     const uint32_t n = min(__ldcg(s2), P.s2_cap);
     const uint2* pairs = reinterpret_cast<const uint2*>(s2 + 4);             // interleaved (index, value)
-    for (uint32_t i = gtid; i < n; i += gsz) { const uint2 e = __ldcg(pairs + i); P.grad[e.x] = __uint_as_float(e.y); }
+    for (uint32_t i = gtid; i < n; i += gsz) { const uint2 e = __ldcg(pairs + i); put_out<kB>(P, e.x, __uint_as_float(e.y)); }
   }
 }
 
@@ -2130,7 +2207,7 @@ DR_D bool phase_active(const EngineParams& P, int ph) {
   }
 }
 
-template <int kMinBlocks, bool kFull>
+template <int kMinBlocks, bool kFull, bool kB>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const __grid_constant__ EngineParams P) {
   __shared__ Smem sm;
   if (threadIdx.x == 0) {
@@ -2161,12 +2238,12 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
       }
     }
     switch (ph) {
-      case kPhAccum: if (P.use_tma) phase_accum<true, kFull>(P, sm); else phase_accum<false, kFull>(P, sm); break;
+      case kPhAccum: if (P.use_tma) phase_accum<true, kFull, kB>(P, sm); else phase_accum<false, kFull, kB>(P, sm); break;
       case kPhFallback: phase_fallback<kFull>(P, sm); break;
       case kPhHist2: phase_hist2(P, sm); break;
       case kPhInsert: phase_insert(P, sm); break;
       case kPhQuery: phase_query(P, sm); break;
-      case kPhEmit: phase_emit<kFull>(P, sm, bar_epoch); break;
+      case kPhEmit: phase_emit<kFull, kB>(P, sm, bar_epoch); break;
       case kPhRankHist: if constexpr (kFull) phase_rank_hist(P, sm); break;
       case kPhRankScan: if constexpr (kFull) phase_rank_scan(P, sm); break;
       case kPhRankScatter: if constexpr (kFull) phase_rank_scatter(P, sm); break;
@@ -2175,11 +2252,11 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
       case kPhFix: if constexpr (kFull) phase_fix(P, sm); break;
       case kPhExpand: if constexpr (kFull) phase_expand(P, sm); break;
       case kPhPush: phase_push(P, sm); break;
-      case kPhSignal: if (!wait_flags(P, 0u, 0u)) return; break;
+      case kPhSignal: if (!wait_flags<kB>(P, 0u, 0u)) return; break;
       case kPhDecode: phase_decode<kFull>(P, sm); break;
-      case kPhCompact: phase_compact<kFull>(P, sm, bar_epoch); break;
-      case kPhSignal2: if (!wait_flags(P, kArenaFlagWords, 100u)) return; break;
-      case kPhScatter: phase_scatter(P); break;
+      case kPhCompact: phase_compact<kFull, kB>(P, sm, bar_epoch); break;
+      case kPhSignal2: if (!wait_flags<kB>(P, kArenaFlagWords, 100u)) return; break;
+      case kPhScatter: phase_scatter<kB>(P); break;
       default: break;
     }
     if (P.debug_times) {
@@ -2200,19 +2277,26 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
 // filter staging; <2> = 64 regs, two CTAs per SM, up to 88 KB each.
 static bool g_attr_set = false;
 
-// ... x two feature sets: <.., false> index-only (plain pairs / bloom), <.., true> + value codecs, run-length index and
-// the shared 'randomk' index
-static const void* kernel_for(int blocks_per_sm, bool full) {
-  if (blocks_per_sm >= 2) return full ? (const void*)dr_engine_kernel<2, true> : (const void*)dr_engine_kernel<2, false>;
-  return full ? (const void*)dr_engine_kernel<1, true> : (const void*)dr_engine_kernel<1, false>;
+// ... x two feature sets: <.., false, ..> index-only (plain pairs / bloom), <.., true, ..> + value codecs, run-length
+// index and the shared 'randomk' index; ... x the gradient type: <.., .., false> fp32 buckets, <.., .., true> bf16 buckets
+// (a separate instantiation, so the fp32 kernels are compiled from exactly the code they had before bf16 existed)
+static const void* kernel_for(int blocks_per_sm, bool full, bool bf16) {
+  if (bf16) {
+    if (blocks_per_sm >= 2) return full ? (const void*)dr_engine_kernel<2, true, true> : (const void*)dr_engine_kernel<2, false, true>;
+    return full ? (const void*)dr_engine_kernel<1, true, true> : (const void*)dr_engine_kernel<1, false, true>;
+  }
+  if (blocks_per_sm >= 2) return full ? (const void*)dr_engine_kernel<2, true, false> : (const void*)dr_engine_kernel<2, false, false>;
+  return full ? (const void*)dr_engine_kernel<1, true, false> : (const void*)dr_engine_kernel<1, false, false>;
 }
 
 static void ensure_attr() {
   if (!g_attr_set) {
-    cudaFuncSetAttribute(dr_engine_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(dr_engine_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(dr_engine_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
-    cudaFuncSetAttribute(dr_engine_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
+    for (int bf16 = 0; bf16 < 2; ++bf16) {
+      for (int full = 0; full < 2; ++full) {
+        cudaFuncSetAttribute(kernel_for(1, full, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        cudaFuncSetAttribute(kernel_for(2, full, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
+      }
+    }
     g_attr_set = true;
   }
 }
@@ -2222,10 +2306,12 @@ int engine_max_grid(int blocks_per_sm, int dyn_smem_bytes) {
   ensure_attr();
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel_for(blocks_per_sm, true), kThreads, (size_t)dyn_smem_bytes);
-  int occ_plain = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_plain, kernel_for(blocks_per_sm, false), kThreads, (size_t)dyn_smem_bytes);
-  if (occ_plain < occ) occ = occ_plain;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel_for(blocks_per_sm, true, false), kThreads, (size_t)dyn_smem_bytes);
+  for (int v = 1; v < 4; ++v) {                  // the grid must be co-resident whichever variant a bucket launches
+    int o = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kernel_for(blocks_per_sm, v & 1, v >> 1), kThreads, (size_t)dyn_smem_bytes);
+    if (o < occ) occ = o;
+  }
   if (occ < 1) occ = 1;
   if (blocks_per_sm > 0 && blocks_per_sm < occ) occ = blocks_per_sm;
   return occ * sms;
@@ -2240,7 +2326,7 @@ cudaError_t engine_launch(const EngineParams& P, int grid, int blocks_per_sm, in
   void* args[] = {const_cast<EngineParams*>(&P)};
   count_launch(1);
   const bool full = P.n_poly != 0 || P.n_poly_tasks != 0 || P.has_rle != 0 || P.has_shared != 0;
-  return cudaLaunchCooperativeKernel(kernel_for(blocks_per_sm, full), dim3(grid), dim3(kThreads), args,
+  return cudaLaunchCooperativeKernel(kernel_for(blocks_per_sm, full, P.bf16 != 0), dim3(grid), dim3(kThreads), args,
                                      (size_t)dyn_smem_bytes, stream);
 }
 

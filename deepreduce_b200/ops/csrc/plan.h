@@ -211,6 +211,15 @@ struct EngineParams {
   int shard;                     // 1: sharded decode + stage-2 exchange (when world > 1)
   uint32_t s2_words;             // words per stage-2 slot: [count, epoch, 0, 0][idx x cap][val x cap]
   uint32_t s2_cap;               // entries per stage-2 slot
+  // bf16 buckets (bf16 != 0, the <.., .., true> kernels; grad is unused): the dense gradient is bf16 in and out, the
+  // residual, the select, the codecs and the wire stay fp32 (widening is exact), and the aggregate is rounded once
+  // (round-to-nearest-even) where it is final.  The bloom apply adds in fp32 into acc32 first; the warp that finishes a
+  // tile rounds it into grad_bf16.
+  uint16_t* grad_bf16;           // [total elements] bf16 bit patterns
+  float* acc32;                  // [acc_tiles * kTile] apply accumulator, row = tile - first tile this rank decodes; zeroed
+                                 // in the accumulate phase for the bloom tiles that are applied
+  uint32_t acc_tiles;            // rows of acc32 (0: no tensor needs the apply)
+  int bf16;
 };
 
 }  // namespace dr

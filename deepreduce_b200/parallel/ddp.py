@@ -3,7 +3,7 @@ per-tensor ``grc.step(grad, name)`` (SURVEY §7.1).
 
 The reference runs strictly after backward, one Python call and 2-3 NCCL
 all_gathers per tensor (SURVEY §3.2, C1).  Here parameters are laid out in flat
-fp32 buckets (``p.grad`` are views), autograd post-accumulate hooks mark
+fp32 or bf16 buckets, one dtype per bucket (``p.grad`` are views), autograd post-accumulate hooks mark
 buckets ready during backward, and each ready bucket is handed to a C++
 background thread that launches the fused exchange kernel on a high-priority
 side stream; ``finish()`` makes the optimizer's stream wait on the done events.
@@ -81,6 +81,38 @@ def _fused_randomk_supported(params: dict) -> bool:
                           and int(params.get('bucket_size', 512)) == 512)
 
 
+BUCKET_DTYPES = (torch.float32, torch.bfloat16)
+
+
+def group_buckets(named, cap_mb: float) -> list:
+    """Cut the ``(name, parameter)`` list into flat buckets, in reverse order (roughly the order gradients become
+    ready).  A bucket holds one dtype: fp32 parameters and bf16 parameters each fill their own buckets, in the order the
+    dtype first appears, cut at ``cap_mb`` MiB of that dtype.  An all-fp32 list gives the buckets it always gave.
+    Other dtypes raise ``ValueError``."""
+    order = list(reversed(named))
+    dtypes = []
+    for n, p in order:
+        if p.dtype not in BUCKET_DTYPES:
+            raise ValueError(f"parameter {n!r} is {p.dtype}: flat buckets hold fp32 or bf16 gradients")
+        if p.dtype not in dtypes:
+            dtypes.append(p.dtype)
+    buckets = []
+    for dt in dtypes:
+        cap = int(cap_mb * 1024 * 1024 / (4 if dt == torch.float32 else 2))
+        cur, cur_n = [], 0
+        for n, p in order:
+            if p.dtype != dt:
+                continue
+            if cur and cur_n + p.numel() > cap:
+                buckets.append(cur)
+                cur, cur_n = [], 0
+            cur.append((n, p))
+            cur_n += p.numel()
+        if cur:
+            buckets.append(cur)
+    return buckets
+
+
 def fused_path(params: dict) -> bool:
     """True if ``DeepReduceDDP`` on CUDA runs ``params`` through the fused bucket engine."""
     return _fused_supported(params) or _fused_randomk_supported(params)
@@ -153,19 +185,9 @@ class DeepReduceDDP:
 
     # ---- bucket construction ------------------------------------------------
     def _build_buckets(self, cap_mb, blocks_per_sm, use_history):
-        cap = int(cap_mb * 1024 * 1024 / 4)
-        order = list(reversed(self.named))           # roughly the order gradients become ready
-        self.buckets: List[List] = []
-        cur, cur_n = [], 0
-        for n, p in order:
-            if cur and cur_n + p.numel() > cap:
-                self.buckets.append(cur)
-                cur, cur_n = [], 0
-            cur.append((n, p))
-            cur_n += p.numel()
-        if cur:
-            self.buckets.append(cur)
+        self.buckets: List[List] = group_buckets(self.named, cap_mb)
         for b, items in enumerate(self.buckets):
+            dtype = items[0][1].dtype
             numels = [p.numel() for _, p in items]
             names = [n for n, _ in items]
             shapes = [tuple(p.shape) for _, p in items]
@@ -189,7 +211,7 @@ class DeepReduceDDP:
                 eng = BucketEngine(plan, device=self.device, group=self.group,
                                    beta=float(self.params.get('beta', 1.0)) if residual else 0.0,
                                    gamma=float(self.params.get('gamma', 1.0)), average=self.params.get('average', True),
-                                   use_history=use_history, blocks_per_sm=blocks_per_sm)
+                                   use_history=use_history, blocks_per_sm=blocks_per_sm, grad_dtype=dtype)
                 self.engines.append(eng)
                 # re-cut the kernel's tile partitions from measured per-CTA phase times (collective; ~12 exchange steps
                 # on synthetic gradients, state reset afterwards) — 'calibrate_partition': False keeps the static cut
@@ -205,14 +227,13 @@ class DeepReduceDDP:
                 flat, views = eng.grad, eng.grad_views
             else:
                 plan = BucketPlan(numels, names, shapes, index=None)
-                flat = torch.zeros(plan.total_elems, dtype=torch.float32, device=self.device)
+                flat = torch.zeros(plan.total_elems, dtype=dtype, device=self.device)
                 views = plan.views(flat)
             self.flat.append(flat)
             first = {}
             for j, o in enumerate(owner):
                 first.setdefault(o, plan.tensors[j])                # the first chunk of every parameter
             for i, (n, p) in enumerate(items):
-                assert p.dtype == torch.float32, "flat buckets hold fp32 master gradients"
                 t = first[i]
                 seg = flat[t.elem_off:t.elem_off + p.numel()]        # chunks are tile multiples: contiguous
                 # the gradient view mirrors the parameter's own (dense) layout — e.g. channels_last conv
@@ -366,7 +387,7 @@ class DeepReduceDDP:
         if self.fused:
             return sum(e.plan.wire_bytes() for e in self.engines)
         if self.dense:
-            return sum(f.numel() * 4 for f in self.flat)
+            return sum(f.numel() * f.element_size() for f in self.flat)
         return int(self.grc.bytes_sent / max(self.step_count, 1))
 
     def stage2_bytes_per_step(self) -> int:
@@ -379,7 +400,7 @@ class DeepReduceDDP:
         return sum(e.stage2_bytes() for e in self.engines)
 
     def dense_bytes(self) -> int:
-        return sum(p.numel() * 4 for _, p in self.named)
+        return sum(p.numel() * p.element_size() for _, p in self.named)
 
     def exchange_stats(self) -> dict:
         """Device-side counters of the last exchanged step, summed over the buckets (fused path): shipped

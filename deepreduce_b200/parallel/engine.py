@@ -381,10 +381,17 @@ class BucketEngine:
                  seed: int = spec.DEFAULT_SEED, spin_limit: int = 20_000_000, world: Optional[int] = None,
                  rank: Optional[int] = None, filter_smem_bytes: Optional[int] = None, use_tma: bool = True,
                  hist_shift: int = 22, shard: Optional[bool] = None, transport: Optional[str] = None,
-                 peer_timeout_ms: Optional[int] = None, fault: int = 0):
+                 peer_timeout_ms: Optional[int] = None, fault: int = 0, grad_dtype: torch.dtype = torch.float32):
+        # grad_dtype=torch.bfloat16: the flat gradient (in: local, out: aggregate) is bf16.  The residual, the select,
+        # the codecs and the wire stay fp32 (widening bf16 is exact), so the engine computes exactly what an fp32 engine
+        # fed the widened gradient computes, and rounds the aggregate once (to nearest even) where it is final.  The
+        # rounding error is not fed back into the residual, as torch's bf16 DDP does with its reduced sum.
+        if grad_dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"grad_dtype must be torch.float32 or torch.bfloat16 (got {grad_dtype})")
         from .. import ops
         self.mod = ops.cuda_module()
         self.plan = plan
+        self.grad_dtype = grad_dtype
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         self.group = group
         if world is None:
@@ -405,7 +412,7 @@ class BucketEngine:
         dev = self.device
         nT, nt = len(plan.tensors), plan.n_tiles
         with torch.cuda.device(dev):
-            self.grad = torch.zeros(plan.total_elems, dtype=torch.float32, device=dev)
+            self.grad = torch.zeros(plan.total_elems, dtype=grad_dtype, device=dev)
             self.resid = torch.zeros(plan.total_elems, dtype=torch.float32, device=dev)
             self.tensor_table = plan.tensor_table().to(dev)
             self.tile_table = plan.tile_table().to(dev)
@@ -428,7 +435,8 @@ class BucketEngine:
             self._setup_arena()
             self.ctx = self.mod.Engine(
                 self.tensor_table.data_ptr(), self.tile_table.data_ptr(), nT, nt, plan.slot_words, plan.payload_words,
-                self.grad.data_ptr(), self.resid.data_ptr(), self.hist.data_ptr(), self.hist_total.data_ptr(),
+                self.grad.data_ptr() if grad_dtype == torch.float32 else 0, self.resid.data_ptr(), self.hist.data_ptr(),
+                self.hist_total.data_ptr(),
                 self.sel.data_ptr(), self.tile_count.data_ptr(),
                 self.barrier.data_ptr(), self.status.data_ptr(), self.arena_ptrs, self.rank, self.world)
             # equal-COST tile ranges per CTA (DR_BALANCE=0: equal counts)
@@ -441,6 +449,14 @@ class BucketEngine:
             self.cuts = None
             self.ctx.set_scratch(self.pos_mask.data_ptr(), self.dec_mask.data_ptr(), self.cand.data_ptr(),
                                  self.cand_cnt.data_ptr())
+            if grad_dtype == torch.bfloat16:
+                # fp32 sums of the bloom apply (every sender of a tile is added before the one rounding): one 4096-float
+                # row per tile this rank decodes; not needed when every bloom tensor is scattered by emit (W = 1, fp32
+                # values on the wire)
+                applied = any(t.mode == MODE_BLOOM and not (self.world == 1 and t.vmode == 0) for t in plan.tensors)
+                acc_tiles = span_max if applied else 0
+                self.acc32 = torch.zeros(max(acc_tiles, 1) * 4096, dtype=torch.float32, device=dev)
+                self.ctx.set_bf16(self.grad.data_ptr(), self.acc32.data_ptr(), acc_tiles)
             # a peer that does not signal within this wall time is fatal (status 2, output poisoned, see wait_flags)
             if peer_timeout_ms is None:
                 peer_timeout_ms = int(os.environ.get("DR_PEER_TIMEOUT_MS", "120000"))
