@@ -35,7 +35,9 @@ def qsgd_encode_oracle(vals: torch.Tensor, q: int, bucket: int, seed: int):
     prev = level_f.floor()
     idx = torch.arange(nb * bucket, device=v.device)
     u = (spec.policy_hash(idx, seed).double() / 4294967296.0).float().view(nb, bucket)
-    lvl = prev + (u < (level_f - prev)).float()
+    # level_f rounds above q when the norm is |v| itself (a bucket dominated by one value): clamp, so that level
+    # q + 1 never wraps the int8 / int16 wire type
+    lvl = (prev + (u < (level_f - prev)).float()).clamp(max=q)
     lvl = (lvl * vp.sign()).flatten()[:K]
     return lvl, norm
 

@@ -92,6 +92,7 @@ static torch::Tensor qsgd_decode(torch::Tensor lvl, torch::Tensor norms, int64_t
 
 static torch::Tensor pack_bits(torch::Tensor vals, int64_t bits) {
   CHECK_CUDA_T(vals);
+  TORCH_CHECK(1 <= bits && bits <= 63, "pack_bits: bits must be in [1, 63], got ", bits);
   c10::cuda::CUDAGuard g(vals.device());
   auto v = vals.to(torch::kInt64).contiguous();
   const int64_t n = v.numel();
@@ -104,6 +105,7 @@ static torch::Tensor pack_bits(torch::Tensor vals, int64_t bits) {
 
 static torch::Tensor unpack_bits(torch::Tensor buf, int64_t n, int64_t bits) {
   CHECK_CUDA_T(buf);
+  TORCH_CHECK(1 <= bits && bits <= 63, "unpack_bits: bits must be in [1, 63], got ", bits);
   c10::cuda::CUDAGuard g(buf.device());
   const int64_t n_words = (n * bits + 31) / 32;
   auto padded = torch::zeros({n_words * 4}, buf.options().dtype(torch::kUInt8));

@@ -1564,6 +1564,7 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
         const float prev = floorf(lf);
         const float u = (float)((double)policy_hash(p, 0x51EDu + P.epoch) / 4294967296.0);
         float l = prev + ((u < (lf - prev)) ? 1.f : 0.f);
+        l = fminf(l, q);     // lf can round above q when norm == |v|; the residual below follows the clamped level
         l = v > 0.f ? l : (v < 0.f ? -l : 0.f);
         if (sm.td.rank_u32) reinterpret_cast<int16_t*>(my_slot + sm.td.off_rankmap)[p] = (int16_t)l;   // quantum_num >= 128
         else reinterpret_cast<int8_t*>(my_slot + sm.td.off_rankmap)[p] = (int8_t)l;

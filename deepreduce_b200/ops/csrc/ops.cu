@@ -127,6 +127,9 @@ __global__ void __launch_bounds__(256) qsgd_encode_kernel(const float* __restric
     const float prev = floorf(lf);
     const float u = (float)((double)policy_hash((uint32_t)(b0 + i), seed) / 4294967296.0);
     float l = prev + ((u < (lf - prev)) ? 1.f : 0.f);
+    // lf rounds to q(1 + 2^-23) when norm == |x| (a bucket dominated by one value): level q + 1 would wrap the
+    // integer type and flip the sign on the wire
+    l = fminf(l, (float)q);
     l = x > 0.f ? l : (x < 0.f ? -l : 0.f);
     lvl[b0 + i] = (OutT)l;
   }
@@ -164,8 +167,12 @@ __global__ void unpack_bits_kernel(const uint32_t* __restrict__ in, int64_t n_wo
     const int s = (int)(bit0 & 31);
     uint64_t lo = in[w];
     uint64_t hi = (w + 1 < n_words) ? in[w + 1] : 0u;
-    const uint64_t win = lo | (hi << 32);
-    out[i] = (int64_t)((win >> s) & ((1ull << bits) - 1ull));
+    uint64_t v = (lo | (hi << 32)) >> s;
+    if (s + bits > 64) {                              // the value spans three words: its top bits are in in[w + 2]
+      const uint64_t top = (w + 2 < n_words) ? in[w + 2] : 0u;
+      v |= top << (64 - s);
+    }
+    out[i] = (int64_t)(v & ((1ull << bits) - 1ull));
   }
 }
 

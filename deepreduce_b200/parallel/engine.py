@@ -761,9 +761,17 @@ def topk_select_cuda(flat: torch.Tensor, k: int):
         slot = eng.slot()
         n_sel, _, _, n_pos = (int(v) for v in slot[SLOT_HEADER_WORDS:SLOT_HEADER_WORDS + 4].tolist())
         n_sel, n_pos = n_sel & 0xFFFFFFFF, n_pos & 0xFFFFFFFF
-        if n_pos > tp.val_cap:                    # more ties at the 22-bit prefix than the slack: exact fallback
-            idxs = torch.topk(x.abs(), k, sorted=False).indices.sort().values
-            return x[idxs].to(flat.dtype), idxs
+        # the select never takes |x| < 2^-140 (a 22-bit key prefix of 0), so fewer than k selected may still leave
+        # non-zeros out
+        n_nz = int(torch.count_nonzero(x)) if n_sel < k else k
+        if n_pos > tp.val_cap or n_nz > n_sel:    # more ties at the 22-bit prefix than the slack, or tiny non-zeros
+            m = min(k, n_nz)                      # exact fallback: stable sort, so ties still go to the smaller index
+            idxs = torch.sort(x.abs(), descending=True, stable=True).indices[:m].sort().values
+            vals = x[idxs]
+            if m < k:
+                vals = torch.cat([vals, vals.new_zeros(k - m)])
+                idxs = torch.cat([idxs, idxs.new_zeros(k - m)])
+            return vals.to(flat.dtype), idxs
         vals = slot[tp.off_vals:tp.off_vals + n_sel].view(torch.float32).clone()
         idxs = slot[tp.off_idx:tp.off_idx + n_sel].to(torch.int64)
         if n_sel > k:                             # drop the smallest of the prefix class; stable => smaller index wins ties
