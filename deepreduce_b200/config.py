@@ -30,6 +30,7 @@ KNOWN_KEYS = frozenset({
     "policy", "sort", "poly_degree", "quantum_num", "bucket_size", "micro-benchmark", "world_size", "average",
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
+    "p2_pick_mask",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -92,6 +93,15 @@ class DeepReduceConfig:
             world_size=None if g("world_size", None) is None else int(g("world_size")),
             hint=bool(g("hint", True)), min_numel=int(g("min_numel", 1000)))
         cfg.validate()
+        # opt-in wire of the fused engine's conflict_sets policy: the sender ships its pick as a bitmask over the positives
+        p2 = g("p2_pick_mask", False)
+        if not isinstance(p2, bool):
+            raise ConfigError(f"'p2_pick_mask' must be True or False (got {p2!r})")
+        if p2 and not (cfg.compressor == "topk" and cfg.deepreduce in ("index", "both") and cfg.index == "bloom"
+                       and cfg.policy in ("conflict_sets", "p2")):
+            raise ConfigError("'p2_pick_mask' applies to the top-k sparsifier with the bloom index and policy "
+                              f"'conflict_sets' (got compressor={cfg.compressor!r}, deepreduce={cfg.deepreduce!r}, "
+                              f"index={cfg.index!r}, policy={cfg.policy!r})")
         return cfg
 
     def validate(self) -> None:

@@ -447,6 +447,10 @@ struct Engine {
   int blocks_per_sm = 2;
   int dyn_smem = 64 * 1024;
   int device = 0;
+  // P2 ('conflict_sets'): sender-stage scratch (p2_tables of parallel/plan.py); n_p2 == 0: no P2 tensor
+  const dr::P2Entry* p2_entries = nullptr;
+  uint32_t n_p2 = 0, p2_max_pos_cap = 0;
+  uint32_t* p2_scratch = nullptr;
 
   Engine(int64_t tensors, int64_t tiles, int64_t n_tensors, int64_t n_tiles, int64_t slot_words,
          int64_t payload_words, int64_t grad, int64_t resid, int64_t hist, int64_t hist_total, int64_t sel,
@@ -490,6 +494,19 @@ struct Engine {
     P.poly_total = (uint32_t)poly_total;
   }
 
+  void set_p2(int64_t entries, int64_t n, int64_t scratch, int64_t max_pos_cap) {
+    TORCH_CHECK(n == 0 || (entries && scratch), "set_p2: null table or scratch");
+    TORCH_CHECK((size_t)((max_pos_cap + 31) / 32) * 4 <= dr::kP2MaxSmemBytes, "set_p2: pos_cap ", max_pos_cap,
+                " exceeds what the draw holds in shared memory");
+    if (n) {                                     // on the engine's device, from the thread that configures it
+      c10::cuda::CUDAGuard guard((c10::DeviceIndex)device);
+      const cudaError_t e = dr::p2_prepare();
+      TORCH_CHECK(e == cudaSuccess, "set_p2: ", cudaGetErrorString(e));
+    }
+    p2_entries = reinterpret_cast<const dr::P2Entry*>(entries); n_p2 = (uint32_t)n;
+    p2_scratch = reinterpret_cast<uint32_t*>(scratch); p2_max_pos_cap = (uint32_t)max_pos_cap;
+  }
+
   void set_has_rle(int v) { P.has_rle = v; }
   void set_has_shared(int v) { P.has_shared = v; }
   // scratch of the candidate / bitmask pipeline (see engine.cu): masks [n_tiles*128] u32 x2, candidate keys
@@ -529,7 +546,36 @@ struct Engine {
     return grid;
   }
 
+  // The phase range [phase_begin, phase_end) as engine launches; with P2 tensors the range is cut where the P2 kernels
+  // run: the sender stage before emit, the header words after it, and (W > 1) the receiver's thinning of the probed
+  // masks before the apply pass.
   void run_on(uint32_t epoch, int phase_begin, int phase_end, cudaStream_t st) {
+    if (n_p2 == 0) { launch_range(epoch, phase_begin, phase_end, st); return; }
+    const uint32_t parity = epoch & 1u;
+    uint32_t* slots = P.arena[P.rank] + dr::kArenaHdrWords + (size_t)parity * (uint32_t)P.world * P.slot_words;
+    dr::P2Args A{P.tensors, P.tiles, p2_entries, n_p2, p2_scratch, P.pos_mask, P.tile_count,
+                 slots + (size_t)P.rank * P.slot_words, epoch, P.seed};
+    int b = phase_begin;
+    auto upto = [&](int e) { if (b < e) launch_range(epoch, b, e, st); b = e; };
+    auto check = [](cudaError_t e, const char* what) { TORCH_CHECK(e == cudaSuccess, what, ": ", cudaGetErrorString(e)); };
+    if (phase_begin <= dr::kPhEmit && dr::kPhEmit < phase_end) {
+      upto(dr::kPhEmit);
+      check(dr::p2_pick_launch(A, p2_max_pos_cap, st), "P2 pick launch failed");
+      upto(dr::kPhEmit + 1);
+      check(dr::p2_header_launch(A, st), "P2 header launch failed");
+    }
+    if (P.world > 1 && phase_begin <= dr::kPhCompact && dr::kPhCompact < phase_end) {
+      upto(dr::kPhCompact);
+      const bool sh = P.shard && P.world > 1;
+      const uint32_t s_begin = sh ? (uint32_t)(((uint64_t)P.n_tiles * P.rank) / P.world) : 0u;
+      const uint32_t s_end = sh ? (uint32_t)(((uint64_t)P.n_tiles * (P.rank + 1)) / P.world) : P.n_tiles;
+      dr::P2Thin T{P.tensors, P.tiles, slots, P.slot_words, P.dec_mask, P.rank, P.world, s_begin, s_end - s_begin};
+      check(dr::p2_thin_launch(T, st), "P2 thin launch failed");
+    }
+    upto(phase_end);
+  }
+
+  void launch_range(uint32_t epoch, int phase_begin, int phase_end, cudaStream_t st) {
     EngineParams Q = P;
     Q.epoch = epoch; Q.phase_begin = phase_begin; Q.phase_end = phase_end;
     TORCH_CHECK(P.pos_mask && P.cand, "Engine: set_scratch() was not called");
@@ -717,6 +763,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("set_poly", &Engine::set_poly)
       .def("set_shard", &Engine::set_shard)
       .def("set_has_rle", &Engine::set_has_rle)
+      .def("set_p2", &Engine::set_p2)
       .def("set_has_shared", &Engine::set_has_shared)
       .def("set_scratch", &Engine::set_scratch)
       .def("set_peer_timeout_ms", &Engine::set_peer_timeout_ms)

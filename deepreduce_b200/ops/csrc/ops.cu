@@ -3,6 +3,7 @@
 // bit packing, Gram-polynomial fit/eval, delta+bp128 integer coding.
 // Each has a plain-torch oracle in the codec module; tests compare them.
 #include "common.cuh"
+#include "conflict_sets.cuh"
 #include "ops.h"
 
 namespace dr {
@@ -585,15 +586,8 @@ void launch_dexp_fit(const float* y, int64_t K, double* out, cudaStream_t st) {
 
 // ---------------------------------------------------------------------------
 // P2 / conflict sets (paper Alg. 1; reference tensorflow/policies.hpp:43-146 — a host C++ routine upstream, and up to
-// round 1 a device -> host -> device bounce here).  The draw is sequential BY DEFINITION (the r-th pick's random
-// number and every set's "untouched since my last visit" test depend on all earlier picks), so the kernel is one
-// warp that walks the conflict sets in (size, bit position) order:
-//   * the chosen-flags of the positives live in shared memory (one bit per positive, indexed by its rank);
-//   * 32 sets are fetched at a time (offset, size, last-visit count, first 4 member ranks per lane) and then visited
-//     one by one with warp shuffles — no global-memory latency on the sequential path for sets of <= 4 members
-//     (the vast majority: a set is the list of positives hashing to one filter bit);
-//   * a set erases its chosen members implicitly (alive = not chosen), `last` keeps the alive count of the previous
-//     visit, exactly the `cs.size() == before` test of the reference.
+// round 1 a device -> host -> device bounce here): one warp runs the draw of conflict_sets.cuh over the sets in visit
+// order, with the chosen flags of the positives in shared memory.
 // Bit-exact with ops/csrc/cpu/native_cpu.cpp::conflict_sets_impl (tests/test_gpu_engine.py).
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(32) conflict_sets_pick_kernel(const uint32_t* __restrict__ set_off, const uint32_t* __restrict__ members,
@@ -604,74 +598,8 @@ __global__ void __launch_bounds__(32) conflict_sets_pick_kernel(const uint32_t* 
   const uint32_t n_words = (n_pos + 31u) >> 5;
   for (uint32_t i = lane; i < n_words; i += 32u) chosen[i] = 0u;
   __syncwarp();
-  auto is_chosen = [&](uint32_t r) { return (chosen[r >> 5] >> (r & 31u)) & 1u; };
-  uint32_t left = min(K, n_pos), draw = 0;
-  while (left > 0) {
-    bool picked = false;
-    for (uint32_t base = 0; base < n_sets && left > 0; base += 32u) {
-      const uint32_t i = base + lane;
-      const bool valid = i < n_sets;
-      const uint32_t off = valid ? set_off[i] : 0u;
-      const uint32_t sz = valid ? set_off[i + 1] - off : 0u;
-      uint32_t lc = valid ? last[i] : 0u;
-      uint32_t m[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) m[j] = ((uint32_t)j < sz) ? members[off + j] : 0u;
-      const uint32_t n_here = min(32u, n_sets - base);
-      for (uint32_t sidx = 0; sidx < n_here && left > 0; ++sidx) {        // warp-uniform, sequential by definition
-        const uint32_t ssz = __shfl_sync(0xFFFFFFFFu, sz, sidx), soff = __shfl_sync(0xFFFFFFFFu, off, sidx);
-        const uint32_t slc = __shfl_sync(0xFFFFFFFFu, lc, sidx);
-        uint32_t a[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) a[j] = __shfl_sync(0xFFFFFFFFu, m[j], sidx);
-        uint32_t cnt = 0;
-        if (ssz <= 4u) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) cnt += ((uint32_t)j < ssz && !is_chosen(a[j])) ? 1u : 0u;
-        } else {
-          for (uint32_t t = lane; t < ssz; t += 32u) cnt += is_chosen(members[soff + t]) ? 0u : 1u;
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, o);
-        }
-        uint32_t nl = cnt;
-        if (cnt == slc && cnt > 0u) {                                       // untouched since my last visit: draw one member
-          uint32_t r = policy_hash(draw, pseed) % cnt;
-          ++draw;
-          uint32_t pick = 0;
-          if (ssz <= 4u) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              if ((uint32_t)j < ssz && !is_chosen(a[j])) { if (r == 0u) pick = a[j]; --r; }
-            }
-          } else {
-            for (uint32_t t = 0; t < ssz; ++t) {                            // every lane walks the (rare) long set identically
-              const uint32_t x = members[soff + t];
-              if (!is_chosen(x)) { if (r == 0u) { pick = x; break; } --r; }
-            }
-          }
-          __syncwarp();
-          if (lane == 0) chosen[pick >> 5] |= 1u << (pick & 31u);
-          __syncwarp();
-          --left;
-          picked = true;
-          nl = cnt - 1u;
-        }
-        if (lane == sidx) lc = nl;
-      }
-      if (valid) last[i] = lc;
-    }
-    if (!picked && left > 0) {                                               // termination fallback: leftmost unchosen positives
-      for (uint32_t r = 0; r < n_pos && left > 0; ++r) {
-        if (!is_chosen(r)) {
-          __syncwarp();
-          if (lane == 0) chosen[r >> 5] |= 1u << (r & 31u);
-          __syncwarp();
-          --left;
-        }
-      }
-    }
-  }
-  __syncwarp();
+  conflict_sets_draw([&](uint32_t i) { const uint32_t off = set_off[i]; return make_uint2(off, set_off[i + 1] - off); },
+                     [&](uint32_t j) { return members[j]; }, last, n_sets, n_pos, K, pseed, chosen);
   for (uint32_t i = lane; i < n_words; i += 32u) chosen_out[i] = chosen[i];
 }
 

@@ -13,6 +13,38 @@ cudaError_t engine_launch(const EngineParams& P, int grid, int blocks_per_sm, in
 void count_launch(int n);
 long long launch_count();
 
+// p2.cu — the P2 ('conflict_sets') bloom policy of the fused engine, launched between phase ranges of the engine
+struct P2Entry {               // one P2 tensor: its id and word offsets into the scratch buffer (parallel/plan.py p2_tables)
+  uint32_t tensor, pos_idx, set_off, cursor, members, ord, last, tmp, misc, pair_cap;
+};
+struct P2Args {                // sender stage
+  const TensorDesc* tensors;
+  const TileInfo* tiles;
+  const P2Entry* entries;
+  uint32_t n_entries;
+  uint32_t* scratch;
+  uint32_t* pos_mask;          // [n_tiles * 128] my positives (thinned to the pick)
+  uint32_t* tile_count;        // [n_tiles] my positives per tile (thinned to the pick)
+  uint32_t* slot;              // my slot of this step
+  uint32_t epoch, seed;
+};
+struct P2Thin {                // receiver: thin the probed masks of every sender but me
+  const TensorDesc* tensors;
+  const TileInfo* tiles;
+  const uint32_t* slots;       // slot of sender 0 of this step's parity in my arena (senders slot_words apart)
+  uint32_t slot_words;
+  uint32_t* dec_mask;          // [world * span * 128], as the engine's decode lays it out
+  int rank, world;
+  uint32_t s_begin, span;      // the tiles I decode
+};
+constexpr size_t kP2MaxSmemBytes = 128 * 1024;   // the pick's chosen bitmap: up to 2^20 positives (plan.py P2_MAX_POS_CAP)
+// the pick kernel's shared-memory limit, set for the CURRENT device (a function attribute is per device): call it on
+// every device that launches p2_pick_launch, before the first launch
+cudaError_t p2_prepare();
+cudaError_t p2_pick_launch(const P2Args& A, uint32_t max_pos_cap, cudaStream_t st);
+cudaError_t p2_header_launch(const P2Args& A, cudaStream_t st);
+cudaError_t p2_thin_launch(const P2Thin& T, cudaStream_t st);
+
 // ops.cu
 void launch_bloom_insert(const int64_t* idx, int64_t n, uint32_t* filter, uint32_t n_hash, uint32_t m_bits,
                          uint32_t seed, cudaStream_t st);

@@ -28,7 +28,9 @@ enum TensorMode : uint32_t {
                     // only the values travel; off_prefix is sender-local scratch (per-tile exclusive prefix)
 };
 
-enum Policy : int { kPolicyLeftmost = 0, kPolicyRandom = 1, kPolicyP0 = 2 };
+// kPolicyP2 ('conflict_sets', opt-in): the sender draws the pick over its positives and ships it as a bitmask (p2.cu);
+// the engine kernel itself treats it as leftmost on the thinned positives
+enum Policy : int { kPolicyLeftmost = 0, kPolicyRandom = 1, kPolicyP0 = 2, kPolicyP2 = 3 };
 
 // 32 x uint32 per tensor (kDescWords)
 struct TensorDesc {
@@ -61,7 +63,11 @@ struct TensorDesc {
   uint32_t poly_ord;     // ordinal among the vmode==1 tensors (selects its bin table)
   uint32_t fixed_thr;    // != 0: 'threshold' sparsifier — select key >= fixed_thr (31-bit |x| pattern), no radix select, variable K
   uint32_t shared_lb;    // kModeShared: static candidate bound on the hash key (multiple of 512; replaces the history bound)
-  uint32_t reserved[5];
+  // ---- P2 ('conflict_sets') bloom tensors; 0 otherwise ----
+  uint32_t pos_cap;        // the pick runs over the first min(n_pos, pos_cap) positives
+  uint32_t off_pos_prefix; // [n_tiles] positives before each tile, capped at pos_cap
+  uint32_t off_pick;       // [ceil(pos_cap / 32)] pick bitmask: bit q <=> the q-th positive carries a value
+  uint32_t reserved[2];
 };
 static_assert(sizeof(TensorDesc) == 128, "TensorDesc must be 32 words");
 constexpr int kDescWords = 32;

@@ -45,15 +45,20 @@ def _fused_supported(params: dict) -> bool:
     takes the GRACE-compatible per-tensor path, unless ``_fused_randomk_supported`` takes it).  Covers every recipe of
     the reference's launch script (run_deepreduce.sh:35-107): top-k or threshold sparsifier x {no codec, index (bloom
     leftmost / random / p0, run-length), value (polyfit, QSGD int8/int16), both}.
-    Not fused: bloom policy 'conflict_sets' (per-tensor GPU kernel), host codecs (Huffman, Deflate, dexp, the integer
-    family), non-512 QSGD buckets."""
+    Bloom policy 'conflict_sets' (P2) is fused only with top-k and ``'p2_pick_mask': True``: the sender then ships its pick as a
+    bitmask over the positives, a different wire from the reference's, where every receiver redraws the pick.
+    Not fused: 'conflict_sets' without that key (per-tensor GPU kernel), host codecs (Huffman, Deflate, dexp, the
+    integer family), non-512 QSGD buckets."""
     if params.get('compressor') not in ('topk', 'threshold') or params.get('communicator', 'allgather') != 'allgather':
         return False
     dr = params.get('deepreduce', None)
     if dr is None:
         return True
     from ..codecs.bloom import canonical_policy
-    pol_ok = canonical_policy(params.get('policy', 'leftmost')) in ('leftmost', 'random', 'p0')
+    policy = canonical_policy(params.get('policy', 'leftmost'))
+    # P2 needs top-k: under 'threshold' K is the slot capacity, so the draw would keep every positive
+    p2_ok = policy == 'conflict_sets' and params.get('p2_pick_mask') is True and params.get('compressor') == 'topk'
+    pol_ok = policy in ('leftmost', 'random', 'p0') or p2_ok
     value_ok = (params.get('value', 'polyfit') == 'polyfit'
                 or (params.get('value') == 'qsgd' and 1 <= int(params.get('quantum_num', 127)) <= 32767
                     and int(params.get('bucket_size', 512)) == 512))

@@ -31,7 +31,7 @@ import torch
 import torch.distributed as dist
 
 from .. import spec
-from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle
+from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
 from .plan import update_cta_speeds
 from .plan import (ARENA_HDR_WORDS, DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID,
                    SLOT_HEADER_WORDS, BucketPlan, rle_stream_words)
@@ -114,6 +114,29 @@ def random_policy_filter(pos: torch.Tensor, n_ins: int, limit: int, epoch: int, 
     return pos, T
 
 
+def conflict_sets_pick_oracle(tp, pos: torch.Tensor, seed: int, epoch: int):
+    """P2 of the fused engine: the draw over the first ``tp.pos_cap`` positives (ascending), as a bitmask over their
+    ranks.  Returns (picked positives ascending, pick words uint32[ceil(pos_cap / 32)])."""
+    head = pos[:tp.pos_cap]
+    if head.numel():
+        sel = conflict_sets_oracle(head, tp.k, tp.n_hash, tp.m_bits, seed, spec.policy_seed(epoch, tp.salt))
+        sel = sel.to(torch.int64).cpu()
+    else:
+        sel = head
+    bits = np.zeros(((tp.pos_cap + 31) // 32) * 32, dtype=np.uint8)
+    bits[torch.searchsorted(head, sel).numpy()] = 1
+    words = np.packbits(bits.reshape(-1, 32)[:, ::-1], axis=1).view(">u4").astype(np.uint32).reshape(-1)
+    return sel, words
+
+
+def conflict_sets_keep_oracle(tp, pos: torch.Tensor, pick_words: np.ndarray) -> torch.Tensor:
+    """Receiver side of P2: the positives whose rank q is below pos_cap and set in the shipped pick."""
+    head = pos[:tp.pos_cap]
+    q = np.arange(head.numel(), dtype=np.int64)
+    keep = (pick_words.astype(np.int64)[q >> 5] >> (q & 31)) & 1
+    return head[torch.from_numpy(keep.astype(bool))]
+
+
 def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, policy: str, seed: int, epoch: int = 1):
     """Encode one tensor into `slot` (uint32 numpy view); returns new residual."""
     if tp.mode == MODE_SHARED:
@@ -147,11 +170,21 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
             # acceptance threshold travels in header word 2, the receiver repeats the test on its own positives
             # (T now names the acceptance threshold: that is what header word 2 carries for this policy)
             pos, T = random_policy_filter(pos, int(sel_topk.numel()), limit, epoch, tp.salt)
+        if policy == "conflict_sets":
+            # P2: the draw over the first pos_cap positives, shipped as a bitmask over their ranks plus the positives
+            # before every tile (ops/csrc/p2.cu); the receiver keeps exactly the picked positives
+            starts_p = torch.arange(tp.n_tiles, dtype=torch.int64) * spec.TILE
+            slot[tp.off_pos_prefix:tp.off_pos_prefix + tp.n_tiles] = \
+                torch.clamp(torch.searchsorted(pos.cpu(), starts_p), max=tp.pos_cap).numpy().astype(np.uint32)
+            pos, pick = conflict_sets_pick_oracle(tp, pos.cpu(), seed, epoch)
+            slot[tp.off_pick:tp.off_pick + pick.size] = pick
         sel = pos[:limit]
         slot[tp.off_filter:tp.off_filter + tp.n_filter_words] = words.cpu().numpy().view(np.uint32)
         starts = torch.arange(tp.n_tiles, dtype=torch.int64) * spec.TILE
         slot[tp.off_prefix:tp.off_prefix + tp.n_tiles] = torch.searchsorted(sel.cpu(), starts).numpy().astype(np.uint32)
         cutoff = int(sel[-1].item()) if int(pos.numel()) >= limit and limit > 0 else 0xFFFFFFFF
+        if policy == "conflict_sets":
+            cutoff = 0xFFFFFFFF                # the pick says which positives carry values
     elif tp.mode == MODE_RLE:
         n_pos = int(sel_topk.numel())
         limit = tp.val_cap
@@ -277,6 +310,11 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
                 pos = pos[bit.bool()]
             if plan.policy == "random":
                 pos, _ = random_policy_filter(pos, 0, 0, int(a[1]), t.salt, T=int(a[d0 + 2]))
+            if plan.policy == "conflict_sets":
+                starts = torch.arange(t.n_tiles, dtype=torch.int64) * spec.TILE
+                pp = torch.from_numpy(a[t.off_pos_prefix:t.off_pos_prefix + t.n_tiles].astype(np.int64))
+                assert torch.equal(torch.clamp(torch.searchsorted(pos, starts), max=t.pos_cap), pp), t.name
+                pos = conflict_sets_keep_oracle(t, pos, a[t.off_pick:t.off_pick + (t.pos_cap + 31) // 32])
             if cutoff != 0xFFFFFFFF:
                 pos = pos[pos <= cutoff]
             idx = pos[:n_sel]
@@ -335,6 +373,7 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
     threshold of the selection, and the wire bytes by component (static, from the plan)."""
     a = slot.detach().cpu().numpy().view(np.uint32) if torch.is_tensor(slot) else np.asarray(slot, dtype=np.uint32)
     per, tot = [], {"k": 0, "n_sel": 0, "n_pos": 0, "false_pos": 0, "value_bytes": 0, "index_bytes": 0}
+    p2_tot = {"beyond_cap": 0, "tensors_beyond_cap": 0}
     for ti, t in enumerate(plan.tensors):
         d0 = SLOT_HEADER_WORDS + DYN_WORDS * ti
         n_sel, cutoff, thr_bits, n_pos = (int(x) for x in a[d0:d0 + 4])
@@ -347,6 +386,8 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
             vbytes = 4 * t.val_cap
         if t.mode == MODE_BLOOM:
             ibytes = 4 * (t.n_filter_words + t.n_tiles + (4 * t.n_tiles if t.off_hint else 0))
+            if t.pos_cap:                                    # P2: positives per tile + the pick bitmask
+                ibytes += 4 * (t.n_tiles + (t.pos_cap + 31) // 32)
             false_pos = max(0, n_pos - min(t.k, n_pos))      # positives beyond the K inserted (upper bound under 22-bit ties)
         elif t.mode == MODE_RLE:
             ibytes = 4 * ((t.n_tiles + 1) // 2 + rle_stream_words(t.val_cap))
@@ -363,9 +404,15 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
             row["accept_rate"] = 1.0 if thr_bits == 0xFFFFFFFF else thr_bits / 2.0 ** 32
         if t.mode == MODE_SHARED:                            # header word 2 is a hash-key threshold, not a magnitude
             row["threshold"] = None
+        if t.pos_cap:                                        # P2: positives past pos_cap that the draw never saw
+            row["beyond_cap"] = max(0, n_pos - t.pos_cap)
+            p2_tot["beyond_cap"] += row["beyond_cap"]
+            p2_tot["tensors_beyond_cap"] += int(row["beyond_cap"] > 0)
         per.append(row)
         for key in tot:
             tot[key] += row[key]
+    if plan.policy == "conflict_sets":
+        tot.update(p2_tot)
     tot["header_bytes"] = 4 * (SLOT_HEADER_WORDS + DYN_WORDS * len(plan.tensors))
     tot["wire_bytes"] = plan.wire_bytes()
     tot["dense_bytes"] = plan.dense_bytes()
@@ -479,6 +526,12 @@ class BucketEngine:
             if getattr(self, "multicast_ptr", 0):
                 self.ctx.set_multicast(self.multicast_ptr)
             self.ctx.set_has_rle(int(any(t.mode == MODE_RLE for t in plan.tensors)))
+            # P2 ('conflict_sets'): scratch of the sender stage the C++ engine launches before emit (ops/csrc/p2.cu)
+            p2_table, n_p2, p2_words, p2_cap = plan.p2_tables()
+            self.p2_table = p2_table.to(dev)
+            self.p2_scratch = torch.zeros(p2_words, dtype=torch.int32, device=dev)
+            if n_p2:
+                self.ctx.set_p2(self.p2_table.data_ptr(), n_p2, self.p2_scratch.data_ptr(), p2_cap)
             self.ctx.set_has_shared(int(any(t.mode == MODE_SHARED for t in plan.tensors)))
             ids, n_poly, tasks, n_tasks = plan.poly_tables()
             self.poly_ids, self.poly_tasks = ids.to(dev), tasks.to(dev)

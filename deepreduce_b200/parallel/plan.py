@@ -20,7 +20,11 @@ from .. import spec
 
 MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED = 0, 1, 2, 3
 KEY_SPAN = 1 << 31                    # select keys are 31-bit
-POLICY_ID = {"leftmost": 0, "random": 1, "p0": 2}
+POLICY_ID = {"leftmost": 0, "random": 1, "p0": 2, "conflict_sets": 3}
+P2_MAX_POS_CAP = 1 << 20              # P2: the draw keeps one chosen bit per positive in shared memory (128 KB)
+P2_ENTRY_WORDS = 10                   # P2 scratch table entry (ops/csrc/p2.cu P2Entry)
+P2_MAX_HASH = 16                      # P2: filter bits per positive the sender stage holds (p2.cu kMaxHash)
+P2_SIZE_CAP = 32                      # P2: sets of at least this many members are ordered by a separate pass (p2.cu kSizeCap)
 SLOT_HEADER_WORDS = 8
 DYN_WORDS = 4
 ARENA_HDR_WORDS = 128
@@ -149,13 +153,16 @@ class TensorPlan:
     poly_ord: int = 0
     fixed_thr: int = 0        # 'threshold' sparsifier: select |x| bit pattern >= fixed_thr (0: top-k radix select)
     shared_lb: int = 0        # MODE_SHARED: static candidate bound on the hash key (randomk_bound)
+    pos_cap: int = 0          # P2: the pick runs over the first min(n_pos, pos_cap) positives
+    off_pos_prefix: int = 0   # P2: [n_tiles] positives before each tile, capped at pos_cap
+    off_pick: int = 0         # P2: [ceil(pos_cap / 32)] pick bitmask over the positives
 
     def words(self) -> List[int]:
         return [self.elem_off, self.numel, self.k, self.tile_begin, self.n_tiles, self.mode, self.m_bits,
                 self.n_hash, self.off_vals, self.off_filter, self.off_prefix, self.off_idx, self.val_cap,
                 self.salt, self.n_filter_words, self.off_hint, self.vmode, self.off_coef, self.off_rankmap,
                 self.off_selidx, self.off_sorted, self.poly_degree, self.rank_u32, self.poly_off, self.poly_ord,
-                self.fixed_thr, self.shared_lb, 0, 0, 0, 0, 0]
+                self.fixed_thr, self.shared_lb, self.pos_cap, self.off_pos_prefix, self.off_pick, 0, 0]
 
 
 @dataclass
@@ -205,6 +212,9 @@ class BucketPlan:
             # GRACE threshold: |x| > threshold  <=>  key > bits(threshold)  <=>  key >= bits(threshold) + 1
             thr = max(0.0, float(self.threshold))
             fixed_thr = int(np.array([thr], dtype=np.float32).view(np.uint32)[0]) + 1
+        if self.policy == "conflict_sets" and (self.index != "bloom" or self.sparsifier != "topk"):
+            # under 'threshold' K is the slot capacity (default d): the draw would keep every positive, false ones too
+            raise ValueError("the fused 'conflict_sets' policy needs the bloom index and the top-k sparsifier")
         if self.policy not in POLICY_ID:
             raise ValueError(f"fused engine supports policies {list(POLICY_ID)}; got {self.policy!r}")
         names = list(self.names) if self.names is not None else [f"t{i}" for i in range(len(self.numels))]
@@ -243,11 +253,19 @@ class BucketPlan:
                 n_hash, m_bits, n_words = spec.bloom_layout(k, d, self.fpr, self.max_hash)
                 tp.mode = MODE_BLOOM
                 tp.m_bits, tp.n_hash, tp.n_filter_words = m_bits, n_hash, n_words
+                fpr = self.fpr if self.fpr is not None else spec.default_fpr(k, d)
                 if self.policy == "p0":
-                    fpr = self.fpr if self.fpr is not None else spec.default_fpr(k, d)
                     tp.val_cap = min(d, k + int(math.ceil(2.0 * fpr * d)) + 64)
                 else:
                     tp.val_cap = k
+                if self.policy == "conflict_sets":
+                    tp.pos_cap = min(d, k + int(math.ceil(2.0 * fpr * d)) + 64)
+                    if n_hash > P2_MAX_HASH:
+                        raise ValueError(f"conflict_sets: tensor {names[i]!r} has {n_hash} hash functions, more than the "
+                                         f"{P2_MAX_HASH} the fused draw holds per positive; lower 'max_hash' or raise 'fpr'")
+                    if tp.pos_cap > P2_MAX_POS_CAP:
+                        raise ValueError(f"conflict_sets: tensor {names[i]!r} would draw over up to {tp.pos_cap} positives, "
+                                         f"more than the {P2_MAX_POS_CAP} the fused draw holds; split it ('split_numel')")
                 word = self._value_region(tp, word, scratch)
                 tp.off_filter = word
                 word = _align(word + n_words, 4)
@@ -256,6 +274,11 @@ class BucketPlan:
                 if self.hint:
                     tp.off_hint = word
                     word = _align(word + 4 * n_tiles, 4)
+                if tp.pos_cap:
+                    tp.off_pos_prefix = word
+                    word = _align(word + n_tiles, 4)
+                    tp.off_pick = word
+                    word = _align(word + (tp.pos_cap + 31) // 32, 4)
             elif self.index == "rle" and d > self.min_numel:
                 # lossless run coding of the selection bitmap, tile-local: a u16 count per tile and, per selected
                 # element, the zeros+ones run offset from the tile start (< 4096 -> 12 bits), bit-packed
@@ -327,6 +350,30 @@ class BucketPlan:
         ids_t = torch.tensor(ids if ids else [0], dtype=torch.int32)
         tasks_t = torch.tensor(tasks if tasks else [(0, 0)], dtype=torch.int32).reshape(-1)
         return ids_t, len(ids), tasks_t, len(tasks)
+
+    def p2_tables(self):
+        """Scratch of the P2 sender stage (ops/csrc/p2.cu): (int32 table of P2_ENTRY_WORDS per P2 tensor, scratch words,
+        largest pos_cap).  Entry: {tensor, pos_idx, set_off, cursor, members, ord, last, tmp, misc, pair_cap} — word
+        offsets into one int32 buffer.  pos_idx[pos_cap]: element of the q-th positive; set_off[m_bits + 1] / cursor
+        [m_bits]: the counting sort of the (filter bit, positive) pairs; members[pos_cap * n_hash]: set members in bit
+        order; ord / last[min(m_bits, pairs)]: the sets' visit order and the draw's last-visit counts (one entry per
+        non-empty filter bit); tmp: reorder scratch of the sets with >= P2_SIZE_CAP members; misc[4]."""
+        rows, off, cap_max = [], 0, 0
+        for i, t in enumerate(self.tensors):
+            if not t.pos_cap:
+                continue
+            pair_cap = t.pos_cap * t.n_hash
+            n_sets = min(t.m_bits, pair_cap)
+            n_large = min(t.m_bits, pair_cap // P2_SIZE_CAP)
+            row = [i]
+            for n in (t.pos_cap, t.m_bits + 1, t.m_bits, pair_cap, n_sets, n_sets, n_large, 4):
+                row.append(off)
+                off = _align(off + n, 4)
+            row.append(pair_cap)
+            rows.append(row)
+            cap_max = max(cap_max, t.pos_cap)
+        table = torch.tensor(rows if rows else [[0] * P2_ENTRY_WORDS], dtype=torch.int32).reshape(-1)
+        return table, len(rows), max(off, 4), cap_max
 
     # ---- device tables -----------------------------------------------------
     def tensor_table(self) -> torch.Tensor:

@@ -53,6 +53,11 @@ def decode_slot_torch(plan, slot: torch.Tensor, seed: int = spec.DEFAULT_SEED):
                 T = int(hdr[d0 + 2])
                 if T != 0xFFFFFFFF:
                     pos = pos[(spec.policy_hash(pos, spec.policy_seed(int(hdr[1]), t.salt)) <= T).to(pos.device)]
+            if plan.policy == "conflict_sets":             # P2: keep the positives whose rank is set in the shipped pick
+                head = pos[:t.pos_cap]
+                q = torch.arange(head.numel(), device=head.device)
+                pick = slot[t.off_pick:t.off_pick + (t.pos_cap + 31) // 32].to(torch.int64).to(head.device) & 0xFFFFFFFF
+                pos = head[((pick[q >> 5] >> (q & 31)) & 1).bool()]
             if cutoff != 0xFFFFFFFF:
                 pos = pos[pos <= cutoff]
             idx = pos[:n_sel]

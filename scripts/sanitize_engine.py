@@ -20,6 +20,7 @@ CASES = [
     (None, "polyfit", {}, True),
     ("bloom", "qsgd", dict(quantum_num=1000), True),
     ("bloom", None, dict(policy="random", fpr=0.02), True),          # not yet run under the sanitizer
+    ("bloom", None, dict(policy="conflict_sets"), True),             # fused P2 (ops/csrc/p2.cu); not yet run under the sanitizer
 ]
 CASES = CASES[:int(os.environ.get("SAN_CASES", len(CASES)))]
 for index, value, kw, tma in CASES:
