@@ -23,7 +23,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 
-CUDA_SOURCES = ["engine.cu", "ops.cu", "p2p.cu", "bn.cu", "p2.cu"]
+CUDA_SOURCES = ["engine.cu", "ops.cu", "p2p.cu", "bn.cu", "p2.cu", "repack.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--expt-relaxed-constexpr", "--expt-extended-lambda", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 

@@ -10,6 +10,7 @@
 #include <c10/cuda/CUDAStream.h>
 #include <torch/extension.h>
 
+#include <algorithm>
 #include <condition_variable>
 #include <deque>
 #include <mutex>
@@ -247,6 +248,88 @@ static torch::Tensor u8_to_nhwc_norm(torch::Tensor in, std::vector<double> mean,
   check_last("u8_to_nhwc_norm");
   return out;
 }
+
+// ---------------------------------------------------------------------------
+// DDP bucket <-> engine flat buffer (repack.cu)
+// ---------------------------------------------------------------------------
+// One per bucket layout.  Built from a host table of {ddp_off, eng_off, numel} segments, which is checked here once:
+// every segment lies inside both buffers, starts on a 16-byte vector of the engine side, and no two segments overlap
+// on either side.  pack / unpack then only check the buffers (dtype, device, size, alignment) against what the table
+// was checked for, and launch one kernel each.
+struct Repack {
+  torch::Tensor table;          // device, int64 [n_seg + 1][4]
+  int64_t n_seg = 0, n_vec = 0, ddp_numel = 0, eng_numel = 0;
+  int elem_bytes = 0;
+  c10::ScalarType dtype;
+
+  // like: a tensor of the buckets' dtype on their device (the table is uploaded there)
+  Repack(torch::Tensor segs, int64_t ddp_numel_, int64_t eng_numel_, torch::Tensor like)
+      : ddp_numel(ddp_numel_), eng_numel(eng_numel_), dtype(like.scalar_type()) {
+    TORCH_CHECK(dtype == torch::kFloat32 || dtype == torch::kBFloat16, "Repack: fp32 or bf16 buckets, got ", dtype);
+    TORCH_CHECK(like.is_cuda(), "Repack: the buckets must be CUDA tensors");
+    const torch::Device device = like.device();
+    TORCH_CHECK(!segs.is_cuda() && segs.scalar_type() == torch::kInt64 && segs.dim() == 2 && segs.size(1) == 3,
+                "Repack: segments must be a host int64 tensor [n, 3] of {ddp_off, eng_off, numel}");
+    elem_bytes = dtype == torch::kFloat32 ? 4 : 2;
+    const int64_t V = 16 / elem_bytes;
+    segs = segs.contiguous();
+    n_seg = segs.size(0);
+    TORCH_CHECK(n_seg < (1 << 30), "Repack: too many segments");
+    auto host = torch::empty({n_seg + 1, 4}, torch::kInt64);
+    const int64_t* s = segs.data_ptr<int64_t>();
+    int64_t* h = host.data_ptr<int64_t>();
+    std::vector<std::pair<int64_t, int64_t>> ddp_ranges, eng_ranges;
+    for (int64_t i = 0; i < n_seg; ++i) {
+      const int64_t d = s[3 * i], e = s[3 * i + 1], n = s[3 * i + 2];
+      TORCH_CHECK(n > 0, "Repack: segment ", i, " is empty");
+      TORCH_CHECK(d >= 0 && d + n <= ddp_numel, "Repack: segment ", i, " [", d, ", ", d + n,
+                  ") lies outside the DDP buffer of ", ddp_numel, " elements");
+      TORCH_CHECK(e >= 0 && e % V == 0, "Repack: segment ", i, " starts at engine element ", e,
+                  ", not on a 16-byte vector");
+      // full vectors are read / written whole: the last one must still lie inside the engine buffer
+      TORCH_CHECK((e + n + V - 1) / V * V <= eng_numel, "Repack: segment ", i, " [", e, ", ", e + n,
+                  ") lies outside the engine buffer of ", eng_numel, " elements");
+      h[4 * i] = d; h[4 * i + 1] = e; h[4 * i + 2] = n; h[4 * i + 3] = n_vec;
+      n_vec += (n + V - 1) / V;
+      ddp_ranges.emplace_back(d, d + n);
+      eng_ranges.emplace_back(e, e + n);
+    }
+    h[4 * n_seg] = 0; h[4 * n_seg + 1] = 0; h[4 * n_seg + 2] = 0; h[4 * n_seg + 3] = n_vec;
+    for (auto* r : {&ddp_ranges, &eng_ranges}) {
+      std::sort(r->begin(), r->end());
+      for (size_t i = 1; i < r->size(); ++i)
+        TORCH_CHECK((*r)[i].first >= (*r)[i - 1].second, "Repack: segments overlap at element ", (*r)[i].first);
+    }
+    table = host.to(device);
+  }
+
+  void check_buffers(const torch::Tensor& ddp, const torch::Tensor& eng) const {
+    for (const torch::Tensor* t : {&ddp, &eng}) {
+      TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->dim() == 1, "Repack: buffers are contiguous 1-D CUDA tensors");
+      TORCH_CHECK(t->scalar_type() == dtype, "Repack: the table was built for ", dtype, " buffers, got ", t->scalar_type());
+      TORCH_CHECK(t->device() == table.device(), "Repack: buffer on ", t->device(), ", table on ", table.device());
+    }
+    TORCH_CHECK(ddp.numel() >= ddp_numel, "Repack: the DDP buffer has ", ddp.numel(), " elements, the table needs ", ddp_numel);
+    TORCH_CHECK(eng.numel() >= eng_numel, "Repack: the engine buffer has ", eng.numel(), " elements, the table needs ", eng_numel);
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(eng.data_ptr()) % 16 == 0, "Repack: the engine buffer must be 16-byte aligned");
+  }
+
+  void pack(torch::Tensor ddp, torch::Tensor eng) const {
+    check_buffers(ddp, eng);
+    c10::cuda::CUDAGuard g(eng.device());
+    cudaError_t e = dr::launch_bucket_repack(true, elem_bytes, ddp.data_ptr(), eng.data_ptr(), table.data_ptr<int64_t>(),
+                                             (int)n_seg, n_vec, cur_stream());
+    TORCH_CHECK(e == cudaSuccess, "bucket_pack: ", cudaGetErrorString(e));
+  }
+
+  void unpack(torch::Tensor eng, torch::Tensor ddp) const {
+    check_buffers(ddp, eng);
+    c10::cuda::CUDAGuard g(eng.device());
+    cudaError_t e = dr::launch_bucket_repack(false, elem_bytes, eng.data_ptr(), ddp.data_ptr(), table.data_ptr<int64_t>(),
+                                             (int)n_seg, n_vec, cur_stream());
+    TORCH_CHECK(e == cudaSuccess, "bucket_unpack: ", cudaGetErrorString(e));
+  }
+};
 
 // ---------------------------------------------------------------------------
 // training BatchNorm (+ ReLU, + residual add) on channels_last bf16 (bn.cu)
@@ -747,6 +830,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("arena_close", [](int64_t p) { dr::arena_close((void*)p); });
   m.def("arena_as_tensor", &arena_as_tensor);
   m.def("enable_peer_access", [](std::vector<int> devices) { return dr::arena_enable_peer_access(devices.data(), (int)devices.size()); });
+  py::class_<Repack>(m, "Repack")
+      .def(py::init<torch::Tensor, int64_t, int64_t, torch::Tensor>(), py::arg("segments"), py::arg("ddp_numel"),
+           py::arg("eng_numel"), py::arg("like"))
+      .def("pack", &Repack::pack, py::arg("ddp"), py::arg("eng"))
+      .def("unpack", &Repack::unpack, py::arg("eng"), py::arg("ddp"))
+      .def_readonly("table", &Repack::table)
+      .def_readonly("n_seg", &Repack::n_seg)
+      .def_readonly("n_vec", &Repack::n_vec);
   m.attr("TILE") = dr::kTile;
   m.attr("ARENA_HDR_WORDS") = dr::kArenaHdrWords;
   m.attr("SLOT_HEADER_WORDS") = dr::kSlotHeaderWords;

@@ -75,6 +75,12 @@ void launch_rle_runs(const int64_t* idx, int64_t n, const uint32_t* excl, int64_
 void launch_rle_expand(const int64_t* ones_excl, const int64_t* run_start, int64_t n_runs, int64_t total, int64_t* out,
                        cudaStream_t st);
 
+// repack.cu — DDP gradient bucket <-> engine flat buffer.  table: int64 [n_seg + 1][4] on the device, row s =
+// {ddp_off, eng_off, numel, vec_begin} (elements; vec_begin counts 16-byte engine-side vectors), row n_seg =
+// {0, 0, 0, n_vec}.  pack: src = DDP buffer, dst = engine buffer; unpack: the other way.  elem_bytes: 4 or 2.
+cudaError_t launch_bucket_repack(bool pack, int elem_bytes, const void* src, void* dst, const int64_t* table, int n_seg,
+                                 int64_t n_vec, cudaStream_t st);
+
 // p2p.cu — symmetric arena over CUDA IPC
 struct ArenaHandle { unsigned char bytes[64]; };
 void* arena_alloc(size_t bytes);                       // cudaMalloc + zero

@@ -144,6 +144,42 @@ def plan_kwargs_from_params(params: dict) -> dict:
     return kw
 
 
+def engine_split_numel(params: dict, blocks_per_sm: int) -> int:
+    """Chunk size of the fused plan for ``params``: tensors whose bloom filter would not fit the kernel's SMEM staging
+    buffer enter the plan as tile-aligned chunks with their own top-k / filter ('split_numel': 'auto', the default; an
+    int pins the chunk size, 0 / None keeps every tensor whole and lets oversize filters be probed from L2)."""
+    sn = params.get('split_numel', 'auto')
+    if sn == 'auto':
+        uses_bloom = params.get('deepreduce') in ('index', 'both') and params.get('index', 'bloom') == 'bloom'
+        from .plan import auto_split_numel
+        sn = auto_split_numel(params.get('compress_ratio', 0.01), params.get('fpr', None),
+                              (160 if blocks_per_sm < 2 else 80) * 1024) if uses_bloom and params.get('compressor') == 'topk' else 0
+    return int(sn or 0)
+
+
+def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: bool, blocks_per_sm: int,
+                grad_dtype: torch.dtype) -> BucketEngine:
+    """The ``BucketEngine`` of one bucket for ``params`` (residual memory, beta / gamma, averaging), with its tile
+    partitions calibrated unless ``'calibrate_partition': False``.  Collective at W > 1."""
+    residual = params.get('memory', 'none') == 'residual'
+    eng = BucketEngine(plan, device=device, group=group,
+                       beta=float(params.get('beta', 1.0)) if residual else 0.0,
+                       gamma=float(params.get('gamma', 1.0)), average=params.get('average', True),
+                       use_history=use_history, blocks_per_sm=blocks_per_sm, grad_dtype=grad_dtype)
+    # re-cut the kernel's tile partitions from measured per-CTA phase times (collective; ~12 exchange steps
+    # on synthetic gradients, state reset afterwards) — 'calibrate_partition': False keeps the static cut
+    if params.get('calibrate_partition', True) and eng.cuts is not None:
+        try:
+            eng.calibrate_partition()
+        except (ValueError, ArithmeticError, IndexError) as e:      # host-side arithmetic only: the static
+            import warnings                                      # per-phase cut is a complete fallback
+            warnings.warn(f"deepreduce_b200: partition calibration skipped ({e!r}); using the static cut")
+            eng.cta_speeds = None
+            eng._set_cuts()
+            eng.resid.zero_(); eng.sel.zero_(); eng.grad.zero_()
+    return eng
+
+
 class DeepReduceDDP:
     def __init__(self, module: nn.Module, params: dict, *, bucket_cap_mb: float = 1e9, overlap: bool = True,
                  group=None, blocks_per_sm: int = 2, use_history: bool = True, background_thread: bool = True,
@@ -198,37 +234,15 @@ class DeepReduceDDP:
             shapes = [tuple(p.shape) for _, p in items]
             owner = list(range(len(items)))
             if self.fused:
-                # tensors whose bloom filter would not fit the kernel's SMEM staging buffer enter the plan as tile-aligned
-                # chunks with their own top-k / filter ('split_numel': 'auto', the default; an int pins the chunk size,
-                # 0 / None keeps every tensor whole and lets oversize filters be probed from L2)
-                sn = self.params.get('split_numel', 'auto')
-                if sn == 'auto':
-                    uses_bloom = self.params.get('deepreduce') in ('index', 'both') and self.params.get('index', 'bloom') == 'bloom'
-                    from .plan import auto_split_numel
-                    sn = auto_split_numel(self.params.get('compress_ratio', 0.01), self.params.get('fpr', None),
-                                          (160 if blocks_per_sm < 2 else 80) * 1024) if uses_bloom and self.params.get('compressor') == 'topk' else 0
+                sn = engine_split_numel(self.params, blocks_per_sm)
                 if sn:
                     from .plan import split_large
                     numels, names, shapes, owner = split_large(numels, names, shapes, int(sn))
             if self.fused:
                 plan = BucketPlan(numels, names, shapes, **plan_kwargs_from_params(self.params))
-                residual = self.params.get('memory', 'none') == 'residual'
-                eng = BucketEngine(plan, device=self.device, group=self.group,
-                                   beta=float(self.params.get('beta', 1.0)) if residual else 0.0,
-                                   gamma=float(self.params.get('gamma', 1.0)), average=self.params.get('average', True),
-                                   use_history=use_history, blocks_per_sm=blocks_per_sm, grad_dtype=dtype)
+                eng = make_engine(plan, self.params, device=self.device, group=self.group, use_history=use_history,
+                                  blocks_per_sm=blocks_per_sm, grad_dtype=dtype)
                 self.engines.append(eng)
-                # re-cut the kernel's tile partitions from measured per-CTA phase times (collective; ~12 exchange steps
-                # on synthetic gradients, state reset afterwards) — 'calibrate_partition': False keeps the static cut
-                if self.params.get('calibrate_partition', True) and eng.cuts is not None:
-                    try:
-                        eng.calibrate_partition()
-                    except (ValueError, ArithmeticError, IndexError) as e:      # host-side arithmetic only: the static
-                        import warnings                                      # per-phase cut is a complete fallback
-                        warnings.warn(f"deepreduce_b200: partition calibration skipped ({e!r}); using the static cut")
-                        eng.cta_speeds = None
-                        eng._set_cuts()
-                        eng.resid.zero_(); eng.sel.zero_(); eng.grad.zero_()
                 flat, views = eng.grad, eng.grad_views
             else:
                 plan = BucketPlan(numels, names, shapes, index=None)
