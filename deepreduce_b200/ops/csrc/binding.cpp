@@ -635,9 +635,9 @@ struct Engine {
   void run_on(uint32_t epoch, int phase_begin, int phase_end, cudaStream_t st) {
     if (n_p2 == 0) { launch_range(epoch, phase_begin, phase_end, st); return; }
     const uint32_t parity = epoch & 1u;
-    uint32_t* slots = P.arena[P.rank] + dr::kArenaHdrWords + (size_t)parity * (uint32_t)P.world * P.slot_words;
+    uint32_t* slots = P.arena[P.rank] + dr::slot_offset(P, parity, 0);
     dr::P2Args A{P.tensors, P.tiles, p2_entries, n_p2, p2_scratch, P.pos_mask, P.tile_count,
-                 slots + (size_t)P.rank * P.slot_words, epoch, P.seed};
+                 P.arena[P.rank] + dr::slot_offset(P, parity, P.rank), epoch, P.seed};
     int b = phase_begin;
     auto upto = [&](int e) { if (b < e) launch_range(epoch, b, e, st); b = e; };
     auto check = [](cudaError_t e, const char* what) { TORCH_CHECK(e == cudaSuccess, what, ": ", cudaGetErrorString(e)); };
@@ -649,9 +649,8 @@ struct Engine {
     }
     if (P.world > 1 && phase_begin <= dr::kPhCompact && dr::kPhCompact < phase_end) {
       upto(dr::kPhCompact);
-      const bool sh = P.shard && P.world > 1;
-      const uint32_t s_begin = sh ? (uint32_t)(((uint64_t)P.n_tiles * P.rank) / P.world) : 0u;
-      const uint32_t s_end = sh ? (uint32_t)(((uint64_t)P.n_tiles * (P.rank + 1)) / P.world) : P.n_tiles;
+      uint32_t s_begin, s_end;
+      dr::decode_span(P, P.rank, s_begin, s_end);
       dr::P2Thin T{P.tensors, P.tiles, slots, P.slot_words, P.dec_mask, P.rank, P.world, s_begin, s_end - s_begin};
       check(dr::p2_thin_launch(T, st), "P2 thin launch failed");
     }
@@ -662,10 +661,10 @@ struct Engine {
     EngineParams Q = P;
     Q.epoch = epoch; Q.phase_begin = phase_begin; Q.phase_end = phase_end;
     TORCH_CHECK(P.pos_mask && P.cand, "Engine: set_scratch() was not called");
-    if (P.bf16 && P.acc_tiles) {                 // one acc32 row per tile of the span engine.cu decode_span gives this rank
-      const uint32_t span = (P.shard && P.world > 1)
-          ? (uint32_t)(((uint64_t)P.n_tiles * (P.rank + 1)) / P.world - ((uint64_t)P.n_tiles * P.rank) / P.world)
-          : P.n_tiles;
+    if (P.bf16 && P.acc_tiles) {                 // one acc32 row per tile this rank decodes
+      uint32_t s_begin, s_end;
+      dr::decode_span(P, P.rank, s_begin, s_end);
+      const uint32_t span = s_end - s_begin;
       TORCH_CHECK(P.acc_tiles >= span, "Engine: the bf16 accumulator covers ", P.acc_tiles, " tiles, the decode span ", span);
     }
     int g = get_grid();

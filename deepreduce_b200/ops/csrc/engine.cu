@@ -31,6 +31,7 @@
 // full/empty ring + warp-private work, probe chains run on dense survivor batches.
 #include "common.cuh"
 #include "plan.h"
+#include "tiles.cuh"
 
 #include <cuda_bf16.h>
 
@@ -60,8 +61,6 @@ namespace {
 
 constexpr uint32_t kErrPeerWait = 2u, kErrResolve = 3u, kErrS2Overflow = 6u, kErrDisagree = 7u;
 constexpr uint32_t kNoTensor = 0xFFFFFFFFu;
-constexpr uint32_t kFullMask = 0xFFFFFFFFu;
-constexpr uint32_t kGroupsPerTile = kTile / 32;       // 128 mask words per tile
 constexpr uint32_t kChunk = 256;                      // candidate capacity per (tile, warp) = the elements a warp owns
 constexpr uint32_t kHalf = kTile / 2;                 // elements per ring stage (g half-tile | r half-tile)
 constexpr uint32_t kStageBytes = 2u * kHalf * 4u;     // 16 KB
@@ -98,22 +97,11 @@ struct Smem {
 extern __shared__ __align__(16) uint32_t g_filter_smem[];   // dynamic: staged bloom filter / TMA ring / stage-2 staging
 
 DR_D uint32_t* slot_ptr(uint32_t* arena, const EngineParams& P, uint32_t parity, int src) {
-  return arena + kArenaHdrWords + (size_t)(parity * (uint32_t)P.world + (uint32_t)src) * P.slot_words;
+  return arena + slot_offset(P, parity, src);
 }
 
 DR_D uint32_t* s2_ptr(uint32_t* arena, const EngineParams& P, uint32_t parity, int src) {
-  return arena + kArenaHdrWords + (size_t)2 * (uint32_t)P.world * P.slot_words +
-         (size_t)(parity * (uint32_t)P.world + (uint32_t)src) * P.s2_words;
-}
-
-DR_D bool sharded(const EngineParams& P) { return P.shard && P.world > 1; }
-
-// tiles this rank decodes: everything (W == 1 / unsharded) or its 1/W slice
-DR_D void decode_span(const EngineParams& P, int owner, uint32_t& s_begin, uint32_t& s_end) {
-  if (sharded(P)) {
-    s_begin = (uint32_t)(((uint64_t)P.n_tiles * (uint32_t)owner) / (uint32_t)P.world);
-    s_end = (uint32_t)(((uint64_t)P.n_tiles * ((uint32_t)owner + 1u)) / (uint32_t)P.world);
-  } else { s_begin = 0; s_end = P.n_tiles; }
+  return arena + s2_offset(P, parity, src);
 }
 
 // this CTA's contiguous share of the decode span (decode and compact use the SAME split, so the CTA that decoded
@@ -145,14 +133,6 @@ DR_D bool bloom_applied(const EngineParams& P, uint32_t mode, uint32_t vmode) {
   return mode == (uint32_t)kModeBloom && !(P.world == 1 && vmode == 0u);
 }
 
-struct Tile { uint32_t tensor, base, n, local0, single; };   // `single`: the tensor has exactly one tile
-
-DR_D Tile load_tile(const EngineParams& P, uint32_t tile) {
-  const uint4 q = __ldg(reinterpret_cast<const uint4*>(P.tiles) + tile);
-  Tile t; t.tensor = q.x; t.base = q.y; t.n = q.z & 0xFFFFu; t.local0 = q.w; t.single = q.z >> 31;
-  return t;
-}
-
 DR_D void load_tensor(const EngineParams& P, uint32_t t, Smem& sm) {
   __syncthreads();
   if (threadIdx.x < kDescWords) {
@@ -163,15 +143,6 @@ DR_D void load_tensor(const EngineParams& P, uint32_t t, Smem& sm) {
 }
 
 DR_D size_t chunk_of(uint32_t tile, uint32_t warp) { return ((size_t)tile * kWarps + warp) * kChunk; }
-
-DR_D uint32_t warp_incl_scan(uint32_t v, uint32_t lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t n = __shfl_up_sync(kFullMask, v, o);
-    if (lane >= (uint32_t)o) v += n;
-  }
-  return v;
-}
 
 // ---------------------------------------------------------------------------
 // radix-select digit resolve: find the bin holding the k-th largest key.
@@ -219,14 +190,29 @@ DR_D void clear_hist(Smem& sm) {
   __syncthreads();
 }
 
-DR_D void flush_hist(uint32_t* __restrict__ gh, Smem& sm) {
+// Merge this CTA's SMEM histogram of tensor t into the global one `gh` (kBins == 2 * kHistBins: the speculative digit-2
+// half that follows it in SMEM goes to `gh2`), zeroing the SMEM bins, and take the tensor's ticket of histogram
+// `which`.  Returns true (CTA-uniform) in the CTA whose merge completes the tensor (ticket count == n_tiles).
+template <int kBins>
+DR_D bool merge_ticket(const EngineParams& P, Smem& sm, int which, uint32_t t, uint32_t* __restrict__ gh,
+                       uint32_t* __restrict__ gh2, uint32_t n_mine, uint32_t n_tiles) {
   __syncthreads();
-  for (int j = threadIdx.x; j < kHistBins; j += kThreads) {
+  for (int j = threadIdx.x; j < kBins; j += kThreads) {
     const uint32_t v = sm.u.hist[j];
-    if (v) { atomicAdd(gh + j, v); sm.u.hist[j] = 0; }
+    if (v) { atomicAdd((j < kHistBins ? gh : gh2 - kHistBins) + j, v); sm.u.hist[j] = 0; }
   }
   __threadfence();                              // merged counts are visible before the ticket is taken
   __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const uint32_t before = atomicAdd(P.hist_total + (size_t)which * P.n_tensors + t, n_mine);
+    sm.s.lb = (before + n_mine == n_tiles) ? 1u : 0u;
+    __threadfence();
+  }
+  __syncthreads();
+  const bool last = sm.s.lb != 0u;
+  __syncthreads();
+  return last;
 }
 
 // Finish one digit of one tensor for this CTA.  If the CTA owns every tile of the tensor the digit is
@@ -242,16 +228,7 @@ DR_D bool finish_digit(const EngineParams& P, Smem& sm, int which, uint32_t t, u
     return true;
   }
   uint32_t* gh = hist_ptr(P, which, t);
-  flush_hist(gh, sm);
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const uint32_t before = atomicAdd(P.hist_total + (size_t)which * P.n_tensors + t, n_mine);
-    sm.s.lb = (before + n_mine == n_tiles) ? 1u : 0u;
-    __threadfence();
-  }
-  __syncthreads();
-  const bool last = sm.s.lb != 0u;
-  __syncthreads();
+  const bool last = merge_ticket<kHistBins>(P, sm, which, t, gh, nullptr, n_mine, n_tiles);
   if (last) resolve_bins([&](int b) { return __ldcg(gh + b); }, kHistBins, k, sm.s);
   return last;
 }
@@ -327,6 +304,20 @@ DR_D void write_final(const EngineParams& P, Smem& sm, uint32_t t, uint32_t bin1
   }
 }
 
+// Digit 2 of a one-tile tensor, from this thread's 8 keys still in registers (0xFFFFFFFF: not an element), once digit 1
+// resolved to (bin1, krem1) and the SMEM histogram is clear.  An unsafe bin1 is the caller's to handle.
+DR_D void finish_single(const EngineParams& P, Smem& sm, uint32_t t, const uint32_t (&keys)[8], uint32_t bin1,
+                        uint32_t krem1) {
+  if (bin1 == kUnsafe) return;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    if (keys[i] != 0xFFFFFFFFu && (keys[i] >> 20) == bin1) atomicAdd(&sm.u.hist[(keys[i] >> 9) & 0x7FFu], 1u);
+  resolve_bins([&](int b) { return sm.u.hist[b]; }, kHistBins, krem1, sm.s);
+  write_final(P, sm, t, bin1);
+  if (threadIdx.x == 0) P.sel[t].done_epoch = P.epoch;
+  clear_hist(sm);
+}
+
 // Digit 1 AND (speculatively) digit 2 of a multi-tile tensor at the end of the accumulate phase.  Every CTA also
 // binned digit 2 of its candidates under the guess that the threshold bin is last step's (`guess`).  The CTA that
 // completes the tensor resolves digit 1; if the guess was right it resolves digit 2 on the spot and the tensor needs
@@ -338,26 +329,7 @@ DR_D void finish_spec(const EngineParams& P, Smem& sm, uint32_t t, uint32_t n_mi
   uint32_t* gh1 = hist_ptr(P, 0, t);
   uint32_t* gh2 = hist_ptr(P, 2, t);
   const bool whole = (n_mine == n_tiles);                 // this CTA saw every tile: resolve from shared memory
-  bool last = whole;
-  if (!whole) {
-    __syncthreads();
-    for (int j = tid; j < 2 * kHistBins; j += kThreads) {
-      const uint32_t v = sm.u.hist[j];
-      if (v) { atomicAdd((j < kHistBins ? gh1 : gh2 - kHistBins) + j, v); sm.u.hist[j] = 0; }
-    }
-    __threadfence();                                      // merged counts are visible before the ticket is taken
-    __syncthreads();
-    if (tid == 0) {
-      __threadfence();
-      const uint32_t before = atomicAdd(P.hist_total + t, n_mine);
-      sm.s.lb = (before + n_mine == n_tiles) ? 1u : 0u;
-      __threadfence();
-    }
-    __syncthreads();
-    last = sm.s.lb != 0u;
-    __syncthreads();
-  }
-  if (!last) return;
+  if (!whole && !merge_ticket<2 * kHistBins>(P, sm, 0, t, gh1, gh2, n_mine, n_tiles)) return;
   if (whole) resolve_bins([&](int b) { return sm.u.hist[b]; }, kHistBins, k, sm.s);
   else resolve_bins([&](int b) { return __ldcg(gh1 + b); }, kHistBins, k, sm.s);
   const uint32_t bin1 = sm.s.res[0], krem1 = sm.s.res[1];
@@ -456,7 +428,7 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   uint32_t p_tile = t0, p_half = 0, p_stage = 0;
   auto issue_next = [&]() -> bool {
     while (p_tile < t_end) {
-      const Tile t = load_tile(P, p_tile);
+      const Tile t = load_tile(P.tiles, p_tile);
       const uint32_t off = p_half * kHalf;
       if (p_half == 1u) { p_half = 0; ++p_tile; } else { p_half = 1u; }
       if (off < t.n) {
@@ -498,7 +470,7 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
   const float beta = P.beta, gamma = P.gamma;
   while (tile < t_end) {
-    Tile ti = load_tile(P, tile);
+    Tile ti = load_tile(P.tiles, tile);
     const uint32_t cur = ti.tensor;
     const TensorDesc* tdp = P.tensors + cur;
     const uint32_t mode = __ldg(&tdp->mode), fixed = __ldg(&tdp->fixed_thr);
@@ -605,7 +577,7 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
       n_mine += 1;
       ++tile;
       if (tile >= t_end) break;
-      const Tile tn = load_tile(P, tile);
+      const Tile tn = load_tile(P.tiles, tile);
       if (tn.tensor != cur) break;
       ti = tn;
     }
@@ -622,15 +594,7 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
       const uint32_t bin1 = sm.s.res[0], krem1 = sm.s.res[1];
       write_digit1(P, sm, cur);
       clear_hist(sm);
-      if (bin1 != kUnsafe) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if (keys[i] != 0xFFFFFFFFu && (keys[i] >> 20) == bin1) atomicAdd(&sm.u.hist[(keys[i] >> 9) & 0x7FFu], 1u);
-        resolve_bins([&](int b) { return sm.u.hist[b]; }, kHistBins, krem1, sm.s);
-        write_final(P, sm, cur, bin1);
-        if (tid == 0) P.sel[cur].done_epoch = P.epoch;
-        clear_hist(sm);
-      }
+      finish_single(P, sm, cur, keys, bin1, krem1);
     } else {
       finish_spec(P, sm, cur, n_mine, __ldg(&tdp->n_tiles), __ldg(&tdp->k), guess);
     }
@@ -648,7 +612,7 @@ DR_D void phase_fallback(const EngineParams& P, Smem& sm) {
   uint32_t tile, t_end;
   tile_range(P, kPartAccum, tile, t_end);
   while (tile < t_end) {
-    const Tile t0 = load_tile(P, tile);
+    const Tile t0 = load_tile(P.tiles, tile);
     const uint32_t cur = t0.tensor;
     const TensorDesc* tdp = P.tensors + cur;
     const uint32_t seg_end = min(t_end, __ldg(&tdp->tile_begin) + __ldg(&tdp->n_tiles));
@@ -660,7 +624,7 @@ DR_D void phase_fallback(const EngineParams& P, Smem& sm) {
     const uint32_t hseed = shared ? policy_seed(P.epoch, __ldg(&tdp->salt)) : 0u;
     uint32_t keys[8];
     for (uint32_t tl = tile; tl < seg_end; ++tl) {
-      const Tile ti = load_tile(P, tl);
+      const Tile ti = load_tile(P.tiles, tl);
       uint32_t cnt = 0;
       uint2* chunk = P.cand + chunk_of(tl, warp);
 #pragma unroll
@@ -695,15 +659,7 @@ DR_D void phase_fallback(const EngineParams& P, Smem& sm) {
         P.sel[cur].bin1 = bin1; P.sel[cur].krem1 = krem1;
       }
       clear_hist(sm);
-      if (bin1 != kUnsafe) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if (keys[i] != 0xFFFFFFFFu && (keys[i] >> 20) == bin1) atomicAdd(&sm.u.hist[(keys[i] >> 9) & 0x7FFu], 1u);
-        resolve_bins([&](int b) { return sm.u.hist[b]; }, kHistBins, krem1, sm.s);
-        write_final(P, sm, cur, bin1);
-        if (tid == 0) P.sel[cur].done_epoch = P.epoch;
-        clear_hist(sm);
-      }
+      finish_single(P, sm, cur, keys, bin1, krem1);
     } else if (finish_digit(P, sm, 1, cur, seg_end - tile, nt, k)) {
       if (tid == 0) {
         if (sm.s.res[0] == kUnsafe) atomicExch(P.status, kErrResolve);
@@ -717,8 +673,6 @@ DR_D void phase_fallback(const EngineParams& P, Smem& sm) {
 // ===========================================================================
 // kModeRle helpers: 12-bit fields, LSB-first, entry j at bit 12*j of the stream
 // ===========================================================================
-DR_D uint32_t rle_stream_words(uint32_t val_cap) { return (val_cap * 12u + 31u) / 32u + 1u; }
-
 DR_D void rle_put(uint32_t* stream, uint32_t j, uint32_t pos) {
   const uint32_t bit = 12u * j, w = bit >> 5, sh = bit & 31u;
   atomicOr(stream + w, pos << sh);
@@ -773,7 +727,7 @@ DR_D void phase_hist2(const EngineParams& P, Smem& sm) {
   uint32_t tile, t_end;
   tile_range(P, kPartAccum, tile, t_end);
   while (tile < t_end) {
-    const Tile t0 = load_tile(P, tile);
+    const Tile t0 = load_tile(P.tiles, tile);
     const uint32_t cur = t0.tensor;
     const TensorDesc* tdp = P.tensors + cur;
     const uint32_t nt = __ldg(&tdp->n_tiles);
@@ -871,7 +825,7 @@ DR_D void phase_insert(const EngineParams& P, Smem& sm) {
   for (int p = 0; p < kPF; ++p) cand_walk_issue(P, cw, tile + (uint32_t)p, t_end, (uint32_t)p);
   for (uint32_t tl = tile, i = 0; tl < t_end; ++tl, ++i) {
     const uint32_t slot = i & (kPF - 1);
-    const Tile ti = load_tile(P, tl);
+    const Tile ti = load_tile(P.tiles, tl);
     cp_async_wait<kPF - 1>();                                              // the oldest group (chunk tl) has landed
     __syncwarp();
     const uint32_t c = cw.cnt[slot];
@@ -969,11 +923,11 @@ DR_D void probe_segment(const EngineParams& P, Smem& sm, const ProbeCtx& c, Load
     it = __shfl_sync(kFullMask, it, 0);
     if (it >= n_items) break;
     const uint32_t tile = c.seg_a + (it >> 2), qd = it & 3u;
-    const Tile ti = load_tile(P, tile);
+    const Tile ti = load_tile(P.tiles, tile);
     const uint32_t tl = tile - c.tile_begin;
     if (c.prefix) {
       const uint32_t pre = __ldcg(c.prefix + tl);
-      if (!(pre < c.n_sel && ti.local0 <= c.cutoff)) continue;             // tile-uniform: nothing of this sender lands here
+      if (!ships_into(pre, c.n_sel, ti.local0, c.cutoff)) continue;        // tile-uniform: nothing of this sender lands here
     }
     uint32_t hw = c.hint ? __ldcg(c.hint + 4u * tl + qd) : 0xFFFFFFFFu;
     const uint32_t n_groups = (ti.n + 31u) >> 5, g0 = qd * 32u;
@@ -1030,7 +984,7 @@ DR_D void phase_query(const EngineParams& P, Smem& sm) {
   uint32_t tile, t_end;
   tile_range(P, kPartQuery, tile, t_end);
   while (tile < t_end) {
-    const Tile t0 = load_tile(P, tile);
+    const Tile t0 = load_tile(P.tiles, tile);
     load_tensor(P, t0.tensor, sm);
     const uint32_t seg_end = min(t_end, sm.td.tile_begin + sm.td.n_tiles);
     if (sm.td.mode == (uint32_t)kModeBloom) {
@@ -1069,23 +1023,6 @@ DR_D void phase_query(const EngineParams& P, Smem& sm) {
 // W == 1 and plain fp32 values: the element is also written into the (zero-filled) dense output — the decode of a
 // rank's own contribution costs nothing extra.
 // ===========================================================================
-DR_D uint32_t hint_nibble(const uint32_t* hint, uint32_t tile_local, uint32_t lane) {
-  if (!hint) return 0xFu;
-  const uint32_t hw = __ldcg(hint + 4u * tile_local + (lane >> 3));
-  return (hw >> ((lane & 7u) * 4u)) & 0xFu;
-}
-
-// this lane's 4 mask words of a tile, restricted to hinted groups that hold real elements
-DR_D void load_masks(const uint32_t* masks, uint32_t tile, uint32_t nib, uint32_t n, uint32_t lane, uint32_t (&mm)[4]) {
-  const uint4 m4 = __ldcg(reinterpret_cast<const uint4*>(masks + (size_t)tile * kGroupsPerTile) + lane);
-  const uint32_t raw[4] = {m4.x, m4.y, m4.z, m4.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const uint32_t g = 4u * lane + (uint32_t)j;
-    mm[j] = (((nib >> j) & 1u) && g * 32u < n) ? raw[j] : 0u;
-  }
-}
-
 // Expand this lane's 4 mask words into the warp's SMEM list: the element with local (in-tile) rank r goes to
 // list[r - base] for r in [base, base + kListCap).  rank0 = local rank of this lane's first element.  Pure ALU + STS:
 // the DRAM-latency work (value gathers) then runs over the list with all lanes busy and independent loads in flight
@@ -1119,7 +1056,7 @@ DR_D void policy_filter(const EngineParams& P, Smem& sm) {
   uint32_t tile, t_end;
   tile_range(P, kPartEmit, tile, t_end);
   while (tile < t_end) {
-    const Tile t0 = load_tile(P, tile);
+    const Tile t0 = load_tile(P.tiles, tile);
     const TensorDesc* tdp = P.tensors + t0.tensor;
     const uint32_t tile_begin = __ldg(&tdp->tile_begin), n_tiles = __ldg(&tdp->n_tiles);
     const uint32_t seg_end = min(t_end, tile_begin + n_tiles);
@@ -1137,7 +1074,7 @@ DR_D void policy_filter(const EngineParams& P, Smem& sm) {
       }
       if (T != 0xFFFFFFFFu) {
         for (uint32_t tl = tile + warp; tl < seg_end; tl += (uint32_t)kWarps) {
-          const Tile ti = load_tile(P, tl);
+          const Tile ti = load_tile(P.tiles, tl);
           uint32_t mm[4];
           load_masks(P.pos_mask, tl, hint_nibble(hint, tl - tile_begin, lane), ti.n, lane, mm);
           uint32_t cnt = 0;
@@ -1182,7 +1119,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   for (uint32_t c0 = t0; c0 < t_end; c0 += (uint32_t)kTile) {
     const uint32_t n_chunk = min((uint32_t)kTile, t_end - c0);
     // ---- exclusive prefix of every tile of the chunk inside its tensor
-    const Tile first = load_tile(P, c0);
+    const Tile first = load_tile(P.tiles, c0);
     {
       const uint32_t tb = __ldg(&P.tensors[first.tensor].tile_begin);
       uint32_t part = 0;
@@ -1201,7 +1138,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
         const uint32_t i = i0 + lane;
         const bool valid = i < n_chunk;
         const uint32_t v = valid ? __ldcg(P.tile_count + c0 + i) : 0u;
-        const uint32_t tens = valid ? load_tile(P, c0 + i).tensor : 0xFFFFFFFEu;
+        const uint32_t tens = valid ? load_tile(P.tiles, c0 + i).tensor : 0xFFFFFFFEu;
         uint32_t prev_t = __shfl_up_sync(kFullMask, tens, 1);
         if (lane == 0) prev_t = carry_tensor;
         uint32_t fl = (tens != prev_t) ? 1u : 0u;                          // a new tensor starts at this tile
@@ -1232,7 +1169,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
       i = __shfl_sync(kFullMask, i, 0);
       if (i >= n_chunk) break;
       const uint32_t tile = c0 + i;
-      const Tile ti = load_tile(P, tile);
+      const Tile ti = load_tile(P.tiles, tile);
       if (ti.tensor != cur) {
         cur = ti.tensor;
         const TensorDesc* tdp = P.tensors + cur;
@@ -1677,8 +1614,8 @@ DR_D bool wait_flags(const EngineParams& P, uint32_t base, uint32_t aux_base) {
     uint32_t tile, t_end;
     decode_range(P, tile, t_end);
     if (tile < t_end) {
-      if constexpr (kB) P.grad_bf16[load_tile(P, tile).base] = 0x7FC0u;
-      else P.grad[load_tile(P, tile).base] = __uint_as_float(0x7FC00000u);
+      if constexpr (kB) P.grad_bf16[load_tile(P.tiles, tile).base] = 0x7FC0u;
+      else P.grad[load_tile(P.tiles, tile).base] = __uint_as_float(0x7FC00000u);
     }
   }
   return !any_bad;
@@ -1720,12 +1657,6 @@ DR_D uint32_t lower_bound_u32(const uint32_t* a, uint32_t n, uint32_t x) {
   return lo;
 }
 
-// dec_mask slot of (sender r, tile): senders are laid out back to back, each with `span` tiles of my slice
-DR_D uint32_t* dec_mask_base(const EngineParams& P, int r, uint32_t s_begin, uint32_t span) {
-  // probe_segment / load_masks index with the GLOBAL tile id: shift the base so that base + tile*128 is the slot
-  return P.dec_mask + ((size_t)r * span) * kGroupsPerTile - (size_t)s_begin * kGroupsPerTile;
-}
-
 template <bool kFull>
 DR_D void phase_decode(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x;
@@ -1742,11 +1673,11 @@ DR_D void phase_decode(const EngineParams& P, Smem& sm) {
   const uint64_t total = (uint64_t)(P.world - 1) * span;                   // (sender != me, tile of my slice) pairs
   uint64_t w0 = total * blockIdx.x / gridDim.x, w1 = total * (blockIdx.x + 1) / gridDim.x;
   while (w0 < w1) {
-    const uint32_t k = (uint32_t)(w0 / span);                              // k-th sender other than me
-    const int r = (int)k + ((int)k >= P.rank ? 1 : 0);
+    const uint32_t k = (uint32_t)(w0 / span);
+    const int r = other_sender(k, P.rank);
     const uint32_t tile = s_begin + (uint32_t)(w0 - (uint64_t)k * span);
     const uint32_t piece_end = s_begin + (uint32_t)min((uint64_t)span, w1 - (uint64_t)k * span);
-    const Tile t0 = load_tile(P, tile);
+    const Tile t0 = load_tile(P.tiles, tile);
     load_tensor(P, t0.tensor, sm);
     const uint32_t seg_end = min(piece_end, sm.td.tile_begin + sm.td.n_tiles);
     if (sm.td.mode == (uint32_t)kModeBloom) {
@@ -1763,7 +1694,7 @@ DR_D void phase_decode(const EngineParams& P, Smem& sm) {
         ProbeCtx c;
         c.hint = sm.td.off_hint ? slot + sm.td.off_hint : nullptr;
         c.prefix = slot + sm.td.off_prefix; c.n_sel = n_sel; c.cutoff = cutoff;
-        c.mask_out = dec_mask_base(P, r, s_begin, span); c.tile_count = nullptr;
+        c.mask_out = dec_mask_base(P.dec_mask, r, s_begin, span); c.tile_count = nullptr;
         c.tile_begin = sm.td.tile_begin; c.seg_a = tile; c.seg_b = seg_end;
         c.n_hash = sm.td.n_hash; c.m_bits = sm.td.m_bits; c.seed = P.seed;
         c.pol_T = 0xFFFFFFFFu; c.pol_seed = 0u;
@@ -1787,6 +1718,71 @@ DR_D void dbg_stamp(const EngineParams& P, int slot, int which) {
   if (P.debug_times && threadIdx.x == 0) P.debug_times[((size_t)slot * gridDim.x + blockIdx.x) * 2 + which] = globaltimer_ns();
 }
 
+// Bloom apply of sender r to tile tl (tile_local inside tensor t) of my decode span, one warp: the sender's positives of
+// the tile (my own query's, or the probe pass's in dec_mask) -> in-tile ranks (prefix table + popcounts) -> values.
+// add(e, coded) runs for every shipped positive, e = in-tile element offset (distinct per sender), coded() = its value
+// before scaling: the caller writes the whole add expression, whose FMA contraction decides the bits.
+// kGateFirst: the header words and the prefix decide whether the tile is skipped before the hint and the masks are
+// loaded (rank-ordered loop); otherwise all of them are issued first, one round trip (item loop).
+template <bool kFull, bool kGateFirst, typename AddFn>
+DR_D void apply_bloom(const EngineParams& P, uint32_t* arena, uint32_t parity, const TensorDesc& td, uint32_t t, int r,
+                      uint32_t tl, uint32_t tile_local, const Tile& ti, uint32_t s_begin, uint32_t span, uint16_t* list,
+                      uint32_t lane, AddFn add) {
+  const uint32_t* slot = slot_ptr(arena, P, parity, r);
+  const DynHeader* dyn = reinterpret_cast<const DynHeader*>(slot + kSlotHeaderWords) + t;
+  const uint32_t n_sel = __ldcg(&dyn->n_sel), cutoff = __ldcg(&dyn->cutoff);
+  if (kGateFirst && n_sel == 0u) return;
+  const uint32_t pre = __ldcg(slot + td.off_prefix + tile_local);
+  if (kGateFirst && !ships_into(pre, n_sel, ti.local0, cutoff)) return;     // warp-uniform: nothing of rank r lands here
+  const uint32_t* hint = td.off_hint ? slot + td.off_hint : nullptr;
+  const float* vals = reinterpret_cast<const float*>(slot + td.off_vals);
+  const float* fitted = P.expand_buf + (size_t)r * P.poly_total + td.poly_off;   // 'both': rank r's curve
+  const uint32_t* masks = (r == P.rank) ? P.pos_mask : dec_mask_base(P.dec_mask, r, s_begin, span);
+  uint32_t mm[4];
+  load_masks(masks, tl, hint_nibble(hint, tile_local, lane), ti.n, lane, mm);
+  if (!kGateFirst && !ships_into(pre, n_sel, ti.local0, cutoff)) return;
+  const uint32_t c = (uint32_t)(__popc(mm[0]) + __popc(mm[1]) + __popc(mm[2]) + __popc(mm[3]));
+  const uint32_t incl = warp_incl_scan(c, lane);
+  const uint32_t total = __shfl_sync(kFullMask, incl, 31);
+  const uint32_t n_take = min(total, n_sel - pre);                         // positives beyond the sender's n_sel were not shipped
+  for (uint32_t base = 0; base < n_take; base += kListCap) {
+    fill_list(list, mm, incl - c, base, lane);
+    __syncwarp();
+    const uint32_t n_here = min(kListCap, n_take - base);
+    for (uint32_t q = lane; q < n_here; q += 32u)
+      add(list[q], [&]() { return coded_value<kFull>(slot, td, vals, fitted, pre + base + q); });
+    __syncwarp();
+  }
+}
+
+// Reserve n entries of my stage-2 slice list at its cursor s2 and store the entries (idx[j], val[j]) there in every
+// peer's arena as interleaved (index, value) pairs: one 8-byte store per entry and peer, or one multicast store.  Run by
+// a group of kN threads (a warp or the CTA), of which this thread is number i; `bcast` hands every thread of the group
+// thread 0's reservation and orders the group's writes of idx / val before the stores.  Entries past s2_cap are
+// dropped: status 6.
+template <uint32_t kN, typename BcastFn>
+DR_D void s2_store(const EngineParams& P, uint32_t parity, uint32_t* s2, uint32_t i, uint32_t n, const uint32_t* idx,
+                   const float* val, BcastFn bcast) {
+  uint32_t gbase = 0;
+  if (i == 0 && n) gbase = atomicAdd(s2, n);
+  gbase = bcast(gbase);
+  uint32_t n_ok = n;
+  if (gbase + n > P.s2_cap) {
+    if (i == 0) atomicExch(P.status, kErrS2Overflow);                      // stage-2 capacity exceeded
+    n_ok = gbase < P.s2_cap ? P.s2_cap - gbase : 0u;
+  }
+  if (P.mc_arena) {
+    uint2* dst = reinterpret_cast<uint2*>(s2_ptr(P.mc_arena, P, parity, P.rank) + 4) + gbase;
+    for (uint32_t j = i; j < n_ok; j += kN) multimem_st_v2(dst + j, make_uint2(idx[j], __float_as_uint(val[j])));
+  } else {
+    for (int h = 1; h < P.world; ++h) {
+      const int peer = (P.rank + h) % P.world;
+      uint2* dst = reinterpret_cast<uint2*>(s2_ptr(P.arena[peer], P, parity, P.rank) + 4) + gbase;
+      for (uint32_t j = i; j < n_ok; j += kN) dst[j] = make_uint2(idx[j], __float_as_uint(val[j]));
+    }
+  }
+}
+
 template <bool kFull, bool kB>
 DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
@@ -1800,7 +1796,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   decode_range(P, t_first, t_last);
   // ---- (1) CTA-level: tensors without a filter (plain pairs, run-length) accumulate a tile in SMEM, rank-major
   for (uint32_t tile = t_first; tile < t_last;) {
-    const Tile t0 = load_tile(P, tile);
+    const Tile t0 = load_tile(P.tiles, tile);
     const uint32_t t = t0.tensor;
     {  // filter-coded tensors (and everything emit already scattered at W == 1) are skipped without a CTA barrier
       const TensorDesc* tdp = P.tensors + t;
@@ -1817,7 +1813,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
       const uint32_t o_sel = __ldcg(&od->n_sel), o_cut = __ldcg(&od->cutoff), o_thr = __ldcg(&od->thr_bits);
       uint16_t* list = reinterpret_cast<uint16_t*>(g_filter_smem);          // in-tile offset of the rank-th positive
       for (; tile < seg_end; ++tile) {
-        const Tile ti = load_tile(P, tile);
+        const Tile ti = load_tile(P.tiles, tile);
         const uint32_t pre = __ldcg(own + sm.td.off_prefix + (tile - sm.td.tile_begin));
         __syncthreads();
         for (int j = tid; j < kTile; j += kThreads) sm.u.acc[j] = 0.0f;
@@ -1868,7 +1864,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
         if (lane == 0 && part) atomicAdd(&sm.s.rle_pre[r], part);
       }
       for (; tile < seg_end; ++tile) {
-        const Tile ti = load_tile(P, tile);
+        const Tile ti = load_tile(P.tiles, tile);
         __syncthreads();
         for (int j = tid; j < kTile; j += kThreads) sm.u.acc[j] = 0.0f;
         __syncthreads();
@@ -1888,7 +1884,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
       }
     } else {
       for (; tile < seg_end; ++tile) {
-        const Tile ti = load_tile(P, tile);
+        const Tile ti = load_tile(P.tiles, tile);
         __syncthreads();
         for (int j = tid; j < kTile; j += kThreads) sm.u.acc[j] = 0.0f;
         __syncthreads();
@@ -1951,26 +1947,8 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
       // at the first failed position (reservations are monotonic, so everything below it was written)
       if (lane == 0) atomicMin(&sm.s.warp_tot[0], pos);
     }
-    uint32_t gbase = 0;
-    if (lane == 0) gbase = atomicAdd(s2, n_st);
-    gbase = __shfl_sync(kFullMask, gbase, 0);
-    uint32_t n_ok = n_st;
-    if (gbase + n_st > P.s2_cap) {
-      if (lane == 0) atomicExch(P.status, kErrS2Overflow);                  // stage-2 capacity exceeded
-      n_ok = gbase < P.s2_cap ? P.s2_cap - gbase : 0u;
-    }
-    __syncwarp();
-    // entries travel as interleaved (index, value) pairs: one 8-byte store per entry and peer (256 B per warp store)
-    if (P.mc_arena) {
-      uint2* dst = reinterpret_cast<uint2*>(s2_ptr(P.mc_arena, P, parity, P.rank) + 4) + gbase;
-      for (uint32_t j = lane; j < n_ok; j += 32u) multimem_st_v2(dst + j, make_uint2(st_idx[j], __float_as_uint(st_val[j])));
-    } else {
-      for (int h = 1; h < P.world; ++h) {
-        const int peer = (P.rank + h) % P.world;
-        uint2* dst = reinterpret_cast<uint2*>(s2_ptr(P.arena[peer], P, parity, P.rank) + 4) + gbase;
-        for (uint32_t j = lane; j < n_ok; j += 32u) dst[j] = make_uint2(st_idx[j], __float_as_uint(st_val[j]));
-      }
-    }
+    s2_store<32u>(P, parity, s2, lane, n_st, st_idx, st_val,
+                  [&](uint32_t g) { g = __shfl_sync(kFullMask, g, 0); __syncwarp(); return g; });
     __syncwarp();
     n_st = 0;
   };
@@ -1978,11 +1956,11 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   TensorDesc td;                                                             // this warp's current tensor (registers / local)
   auto warp_tensor = [&](uint32_t t) {
     cur = t;
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(P.tensors + cur);
-    td.mode = __ldg(src + 5); td.n_hash = 0; td.tile_begin = __ldg(src + 3);
-    td.off_vals = __ldg(src + 8); td.off_prefix = __ldg(src + 10); td.off_hint = __ldg(src + 15);
-    td.vmode = __ldg(src + 16); td.off_coef = __ldg(src + 17); td.off_rankmap = __ldg(src + 18);
-    td.poly_degree = __ldg(src + 21); td.rank_u32 = __ldg(src + 22); td.poly_off = __ldg(src + 23);
+    const TensorDesc& src = P.tensors[cur];
+    td.mode = __ldg(&src.mode); td.n_hash = 0; td.tile_begin = __ldg(&src.tile_begin);
+    td.off_vals = __ldg(&src.off_vals); td.off_prefix = __ldg(&src.off_prefix); td.off_hint = __ldg(&src.off_hint);
+    td.vmode = __ldg(&src.vmode); td.off_coef = __ldg(&src.off_coef); td.off_rankmap = __ldg(&src.off_rankmap);
+    td.poly_degree = __ldg(&src.poly_degree); td.rank_u32 = __ldg(&src.rank_u32); td.poly_off = __ldg(&src.poly_off);
   };
   const bool fast = !P.deterministic && P.world > 1;
   if (fast) {
@@ -1994,37 +1972,15 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
     for (uint64_t it = (uint64_t)blockIdx.x * kWarps + warp; it < n_items; it += n_warps) {
       const int r = (int)(it / span);
       const uint32_t tl = s_begin + (uint32_t)(it - (uint64_t)r * span);
-      const Tile ti = load_tile(P, tl);
+      const Tile ti = load_tile(P.tiles, tl);
       if (ti.tensor != cur) warp_tensor(ti.tensor);
       if (td.mode != (uint32_t)kModeBloom) continue;
-      const uint32_t tile_local = tl - td.tile_begin;
-      const uint32_t* slot = slot_ptr(arena, P, parity, r);
-      const DynHeader* dyn = reinterpret_cast<const DynHeader*>(slot + kSlotHeaderWords) + cur;
-      // one round trip: header words, prefix, hint and masks are independent loads
-      const uint32_t n_sel = __ldcg(&dyn->n_sel), cutoff = __ldcg(&dyn->cutoff);
-      const uint32_t pre = __ldcg(slot + td.off_prefix + tile_local);
-      const uint32_t* hint = td.off_hint ? slot + td.off_hint : nullptr;
-      const uint32_t* masks = (r == P.rank) ? P.pos_mask : dec_mask_base(P, r, s_begin, span);
-      uint32_t mm[4];
-      load_masks(masks, tl, hint_nibble(hint, tile_local, lane), ti.n, lane, mm);
-      if (n_sel == 0u || !(pre < n_sel && ti.local0 <= cutoff)) continue;   // warp-uniform
-      const float* vals = reinterpret_cast<const float*>(slot + td.off_vals);
-      const float* fitted = P.expand_buf + (size_t)r * P.poly_total + td.poly_off;
-      const uint32_t c = (uint32_t)(__popc(mm[0]) + __popc(mm[1]) + __popc(mm[2]) + __popc(mm[3]));
-      const uint32_t incl = warp_incl_scan(c, lane);
-      const uint32_t total = __shfl_sync(kFullMask, incl, 31);
-      const uint32_t n_take = min(total, n_sel - pre);
-      for (uint32_t base = 0; base < n_take; base += kListCap) {
-        fill_list(list, mm, incl - c, base, lane);
-        __syncwarp();
-        const uint32_t n_here = min(kListCap, n_take - base);
-        for (uint32_t q = lane; q < n_here; q += 32u) {
-          const float v = coded_value<kFull>(slot, td, vals, fitted, pre + base + q) * P.scale;
-          if constexpr (kB) atomicAdd(P.acc32 + (size_t)(tl - s_begin) * kTile + list[q], v);   // the tile's acc32 row
-          else atomicAdd(P.grad + ti.base + list[q], v);
-        }
-        __syncwarp();
-      }
+      apply_bloom<kFull, false>(P, arena, parity, td, cur, r, tl, tl - td.tile_begin, ti, s_begin, span, list, lane,
+                                [&](uint32_t e, auto coded) {
+        const float v = coded() * P.scale;
+        if constexpr (kB) atomicAdd(P.acc32 + (size_t)(tl - s_begin) * kTile + e, v);   // the tile's acc32 row
+        else atomicAdd(P.grad + ti.base + e, v);
+      });
     }
     __syncthreads();
     dbg_stamp(P, 6, 1);
@@ -2037,41 +1993,19 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   __syncthreads();
   dbg_stamp(P, 8, 0);
   for (uint32_t tl = t_first + warp; tl < t_last; tl += kWarps) {
-    const Tile ti = load_tile(P, tl);
+    const Tile ti = load_tile(P.tiles, tl);
     if (ti.tensor != cur) warp_tensor(ti.tensor);
     const bool apply = !fast && td.mode == (uint32_t)kModeBloom && !(P.world == 1 && td.vmode == 0u);
     if (apply) {
       const uint32_t tile_local = tl - td.tile_begin;
       for (int r = 0; r < P.world; ++r) {
-        const uint32_t* slot = slot_ptr(arena, P, parity, r);
-        const DynHeader* dyn = reinterpret_cast<const DynHeader*>(slot + kSlotHeaderWords) + cur;
-        const uint32_t n_sel = __ldcg(&dyn->n_sel), cutoff = __ldcg(&dyn->cutoff);
-        if (n_sel == 0u) continue;
-        const uint32_t pre = __ldcg(slot + td.off_prefix + tile_local);
-        if (!(pre < n_sel && ti.local0 <= cutoff)) continue;               // warp-uniform: nothing of rank r lands here
-        const uint32_t* hint = td.off_hint ? slot + td.off_hint : nullptr;
-        const float* vals = reinterpret_cast<const float*>(slot + td.off_vals);
-        const float* fitted = P.expand_buf + (size_t)r * P.poly_total + td.poly_off;   // 'both': rank r's curve
-        const uint32_t* masks = (r == P.rank) ? P.pos_mask : dec_mask_base(P, r, s_begin, span);
-        uint32_t mm[4];
-        load_masks(masks, tl, hint_nibble(hint, tile_local, lane), ti.n, lane, mm);
-        const uint32_t c = (uint32_t)(__popc(mm[0]) + __popc(mm[1]) + __popc(mm[2]) + __popc(mm[3]));
-        const uint32_t incl = warp_incl_scan(c, lane);
-        const uint32_t total = __shfl_sync(kFullMask, incl, 31);
-        const uint32_t n_take = min(total, n_sel - pre);                   // positives beyond the sender's n_sel were not shipped
-        for (uint32_t base = 0; base < n_take; base += kListCap) {
-          fill_list(list, mm, incl - c, base, lane);
-          __syncwarp();
-          const uint32_t n_here = min(kListCap, n_take - base);
-          for (uint32_t q = lane; q < n_here; q += 32u) {
-            const uint32_t e = list[q];
-            float* o;                                                      // bf16: the tile's acc32 row
-            if constexpr (kB) o = P.acc32 + (size_t)(tl - s_begin) * kTile + e;
-            else o = P.grad + ti.base + e;
-            *o = *o + coded_value<kFull>(slot, td, vals, fitted, pre + base + q) * P.scale;
-          }
-          __syncwarp();
-        }
+        apply_bloom<kFull, true>(P, arena, parity, td, cur, r, tl, tile_local, ti, s_begin, span, list, lane,
+                                 [&](uint32_t e, auto coded) {
+          float* o;                                                        // bf16: the tile's acc32 row
+          if constexpr (kB) o = P.acc32 + (size_t)(tl - s_begin) * kTile + e;
+          else o = P.grad + ti.base + e;
+          *o = *o + coded() * P.scale;
+        });
       }
     }
     if constexpr (kB) {
@@ -2135,24 +2069,11 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
     __syncthreads();                                                         // every warp's entries are staged / stored
     if (cta_stage) {
       const uint32_t n = min(min(sm.s.res[2], kCtaCap), sm.s.warp_tot[0]);
-      if (tid == 0) sm.s.res[3] = n ? atomicAdd(s2, n) : 0u;
-      __syncthreads();
-      const uint32_t gbase = sm.s.res[3];
-      uint32_t n_ok = n;
-      if (gbase + n > P.s2_cap) {
-        if (tid == 0) atomicExch(P.status, kErrS2Overflow);
-        n_ok = gbase < P.s2_cap ? P.s2_cap - gbase : 0u;
-      }
-      if (P.mc_arena) {
-        uint2* dst = reinterpret_cast<uint2*>(s2_ptr(P.mc_arena, P, parity, P.rank) + 4) + gbase;
-        for (uint32_t j = tid; j < n_ok; j += kThreads) multimem_st_v2(dst + j, make_uint2(cta_idx[j], __float_as_uint(cta_val[j])));
-      } else {
-        for (int h = 1; h < P.world; ++h) {
-          const int peer = (P.rank + h) % P.world;
-          uint2* dst = reinterpret_cast<uint2*>(s2_ptr(P.arena[peer], P, parity, P.rank) + 4) + gbase;
-          for (uint32_t j = tid; j < n_ok; j += kThreads) dst[j] = make_uint2(cta_idx[j], __float_as_uint(cta_val[j]));
-        }
-      }
+      s2_store<(uint32_t)kThreads>(P, parity, s2, tid, n, cta_idx, cta_val, [&](uint32_t g) {
+        if (tid == 0) sm.s.res[3] = g;
+        __syncthreads();
+        return sm.s.res[3];
+      });
       __syncthreads();
     }
     dbg_stamp(P, 8, 1);

@@ -22,48 +22,22 @@
 #include "conflict_sets.cuh"
 #include "ops.h"
 #include "plan.h"
+#include "tiles.cuh"
 
 namespace dr {
 namespace {
 
-constexpr uint32_t kFull = 0xFFFFFFFFu;
-constexpr uint32_t kGroups = kTile / 32;          // mask words per tile
 constexpr int kPickThreads = 1024;
 constexpr int kPickWarps = kPickThreads / 32;
 constexpr uint32_t kSizeCap = 32;                 // sets of >= kSizeCap members are ordered by an all-pairs rank pass
 constexpr uint32_t kMaxHash = 16;
-
-DR_D uint4 tile_row(const TileInfo* tiles, uint32_t tile) { return __ldg(reinterpret_cast<const uint4*>(tiles) + tile); }
-
-// this lane's 4 mask words of a tile, restricted to the hinted groups that hold elements (as the engine reads them)
-DR_D void tile_masks(const uint32_t* masks, uint32_t tile, const uint32_t* hint, uint32_t tile_local, uint32_t n,
-                     uint32_t lane, uint32_t (&mm)[4]) {
-  uint32_t nib = 0xFu;
-  if (hint) nib = (__ldcg(hint + 4u * tile_local + (lane >> 3)) >> ((lane & 7u) * 4u)) & 0xFu;
-  const uint4 m4 = __ldcg(reinterpret_cast<const uint4*>(masks + (size_t)tile * kGroups) + lane);
-  const uint32_t raw[4] = {m4.x, m4.y, m4.z, m4.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const uint32_t g = 4u * lane + (uint32_t)j;
-    mm[j] = (((nib >> j) & 1u) && g * 32u < n) ? raw[j] : 0u;
-  }
-}
-
-DR_D uint32_t warp_scan_incl(uint32_t v, uint32_t lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t n = __shfl_up_sync(kFull, v, o);
-    if (lane >= (uint32_t)o) v += n;
-  }
-  return v;
-}
 
 // Keep the positives of a tile whose rank q = q0 + (in-tile rank) is below pos_cap and set in `pick`; returns the
 // kept count of the warp's tile (warp-uniform) and leaves the kept masks in mm.
 template <typename PickFn>
 DR_D uint32_t thin_tile(uint32_t (&mm)[4], uint32_t q0, uint32_t pos_cap, uint32_t lane, PickFn picked) {
   const uint32_t c = (uint32_t)(__popc(mm[0]) + __popc(mm[1]) + __popc(mm[2]) + __popc(mm[3]));
-  uint32_t q = q0 + warp_scan_incl(c, lane) - c, kept = 0;
+  uint32_t q = q0 + warp_incl_scan(c, lane) - c, kept = 0;
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     uint32_t w = mm[j], keep = 0u;
@@ -77,7 +51,7 @@ DR_D uint32_t thin_tile(uint32_t (&mm)[4], uint32_t q0, uint32_t pos_cap, uint32
     kept += (uint32_t)__popc(keep);
   }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(kFull, kept, o);
+  for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(kFullMask, kept, o);
   return kept;
 }
 
@@ -98,13 +72,13 @@ DR_D uint32_t distinct_bits(uint32_t x, uint32_t seed, uint32_t n_hash, uint32_t
 // s_warp: kPickWarps + 1 words of shared memory
 DR_D uint32_t block_scan_incl(uint32_t v, uint32_t* s_warp, uint32_t& total) {
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-  const uint32_t incl = warp_scan_incl(v, lane);
+  const uint32_t incl = warp_incl_scan(v, lane);
   __syncthreads();
   if (lane == 31u) s_warp[warp] = incl;
   __syncthreads();
   if (warp == 0) {
     const uint32_t w = s_warp[lane];
-    const uint32_t wi = warp_scan_incl(w, lane);
+    const uint32_t wi = warp_incl_scan(w, lane);
     s_warp[lane] = wi - w;
     if (lane == 31u) s_warp[kPickWarps] = wi;
   }
@@ -156,15 +130,15 @@ __global__ void __launch_bounds__(kPickThreads) p2_pick_kernel(const P2Args A) {
   for (uint32_t t = warp; t < n_tiles; t += kPickWarps) {
     const uint32_t pre = pos_prefix[t];
     if (pre >= pos_cap) continue;                                            // warp-uniform
-    const uint4 ti = tile_row(A.tiles, tile_begin + t);
+    const Tile ti = load_tile(A.tiles, tile_begin + t);
     uint32_t mm[4];
-    tile_masks(A.pos_mask, tile_begin + t, hint, t, ti.z & 0xFFFFu, lane, mm);
+    load_masks(A.pos_mask, tile_begin + t, hint_nibble(hint, t, lane), ti.n, lane, mm);
     const uint32_t c = (uint32_t)(__popc(mm[0]) + __popc(mm[1]) + __popc(mm[2]) + __popc(mm[3]));
-    uint32_t q = pre + warp_scan_incl(c, lane) - c;
+    uint32_t q = pre + warp_incl_scan(c, lane) - c;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       for (uint32_t w = mm[j]; w; w &= w - 1u, ++q)
-        if (q < pos_cap) pos_idx[q] = ti.w + (4u * lane + (uint32_t)j) * 32u + (uint32_t)(__ffs((int)w) - 1);
+        if (q < pos_cap) pos_idx[q] = ti.local0 + (4u * lane + (uint32_t)j) * 32u + (uint32_t)(__ffs((int)w) - 1);
     }
   }
   __syncthreads();
@@ -213,10 +187,10 @@ __global__ void __launch_bounds__(kPickThreads) p2_pick_kernel(const P2Args A) {
     uint32_t base = 0;
     for (uint32_t cls = 1; cls <= kSizeCap; ++cls) {
       const uint32_t v = s_cls[lane][cls];
-      const uint32_t incl = warp_scan_incl(v, lane);
+      const uint32_t incl = warp_incl_scan(v, lane);
       s_cls[lane][cls] = base + incl - v;
       if (cls == kSizeCap && lane == 0) s_misc[1] = base;                  // first large set
-      base += __shfl_sync(kFull, incl, 31);
+      base += __shfl_sync(kFullMask, incl, 31);
     }
     if (lane == 0) s_misc[0] = base;                                        // number of sets
   }
@@ -229,7 +203,7 @@ __global__ void __launch_bounds__(kPickThreads) p2_pick_kernel(const P2Args A) {
       const uint32_t b = b0 + lane;
       const uint32_t s = b < hi ? __ldcg(set_off + b + 1) - __ldcg(set_off + b) : 0u;
       const uint32_t cls = s ? min(s, kSizeCap) : 0xFFFFFFFFu;
-      const uint32_t peers = __match_any_sync(kFull, cls);
+      const uint32_t peers = __match_any_sync(kFullMask, cls);
       if (s) ord[s_cls[warp][cls] + (uint32_t)__popc(peers & lt)] = b;
       __syncwarp();
       if (s && (peers & lt) == 0u) s_cls[warp][cls] += (uint32_t)__popc(peers);
@@ -270,12 +244,12 @@ __global__ void __launch_bounds__(kPickThreads) p2_pick_kernel(const P2Args A) {
   for (uint32_t i = tid; i < n_words; i += kPickThreads) pick[i] = chosen[i];
   for (uint32_t t = warp; t < n_tiles; t += kPickWarps) {
     const uint32_t tile = tile_begin + t;
-    const uint4 ti = tile_row(A.tiles, tile);
+    const Tile ti = load_tile(A.tiles, tile);
     uint32_t mm[4];
-    tile_masks(A.pos_mask, tile, hint, t, ti.z & 0xFFFFu, lane, mm);
+    load_masks(A.pos_mask, tile, hint_nibble(hint, t, lane), ti.n, lane, mm);
     const uint32_t kept = thin_tile(mm, pos_prefix[t], pos_cap, lane,
                                     [&](uint32_t q) { return ((chosen[q >> 5] >> (q & 31u)) & 1u) != 0u; });
-    reinterpret_cast<uint4*>(A.pos_mask + (size_t)tile * kGroups)[lane] = make_uint4(mm[0], mm[1], mm[2], mm[3]);
+    reinterpret_cast<uint4*>(A.pos_mask + (size_t)tile * kGroupsPerTile)[lane] = make_uint4(mm[0], mm[1], mm[2], mm[3]);
     if (lane == 0) A.tile_count[tile] = kept;
   }
   if (tid == 0) A.scratch[E.misc] = n_pos;
@@ -300,26 +274,26 @@ __global__ void __launch_bounds__(256) p2_thin_kernel(const P2Thin T) {
   const uint64_t n_warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
   for (uint64_t it = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); it < n_items; it += n_warps) {
     const uint32_t k = (uint32_t)(it / T.span);
-    const int r = (int)k + ((int)k >= T.rank ? 1 : 0);
+    const int r = other_sender(k, T.rank);
     const uint32_t tl = T.s_begin + (uint32_t)(it - (uint64_t)k * T.span);
-    const uint4 ti = tile_row(T.tiles, tl);
-    const TensorDesc* td = T.tensors + ti.x;
+    const Tile ti = load_tile(T.tiles, tl);
+    const TensorDesc* td = T.tensors + ti.tensor;
     const uint32_t pos_cap = __ldg(&td->pos_cap);
     if (pos_cap == 0u || __ldg(&td->mode) != (uint32_t)kModeBloom) continue;
     const uint32_t* slot = T.slots + (size_t)r * T.slot_words;
-    const DynHeader* dyn = reinterpret_cast<const DynHeader*>(slot + kSlotHeaderWords) + ti.x;
+    const DynHeader* dyn = reinterpret_cast<const DynHeader*>(slot + kSlotHeaderWords) + ti.tensor;
     const uint32_t n_sel = __ldcg(&dyn->n_sel), cutoff = __ldcg(&dyn->cutoff);
     const uint32_t tile_local = tl - __ldg(&td->tile_begin);
     const uint32_t pre = __ldcg(slot + __ldg(&td->off_prefix) + tile_local);
-    if (n_sel == 0u || !(pre < n_sel && ti.w <= cutoff)) continue;
+    if (!ships_into(pre, n_sel, ti.local0, cutoff)) continue;
     const uint32_t oh = __ldg(&td->off_hint);
-    uint32_t* masks = T.dec_mask + ((size_t)r * T.span - T.s_begin) * kGroups;   // indexed by the global tile, as the engine does
+    uint32_t* masks = dec_mask_base(T.dec_mask, r, T.s_begin, T.span);
     uint32_t mm[4];
-    tile_masks(masks, tl, oh ? slot + oh : nullptr, tile_local, ti.z & 0xFFFFu, lane, mm);
+    load_masks(masks, tl, hint_nibble(oh ? slot + oh : nullptr, tile_local, lane), ti.n, lane, mm);
     const uint32_t* pick = slot + __ldg(&td->off_pick);
     thin_tile(mm, __ldcg(slot + __ldg(&td->off_pos_prefix) + tile_local), pos_cap, lane,
               [&](uint32_t q) { return ((__ldcg(pick + (q >> 5)) >> (q & 31u)) & 1u) != 0u; });
-    reinterpret_cast<uint4*>(masks + (size_t)tl * kGroups)[lane] = make_uint4(mm[0], mm[1], mm[2], mm[3]);
+    reinterpret_cast<uint4*>(masks + (size_t)tl * kGroupsPerTile)[lane] = make_uint4(mm[0], mm[1], mm[2], mm[3]);
   }
 }
 

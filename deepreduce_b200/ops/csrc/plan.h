@@ -11,6 +11,7 @@
 //    size all_gather + pad-to-max of the GRACE communicator (tensors_size_are_same=False, :59,108) disappears;
 //  * DynHeader.n_sel/cutoff is policy `leftmost` / `p0` (:479-492) expressed so the receiver needs no sort.
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 
 namespace dr {
@@ -227,5 +228,33 @@ struct EngineParams {
   uint32_t acc_tiles;            // rows of acc32 (0: no tensor needs the apply)
   int bf16;
 };
+
+// Slot and slice layout, shared by the kernel and the host that launches it (binding.cpp)
+#ifdef __CUDACC__
+#define DR_PLAN_HD __host__ __device__ __forceinline__
+#else
+#define DR_PLAN_HD inline
+#endif
+
+DR_PLAN_HD bool sharded(const EngineParams& P) { return P.shard && P.world > 1; }
+
+// tiles rank `owner` decodes: everything (W == 1 / unsharded) or its 1/W slice
+DR_PLAN_HD void decode_span(const EngineParams& P, int owner, uint32_t& s_begin, uint32_t& s_end) {
+  if (sharded(P)) {
+    s_begin = (uint32_t)(((uint64_t)P.n_tiles * (uint32_t)owner) / (uint32_t)P.world);
+    s_end = (uint32_t)(((uint64_t)P.n_tiles * ((uint32_t)owner + 1u)) / (uint32_t)P.world);
+  } else { s_begin = 0; s_end = P.n_tiles; }
+}
+
+// word offset in an arena of sender `src`'s slot of the given parity (parallel/plan.py BucketPlan.slot_offset)
+DR_PLAN_HD size_t slot_offset(const EngineParams& P, uint32_t parity, int src) {
+  return kArenaHdrWords + (size_t)(parity * (uint32_t)P.world + (uint32_t)src) * P.slot_words;
+}
+
+// word offset in an arena of sender `src`'s stage-2 slot of the given parity (BucketPlan.stage2_offset)
+DR_PLAN_HD size_t s2_offset(const EngineParams& P, uint32_t parity, int src) {
+  return kArenaHdrWords + (size_t)2 * (uint32_t)P.world * P.slot_words +
+         (size_t)(parity * (uint32_t)P.world + (uint32_t)src) * P.s2_words;
+}
 
 }  // namespace dr

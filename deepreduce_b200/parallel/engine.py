@@ -33,7 +33,7 @@ import torch.distributed as dist
 from .. import spec
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
 from .plan import update_cta_speeds
-from .plan import (ARENA_HDR_WORDS, DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID,
+from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID,
                    SLOT_HEADER_WORDS, BucketPlan, rle_stream_words)
 
 (PH_ACCUM, PH_FALLBACK, PH_HIST2, PH_INSERT, PH_QUERY, PH_EMIT, PH_RANK_HIST, PH_RANK_SCAN, PH_RANK_SCATTER,
@@ -714,7 +714,7 @@ class BucketEngine:
         collectives and no size exchange (static offsets), cf. the reference's 2-3 all_gathers per tensor."""
         W, sw = self.world, self.plan.slot_words
         self.ctx.run(self.epoch, PH_ACCUM, PH_PUSH)
-        base = ARENA_HDR_WORDS + (self.epoch & 1) * W * sw
+        base = self.plan.slot_offset(W, self.epoch & 1, 0)
         out = self.arena[base:base + W * sw]
         dist.all_gather_into_tensor(out, out[self.rank * sw:(self.rank + 1) * sw], group=self.group)
         self.ctx.run(self.epoch, PH_EXPAND, PH_PUSH2)      # expand, probe pass, apply pass (unsharded: no stage 2)
@@ -734,7 +734,7 @@ class BucketEngine:
         """int32 view of the local copy of `src_rank`'s slot for `epoch`."""
         e = self.epoch if epoch is None else epoch
         r = self.rank if src_rank is None else src_rank
-        off = ARENA_HDR_WORDS + ((e & 1) * self.world + r) * self.plan.slot_words
+        off = self.plan.slot_offset(self.world, e & 1, r)
         return self.arena[off:off + self.plan.payload_words]
 
     def stats(self, src_rank: Optional[int] = None, epoch: Optional[int] = None) -> dict:
@@ -747,9 +747,8 @@ class BucketEngine:
         """Bytes this rank pushed in the stage-2 exchange of the last step (8 B per entry, to W-1 peers)."""
         if not (self.shard and self.world > 1):
             return 0
-        cap, s2w = self.plan.stage2_layout(self.world)
-        off = ARENA_HDR_WORDS + 2 * self.world * self.plan.slot_words + ((self.epoch & 1) * self.world + self.rank) * s2w
-        n = min(int(self.arena[off].item()), cap)
+        cap = self.plan.stage2_layout(self.world)[0]
+        n = min(int(self.arena[self.plan.stage2_offset(self.world, self.epoch & 1, self.rank)].item()), cap)
         return 8 * n * (self.world - 1)
 
     def check_status(self):

@@ -454,6 +454,14 @@ class BucketPlan:
             words += 2 * world * self.stage2_layout(world)[1]
         return words
 
+    def slot_offset(self, world: int, parity: int, src: int) -> int:
+        """Word offset in an arena of sender `src`'s slot of the given step parity (plan.h ``slot_offset``)."""
+        return ARENA_HDR_WORDS + (parity * world + src) * self.slot_words
+
+    def stage2_offset(self, world: int, parity: int, src: int) -> int:
+        """Word offset in an arena of sender `src`'s stage-2 slot of the given step parity (plan.h ``s2_offset``)."""
+        return ARENA_HDR_WORDS + 2 * world * self.slot_words + (parity * world + src) * self.stage2_layout(world)[1]
+
     # ---- accounting --------------------------------------------------------
     def wire_bytes(self) -> int:
         """Bytes a rank ships per step (the pushed payload)."""
