@@ -30,7 +30,7 @@ KNOWN_KEYS = frozenset({
     "policy", "sort", "poly_degree", "quantum_num", "bucket_size", "micro-benchmark", "world_size", "average",
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
-    "p2_pick_mask",
+    "p2_pick_mask", "fused_rle_values",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -102,6 +102,19 @@ class DeepReduceConfig:
             raise ConfigError("'p2_pick_mask' applies to the top-k sparsifier with the bloom index and policy "
                               f"'conflict_sets' (got compressor={cfg.compressor!r}, deepreduce={cfg.deepreduce!r}, "
                               f"index={cfg.index!r}, policy={cfg.policy!r})")
+        # opt-in route of 'both' + run-length index through the fused engine (the value codec rides behind the index);
+        # without it that combination keeps the per-tensor path and its checkpoints
+        rv = g("fused_rle_values", False)
+        if not isinstance(rv, bool):
+            raise ConfigError(f"'fused_rle_values' must be True or False (got {rv!r})")
+        if rv and not (cfg.compressor in ("topk", "threshold") and cfg.communicator == "allgather"
+                       and cfg.deepreduce == "both" and cfg.index == "rle"
+                       and (cfg.value == "polyfit" or (cfg.value == "qsgd" and cfg.bucket_size == 512))):
+            raise ConfigError("'fused_rle_values' applies to the top-k or threshold sparsifier with 'deepreduce': 'both', "
+                              "'index': 'rle' and 'value' 'polyfit' or 'qsgd' (bucket_size 512) over 'allgather' (got "
+                              f"compressor={cfg.compressor!r}, communicator={cfg.communicator!r}, "
+                              f"deepreduce={cfg.deepreduce!r}, index={cfg.index!r}, value={cfg.value!r}, "
+                              f"bucket_size={cfg.bucket_size})")
         return cfg
 
     def validate(self) -> None:

@@ -1873,9 +1873,11 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           const uint32_t c = __ldcg(reinterpret_cast<const uint16_t*>(slot + sm.td.off_prefix) + (tile - sm.td.tile_begin));
           const uint32_t pre = sm.s.rle_pre[r];
           const float* vals = reinterpret_cast<const float*>(slot + sm.td.off_vals);
+          const float* fitted = P.expand_buf + (size_t)r * P.poly_total + sm.td.poly_off;   // 'both': rank r's curve
           for (uint32_t j = tid; j < c; j += kThreads) {
             const uint32_t rp = pre + j;
-            if (rp < sm.td.val_cap) sm.u.acc[rle_get(slot + sm.td.off_idx, rp)] += __ldcg(vals + rp) * P.scale;   // distinct positions per sender
+            if (rp < sm.td.val_cap)                         // distinct positions per sender
+              sm.u.acc[rle_get(slot + sm.td.off_idx, rp)] += coded_value<kFull>(slot, sm.td, vals, fitted, rp) * P.scale;
           }
           __syncthreads();                                  // senders are added in rank order: deterministic sums
           if (tid == 0) sm.s.rle_pre[r] = pre + c;

@@ -9,6 +9,7 @@ background thread that launches the fused exchange kernel on a high-priority
 side stream; ``finish()`` makes the optimizer's stream wait on the done events.
 
 CUDA + ('topk' [+ 'index': 'bloom' | plain])  -> fused engine (one kernel/bucket)
+CUDA + 'both' + 'rle' + 'fused_rle_values'    -> fused engine, value codec over the run-length index
 CUDA + 'randomk' [+ QSGD values]              -> fused engine, values only on the wire (shared-seed index)
 CUDA + 'none'/'allreduce'                     -> dense NCCL all-reduce of the flat bucket
 anything else (CPU/gloo, other codecs)        -> GRACE-compatible per-tensor path
@@ -47,6 +48,8 @@ def _fused_supported(params: dict) -> bool:
     leftmost / random / p0, run-length), value (polyfit, QSGD int8/int16), both}.
     Bloom policy 'conflict_sets' (P2) is fused only with top-k and ``'p2_pick_mask': True``: the sender then ships its pick as a
     bitmask over the positives, a different wire from the reference's, where every receiver redraws the pick.
+    'both' with the run-length index is fused only with ``'fused_rle_values': True``: without the key that dict keeps
+    the per-tensor route it always had (and its checkpoint format).
     Not fused: 'conflict_sets' without that key (per-tensor GPU kernel), host codecs (Huffman, Deflate, dexp, the
     integer family), non-512 QSGD buckets."""
     if params.get('compressor') not in ('topk', 'threshold') or params.get('communicator', 'allgather') != 'allgather':
@@ -70,6 +73,9 @@ def _fused_supported(params: dict) -> bool:
         return value_ok                  # coded values + plain indices
     if dr == 'both' and params.get('index', 'bloom') == 'bloom':
         return pol_ok and value_ok
+    if dr == 'both' and params.get('index') == 'rle':
+        # the bloom policies do not apply to a lossless index; the fused plan refuses 'conflict_sets' outside bloom
+        return params.get('fused_rle_values') is True and value_ok and policy != 'conflict_sets'
     return False
 
 

@@ -178,7 +178,7 @@ class BucketPlan:
     max_hash: int = 16
     ks: Optional[Sequence[int]] = None    # explicit per-tensor K (overrides compress_ratio)
     hint: bool = True                     # ship the 1-bit-per-32-elements occupancy hint next to each bloom filter
-    value: Optional[str] = None           # None (fp32 values), 'polyfit' or 'qsgd' ('both': bloom index + value codec)
+    value: Optional[str] = None           # None (fp32 values), 'polyfit' or 'qsgd' ('both': bloom or rle index + value codec)
     quantum_num: int = 127                # QSGD levels (int8 on the wire)
     poly_degree: int = 5
     poly_min_k: int = 512                 # tensors shipping fewer values keep them as fp32 (the fit header would be larger)
@@ -193,8 +193,6 @@ class BucketPlan:
     def __post_init__(self):
         if self.index not in (None, "bloom", "rle"):
             raise ValueError(f"fused engine index codecs: None, 'bloom', 'rle'; got {self.index!r}")
-        if self.index == "rle" and self.value is not None:
-            raise NotImplementedError("value codecs are fused with the bloom index or plain indices, not with 'rle'")
         if self.value not in (None, "polyfit", "qsgd"):
             raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd'; got {self.value!r}")
         if self.sparsifier not in ("topk", "threshold", "randomk"):
@@ -281,11 +279,11 @@ class BucketPlan:
                     word = _align(word + (tp.pos_cap + 31) // 32, 4)
             elif self.index == "rle" and d > self.min_numel:
                 # lossless run coding of the selection bitmap, tile-local: a u16 count per tile and, per selected
-                # element, the zeros+ones run offset from the tile start (< 4096 -> 12 bits), bit-packed
+                # element, the zeros+ones run offset from the tile start (< 4096 -> 12 bits), bit-packed; the values
+                # (fp32, or a value codec with its fp32 values in sender-local scratch) come first
                 tp.mode = MODE_RLE
                 tp.val_cap = k
-                tp.off_vals = word
-                word = _align(word + k, 4)
+                word = self._value_region(tp, word, scratch)
                 tp.off_prefix = word
                 word = _align(word + (n_tiles + 1) // 2, 4)
                 tp.off_idx = word
