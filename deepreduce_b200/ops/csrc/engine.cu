@@ -1287,12 +1287,22 @@ DR_D uint32_t load_rank(const uint32_t* slot, const TensorDesc& td, uint32_t p) 
 }
 
 // ---- exact descending rank: counting sort on 13 bits of the order-preserving key + all-pairs inside a bin ----
-// Bins are monotone non-increasing in the value and centred on the tensor's selection threshold T (31-bit
-// key): per sign 1024 coarse bins above 4T (16 per octave), 2048 fine bins on [T, 4T) (relative width 2^-10)
-// and 1024 coarse bins below T (false positives carry arbitrary small values).  Exactness never depends on
+// order_key: the float's bits made monotone as an unsigned integer (sign-magnitude flipped), with -0.0 folded onto
+// +0.0.  Equal values get equal keys, so ties (the two zeros included) are broken by position alone, as the stable
+// descending sort of the specification does; and a NaN still gets a key, so the ranks are a permutation whatever
+// the values are (a NaN's place among them is unspecified).
+DR_D uint32_t order_key(float v) {
+  const uint32_t b = __float_as_uint(v) == 0x80000000u ? 0u : __float_as_uint(v);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+// Bins are monotone non-increasing in the order key and centred on the tensor's selection threshold T (31-bit
+// magnitude key): per sign 1024 coarse bins above 4T (16 per octave), 2048 fine bins on [T, 4T) (relative width
+// 2^-10) and 1024 coarse bins below T (false positives carry arbitrary small values).  Exactness never depends on
 // the binning — phase 9 counts inside the bin — only the amount of in-bin work does.
-DR_D uint32_t rank_bin(float v, uint32_t T) {
-  const uint32_t bits = __float_as_uint(v), key = bits & 0x7FFFFFFFu;
+DR_D uint32_t rank_bin(uint32_t ok, uint32_t T) {
+  const bool neg = !(ok & 0x80000000u);
+  const uint32_t key = (neg ? ~ok : ok) & 0x7FFFFFFFu;
   uint32_t pb;                                   // 0 = largest magnitude ... 4095 = smallest
   if (key >= T) {
     const uint32_t d = key - T;
@@ -1301,7 +1311,7 @@ DR_D uint32_t rank_bin(float v, uint32_t T) {
   } else {
     pb = 3072u + min(1023u, (T >> 19) - (key >> 19));
   }
-  return (bits & 0x80000000u) ? (4096u + (4095u - pb)) : pb;
+  return neg ? (4096u + (4095u - pb)) : pb;
 }
 
 // phase 6: bin populations
@@ -1316,7 +1326,7 @@ DR_D void phase_rank_hist(const EngineParams& P, Smem& sm) {
     const uint32_t n = __ldcg(&dyn->n_sel), p = p0 + threadIdx.x;
     if (p < n) {
       const float v = __ldcg(reinterpret_cast<const float*>(my_slot + sm.td.off_vals) + p);
-      atomicAdd(P.poly_bins + (size_t)sm.td.poly_ord * 2 * kRankBins + rank_bin(v, __ldcg(&P.sel[t].thr)), 1u);
+      atomicAdd(P.poly_bins + (size_t)sm.td.poly_ord * 2 * kRankBins + rank_bin(order_key(v), __ldcg(&P.sel[t].thr)), 1u);
     }
   }
 }
@@ -1358,7 +1368,7 @@ DR_D void phase_rank_scatter(const EngineParams& P, Smem& sm) {
     if (p < n) {
       const float v = __ldcg(reinterpret_cast<const float*>(my_slot + sm.td.off_vals) + p);
       uint32_t* tab = P.poly_bins + (size_t)sm.td.poly_ord * 2 * kRankBins;
-      const uint32_t b = rank_bin(v, __ldcg(&P.sel[t].thr));
+      const uint32_t b = rank_bin(order_key(v), __ldcg(&P.sel[t].thr));
       // the count array is re-used as the running cursor: it is decremented down to 0 while filling the bin
       const uint32_t within = atomicSub(tab + b, 1u) - 1u;
       const uint32_t pos = __ldcg(tab + kRankBins + b) + within;
@@ -1383,13 +1393,13 @@ DR_D void phase_rank_exact(const EngineParams& P, Smem& sm) {
       const float* bv = P.bucket_val + sm.td.poly_off;
       const uint32_t* bp = P.bucket_pos + sm.td.poly_off;
       v = __ldcg(bv + i);
-      const uint32_t p = __ldcg(bp + i), b = rank_bin(v, __ldcg(&P.sel[t].thr));
+      const uint32_t p = __ldcg(bp + i), k = order_key(v), b = rank_bin(k, __ldcg(&P.sel[t].thr));
       const uint32_t* start = P.poly_bins + (size_t)sm.td.poly_ord * 2 * kRankBins + kRankBins;
       const uint32_t lo = __ldcg(start + b), hi = (b + 1 < (uint32_t)kRankBins) ? __ldcg(start + b + 1) : n;
       uint32_t rank = lo;
-      for (uint32_t q = lo; q < hi; ++q) {
-        const float w = __ldcg(bv + q);
-        rank += (w > v || (w == v && __ldcg(bp + q) < p)) ? 1u : 0u;
+      for (uint32_t q = lo; q < hi; ++q) {               // (key, position) is a strict total order: a permutation
+        const uint32_t kw = order_key(__ldcg(bv + q));
+        rank += (kw > k || (kw == k && __ldcg(bp + q) < p)) ? 1u : 0u;
       }
       if (sm.td.rank_u32) my_slot[sm.td.off_rankmap + p] = rank;
       else reinterpret_cast<uint16_t*>(my_slot + sm.td.off_rankmap)[p] = (uint16_t)rank;

@@ -295,49 +295,10 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
     assert int(a[0]) == MAGIC and int(a[2]) == len(plan.tensors), "not a slot of this plan"
     out = torch.zeros(plan.total_elems, dtype=torch.float32)
     for ti, t in enumerate(plan.tensors):
-        d0 = SLOT_HEADER_WORDS + DYN_WORDS * ti
-        n_sel, cutoff = int(a[d0]), int(a[d0 + 1])
-        if n_sel == 0:
-            continue
-        if t.mode == MODE_BLOOM:
-            words = torch.from_numpy(a[t.off_filter:t.off_filter + t.n_filter_words].view(np.int32).copy())
-            pos = bloom_query_oracle(words, t.numel, t.n_hash, t.m_bits, seed)          # ascending positives of the universe
-            if t.off_hint:                                                               # only inside occupied 32-element groups
-                hint = a[t.off_hint:t.off_hint + 4 * t.n_tiles]
-                grp = pos // 32                                                          # group id: tile*128 + (e // 32)
-                tile, gi = grp // 128, grp % 128
-                bit = (torch.from_numpy(hint.astype(np.int64))[tile * 4 + gi // 32] >> (gi % 32)) & 1
-                pos = pos[bit.bool()]
-            if plan.policy == "random":
-                pos, _ = random_policy_filter(pos, 0, 0, int(a[1]), t.salt, T=int(a[d0 + 2]))
-            if plan.policy == "conflict_sets":
-                starts = torch.arange(t.n_tiles, dtype=torch.int64) * spec.TILE
-                pp = torch.from_numpy(a[t.off_pos_prefix:t.off_pos_prefix + t.n_tiles].astype(np.int64))
-                assert torch.equal(torch.clamp(torch.searchsorted(pos, starts), max=t.pos_cap), pp), t.name
-                pos = conflict_sets_keep_oracle(t, pos, a[t.off_pick:t.off_pick + (t.pos_cap + 31) // 32])
-            if cutoff != 0xFFFFFFFF:
-                pos = pos[pos <= cutoff]
-            idx = pos[:n_sel]
-            # the per-tile prefix table must agree with what the receiver recomputes (the kernel starts ranks from it)
-            starts = torch.arange(t.n_tiles, dtype=torch.int64) * spec.TILE
-            pre = torch.from_numpy(a[t.off_prefix:t.off_prefix + t.n_tiles].astype(np.int64))
-            assert torch.equal(torch.minimum(torch.searchsorted(pos, starts), torch.tensor(n_sel)), pre), t.name
-        elif t.mode == MODE_RLE:
-            cnt = a[t.off_prefix:t.off_prefix + (t.n_tiles + 1) // 2].view(np.uint16)[:t.n_tiles].astype(np.int64)
-            assert int(cnt.sum()) == n_sel, t.name
-            local = rle_unpack12(a[t.off_idx:t.off_idx + rle_stream_words(t.val_cap)], n_sel)
-            idx = torch.from_numpy(np.repeat(np.arange(t.n_tiles, dtype=np.int64), cnt) * spec.TILE + local)
-        elif t.mode == MODE_SHARED:
-            # the index set is drawn again from the plan and the epoch in slot word 1; the sender's threshold must match
-            pos, thr = select_randomk_oracle(t.numel, t.k, int(a[1]), t.salt)
-            assert thr == int(a[d0 + 2]), (t.name, thr, int(a[d0 + 2]))
-            if cutoff != 0xFFFFFFFF:
-                pos = pos[pos <= cutoff]
-            idx = pos[:n_sel]
-            assert int(idx.numel()) == n_sel, t.name
-        else:
-            idx = torch.from_numpy(a[t.off_idx:t.off_idx + n_sel].astype(np.int64))
+        idx = shipped_index_oracle(plan, a, ti, seed=seed)
         n = int(idx.numel())
+        if n == 0:
+            continue
         if t.vmode == 1:
             from ..codecs.polyfit import MAX_SEGMENTS, get_segments, polyfit_eval_oracle
             nc = MAX_SEGMENTS * (t.poly_degree + 1)
@@ -361,6 +322,56 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
             vals = torch.from_numpy(a[t.off_vals:t.off_vals + n].view(np.float32).copy())
         out[t.elem_off:t.elem_off + t.numel].index_add_(0, idx, vals.float())
     return out
+
+
+def shipped_index_oracle(plan: BucketPlan, slot, ti: int, *, seed=spec.DEFAULT_SEED) -> torch.Tensor:
+    """The ascending element indices (within tensor ``ti``) whose values one sender's slot carries, rebuilt from the
+    plan and the slot's words alone; the p-th shipped value belongs to the p-th index."""
+    a = slot.detach().cpu().numpy().view(np.uint32) if torch.is_tensor(slot) else np.asarray(slot, dtype=np.uint32)
+    t = plan.tensors[ti]
+    d0 = SLOT_HEADER_WORDS + DYN_WORDS * ti
+    n_sel, cutoff = int(a[d0]), int(a[d0 + 1])
+    if n_sel == 0:
+        return torch.empty(0, dtype=torch.int64)
+    if t.mode == MODE_BLOOM:
+        words = torch.from_numpy(a[t.off_filter:t.off_filter + t.n_filter_words].view(np.int32).copy())
+        pos = bloom_query_oracle(words, t.numel, t.n_hash, t.m_bits, seed)          # ascending positives of the universe
+        if t.off_hint:                                                               # only inside occupied 32-element groups
+            hint = a[t.off_hint:t.off_hint + 4 * t.n_tiles]
+            grp = pos // 32                                                          # group id: tile*128 + (e // 32)
+            tile, gi = grp // 128, grp % 128
+            bit = (torch.from_numpy(hint.astype(np.int64))[tile * 4 + gi // 32] >> (gi % 32)) & 1
+            pos = pos[bit.bool()]
+        if plan.policy == "random":
+            pos, _ = random_policy_filter(pos, 0, 0, int(a[1]), t.salt, T=int(a[d0 + 2]))
+        if plan.policy == "conflict_sets":
+            starts = torch.arange(t.n_tiles, dtype=torch.int64) * spec.TILE
+            pp = torch.from_numpy(a[t.off_pos_prefix:t.off_pos_prefix + t.n_tiles].astype(np.int64))
+            assert torch.equal(torch.clamp(torch.searchsorted(pos, starts), max=t.pos_cap), pp), t.name
+            pos = conflict_sets_keep_oracle(t, pos, a[t.off_pick:t.off_pick + (t.pos_cap + 31) // 32])
+        if cutoff != 0xFFFFFFFF:
+            pos = pos[pos <= cutoff]
+        idx = pos[:n_sel]
+        # the per-tile prefix table must agree with what the receiver recomputes (the kernel starts ranks from it)
+        starts = torch.arange(t.n_tiles, dtype=torch.int64) * spec.TILE
+        pre = torch.from_numpy(a[t.off_prefix:t.off_prefix + t.n_tiles].astype(np.int64))
+        assert torch.equal(torch.minimum(torch.searchsorted(pos, starts), torch.tensor(n_sel)), pre), t.name
+    elif t.mode == MODE_RLE:
+        cnt = a[t.off_prefix:t.off_prefix + (t.n_tiles + 1) // 2].view(np.uint16)[:t.n_tiles].astype(np.int64)
+        assert int(cnt.sum()) == n_sel, t.name
+        local = rle_unpack12(a[t.off_idx:t.off_idx + rle_stream_words(t.val_cap)], n_sel)
+        idx = torch.from_numpy(np.repeat(np.arange(t.n_tiles, dtype=np.int64), cnt) * spec.TILE + local)
+    elif t.mode == MODE_SHARED:
+        # the index set is drawn again from the plan and the epoch in slot word 1; the sender's threshold must match
+        pos, thr = select_randomk_oracle(t.numel, t.k, int(a[1]), t.salt)
+        assert thr == int(a[d0 + 2]), (t.name, thr, int(a[d0 + 2]))
+        if cutoff != 0xFFFFFFFF:
+            pos = pos[pos <= cutoff]
+        idx = pos[:n_sel]
+        assert int(idx.numel()) == n_sel, t.name
+    else:
+        idx = torch.from_numpy(a[t.off_idx:t.off_idx + n_sel].astype(np.int64))
+    return idx
 
 
 # ---------------------------------------------------------------------------
