@@ -30,7 +30,7 @@ KNOWN_KEYS = frozenset({
     "policy", "sort", "poly_degree", "quantum_num", "bucket_size", "micro-benchmark", "world_size", "average",
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
-    "p2_pick_mask", "fused_rle_values",
+    "p2_pick_mask", "fused_rle_values", "fused_dexp",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -115,6 +115,22 @@ class DeepReduceConfig:
                               f"compressor={cfg.compressor!r}, communicator={cfg.communicator!r}, "
                               f"deepreduce={cfg.deepreduce!r}, index={cfg.index!r}, value={cfg.value!r}, "
                               f"bucket_size={cfg.bucket_size})")
+        # opt-in route of double-exponential values through the fused engine (two curves per tensor, one per sign run,
+        # over the fused rank map); without it 'dexp' keeps the per-tensor path, its wire and its checkpoints
+        fd = g("fused_dexp", False)
+        if not isinstance(fd, bool):
+            raise ConfigError(f"'fused_dexp' must be True or False (got {fd!r})")
+        if fd and not (cfg.compressor in ("topk", "threshold") and cfg.communicator == "allgather"
+                       and cfg.deepreduce in ("value", "both") and cfg.value in ("dexp", "double_exp")
+                       and ((cfg.index == "bloom" and (cfg.policy in ("leftmost", "leftmostK", "random", "randomK", "p0",
+                                                                      "policy_zero") or p2))
+                            or (cfg.index == "rle" and cfg.policy not in ("conflict_sets", "p2")))):
+            raise ConfigError("'fused_dexp' applies to the top-k or threshold sparsifier with 'deepreduce': 'value' or "
+                              "'both', 'value': 'dexp' and 'index' 'bloom' (policy leftmost, random, p0, or conflict_sets "
+                              "with 'p2_pick_mask') or 'rle', over 'allgather' (got "
+                              f"compressor={cfg.compressor!r}, communicator={cfg.communicator!r}, "
+                              f"deepreduce={cfg.deepreduce!r}, value={cfg.value!r}, index={cfg.index!r}, "
+                              f"policy={cfg.policy!r})")
         return cfg
 
     def validate(self) -> None:

@@ -30,6 +30,7 @@
 // v10 -> v11 (profiles/): 4 passes over d -> 1, per-tile CTA barriers -> mbarrier
 // full/empty ring + warp-private work, probe chains run on dense survivor batches.
 #include "common.cuh"
+#include "dexp_fit.cuh"
 #include "plan.h"
 #include "tiles.cuh"
 
@@ -86,6 +87,7 @@ struct Smem {
     uint32_t q[kWarps][64];                   // probe passes: per-warp survivor ring
     uint32_t excl[kTile];                     // emit: exclusive prefixes of a chunk of tiles
     uint32_t sel[kWarps][32];                 // insert: selected elements of one warp iteration
+    DexpScratch dexp;                         // fit phase: one double-exponential fit
   } u;
   ScanSmem s;
   TensorDesc td;                              // current tensor
@@ -1281,6 +1283,26 @@ DR_D float poly_value(const float* __restrict__ coef, const int* start, int n_se
   return acc;
 }
 
+// 'dexp' (vmode 3): two double-exponential curves per tensor, over the rank map's two sign runs.  Coefficient words
+// (fp32): {a, b, p, q} of the positive run by ascending value, then {a, b, p, q} of the magnitudes of the rest (the
+// values <= 0) by ascending |v|; each on its own abscissa x_i = (i + 1) / run length.
+DR_D bool ranked(uint32_t vmode) { return vmode == 1u || vmode == 3u; }
+
+// words before the {num_pos, n} tail of a ranked tensor's header
+DR_D uint32_t coef_words(uint32_t vmode, uint32_t deg) { return vmode == 3u ? kDexpCoefWords : kMaxSeg * (deg + 1u); }
+
+// fitted value of rank j (descending order) from the shipped fp32 words: the sender's residual and every receiver's
+// decode go through this one evaluation, in fp64 without contraction (the oracle's torch order), rounded once
+DR_D float dexp_value(const float* __restrict__ coef, uint32_t num_pos, uint32_t n, uint32_t j) {
+  const bool pos = j < num_pos;
+  const uint32_t len = pos ? num_pos : n - num_pos, i = pos ? num_pos - 1u - j : j - num_pos;
+  const float* c = coef + (pos ? 0 : 4);
+  const double x = (double)(i + 1u) / (double)len;
+  const double v = __dadd_rn(__dmul_rn((double)__ldcg(c), exp(__dmul_rn((double)__ldcg(c + 2), x))),
+                             __dmul_rn((double)__ldcg(c + 1), exp(__dmul_rn((double)__ldcg(c + 3), x))));
+  return pos ? (float)v : -(float)v;
+}
+
 DR_D uint32_t load_rank(const uint32_t* slot, const TensorDesc& td, uint32_t p) {
   return td.rank_u32 ? __ldcg(slot + td.off_rankmap + p)
                      : (uint32_t)__ldcg(reinterpret_cast<const uint16_t*>(slot + td.off_rankmap) + p);
@@ -1321,7 +1343,7 @@ DR_D void phase_rank_hist(const EngineParams& P, Smem& sm) {
   for (uint32_t task = blockIdx.x; task < P.n_poly_tasks; task += gridDim.x) {
     const uint32_t t = __ldg(P.poly_tasks + 2 * task), p0 = __ldg(P.poly_tasks + 2 * task + 1);
     load_tensor(P, t, sm);
-    if (sm.td.vmode != 1) continue;
+    if (!ranked(sm.td.vmode)) continue;
     const DynHeader* dyn = reinterpret_cast<const DynHeader*>(my_slot + kSlotHeaderWords) + t;
     const uint32_t n = __ldcg(&dyn->n_sel), p = p0 + threadIdx.x;
     if (p < n) {
@@ -1362,7 +1384,7 @@ DR_D void phase_rank_scatter(const EngineParams& P, Smem& sm) {
   for (uint32_t task = blockIdx.x; task < P.n_poly_tasks; task += gridDim.x) {
     const uint32_t t = __ldg(P.poly_tasks + 2 * task), p0 = __ldg(P.poly_tasks + 2 * task + 1);
     load_tensor(P, t, sm);
-    if (sm.td.vmode != 1) continue;
+    if (!ranked(sm.td.vmode)) continue;
     const DynHeader* dyn = reinterpret_cast<const DynHeader*>(my_slot + kSlotHeaderWords) + t;
     const uint32_t n = __ldcg(&dyn->n_sel), p = p0 + threadIdx.x;
     if (p < n) {
@@ -1385,7 +1407,7 @@ DR_D void phase_rank_exact(const EngineParams& P, Smem& sm) {
   for (uint32_t task = blockIdx.x; task < P.n_poly_tasks; task += gridDim.x) {
     const uint32_t t = __ldg(P.poly_tasks + 2 * task), p0 = __ldg(P.poly_tasks + 2 * task + 1);
     load_tensor(P, t, sm);
-    if (sm.td.vmode != 1) continue;
+    if (!ranked(sm.td.vmode)) continue;
     const DynHeader* dyn = reinterpret_cast<const DynHeader*>(my_slot + kSlotHeaderWords) + t;
     const uint32_t n = __ldcg(&dyn->n_sel), i = p0 + threadIdx.x;   // i = position in the grouped arrays
     float v = 0.f;
@@ -1407,14 +1429,15 @@ DR_D void phase_rank_exact(const EngineParams& P, Smem& sm) {
     }
     const uint32_t pc = __syncthreads_count(i < n && v > 0.f);
     if (threadIdx.x == 0) {
-      uint32_t* tail = my_slot + sm.td.off_coef + kMaxSeg * (sm.td.poly_degree + 1);
+      uint32_t* tail = my_slot + sm.td.off_coef + coef_words(sm.td.vmode, sm.td.poly_degree);
       if (pc) atomicAdd(tail, pc);
       if (p0 == 0) tail[1] = n;
     }
   }
 }
 
-// phase 10: one warp per (tensor, segment): Gram least squares  c_k = sum p_k y / sum p_k^2
+// phase 10: one warp per (tensor, segment): Gram least squares  c_k = sum p_k y / sum p_k^2;
+// 'dexp' tensors: one CTA per (tensor, sign run), the double-exponential regression of dexp_fit.cuh
 DR_D void phase_fit(const EngineParams& P, Smem& sm) {
   const uint32_t parity = P.epoch & 1u;
   uint32_t* my_slot = slot_ptr(P.arena[P.rank], P, parity, P.rank);
@@ -1423,6 +1446,7 @@ DR_D void phase_fit(const EngineParams& P, Smem& sm) {
   for (uint32_t task = gw; task < P.n_poly * kMaxSeg; task += nw) {
     const uint32_t t = __ldg(P.poly_tensors + task / kMaxSeg), s = task % kMaxSeg;
     const TensorDesc* td = P.tensors + t;
+    if (__ldg(&td->vmode) != 1u) continue;
     const uint32_t off_coef = __ldg(&td->off_coef), off_sorted = __ldg(&td->off_sorted);
     const int deg = (int)__ldg(&td->poly_degree);
     const uint32_t* tail = my_slot + off_coef + kMaxSeg * (deg + 1);
@@ -1479,6 +1503,24 @@ DR_D void phase_fit(const EngineParams& P, Smem& sm) {
     for (int k = 0; k <= kMaxDeg; ++k)
       if ((int)lane == k && k <= deg) coef[k] = (k <= deg_eff && den[k] > 0.f) ? num[k] / den[k] : 0.f;
   }
+  // 'dexp': one CTA per (tensor, sign run) runs the fp64 regression over the sorted values of that run
+  for (uint32_t task = blockIdx.x; task < 2u * P.n_poly; task += gridDim.x) {
+    const uint32_t t = __ldg(P.poly_tensors + task / 2u), neg = task & 1u;
+    const TensorDesc* td = P.tensors + t;
+    if (__ldg(&td->vmode) != 3u) continue;
+    float* coef = reinterpret_cast<float*>(my_slot + __ldg(&td->off_coef));
+    const uint32_t* tail = my_slot + __ldg(&td->off_coef) + kDexpCoefWords;
+    const uint32_t num_pos = __ldcg(tail), n = __ldcg(tail + 1);
+    const float* ys = reinterpret_cast<const float*>(my_slot + __ldg(&td->off_sorted)) + num_pos;   // the split
+    double c[4];
+    // positive run: descending ranks num_pos-1 .. 0; the rest: |v| = -v in rank order
+    dexp_fit_block<kThreads>([&](int64_t k) { return neg ? -(double)__ldcg(ys + k) : (double)__ldcg(ys - 1 - k); },
+                             (int64_t)(neg ? n - num_pos : num_pos), sm.u.dexp, c);
+    if (threadIdx.x == 0) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) coef[4 * neg + i] = (float)c[i];
+    }
+  }
 }
 
 // phase 11: error feedback sees the fit error: resid[idx_p] = value_p - fitted_p
@@ -1520,15 +1562,17 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
       continue;
     }
     const int deg = (int)sm.td.poly_degree;
-    const uint32_t* tail = my_slot + sm.td.off_coef + kMaxSeg * (deg + 1);
+    const uint32_t* tail = my_slot + sm.td.off_coef + coef_words(sm.td.vmode, deg);
     const int num_pos = (int)__ldcg(tail), n = (int)__ldcg(tail + 1);
     if ((int)p0 >= n) continue;
-    if (threadIdx.x == 0) build_segments(n, num_pos, sm.seg_start, sm.n_seg);
+    const bool dexp = sm.td.vmode == 3u;
+    if (threadIdx.x == 0 && !dexp) build_segments(n, num_pos, sm.seg_start, sm.n_seg);
     __syncthreads();
     const uint32_t p = p0 + threadIdx.x;
     if ((int)p < n) {
-      const float fitted = poly_value(reinterpret_cast<const float*>(my_slot + sm.td.off_coef), sm.seg_start, sm.n_seg,
-                                      deg, load_rank(my_slot, sm.td, p));
+      const float* coef = reinterpret_cast<const float*>(my_slot + sm.td.off_coef);
+      const uint32_t rank = load_rank(my_slot, sm.td, p);
+      const float fitted = dexp ? dexp_value(coef, num_pos, n, rank) : poly_value(coef, sm.seg_start, sm.n_seg, deg, rank);
       const float v = __ldcg(reinterpret_cast<const float*>(my_slot + sm.td.off_vals) + p);
       P.resid[__ldcg(my_slot + sm.td.off_selidx + p)] = v - fitted;
     }
@@ -1543,18 +1587,20 @@ DR_D void phase_expand(const EngineParams& P, Smem& sm) {
     const uint32_t r = wt / P.n_poly_tasks, task = wt - r * P.n_poly_tasks;
     const uint32_t t = __ldg(P.poly_tasks + 2 * task), j0 = __ldg(P.poly_tasks + 2 * task + 1);
     load_tensor(P, t, sm);
-    if (sm.td.vmode != 1) continue;
+    if (!ranked(sm.td.vmode)) continue;
     const uint32_t* slot = slot_ptr(arena, P, parity, (int)r);
     const int deg = (int)sm.td.poly_degree;
-    const uint32_t* tail = slot + sm.td.off_coef + kMaxSeg * (deg + 1);
+    const uint32_t* tail = slot + sm.td.off_coef + coef_words(sm.td.vmode, deg);
     const int num_pos = (int)__ldcg(tail), n = (int)__ldcg(tail + 1);
     if ((int)j0 >= n) continue;
-    if (threadIdx.x == 0) build_segments(n, num_pos, sm.seg_start, sm.n_seg);
+    const bool dexp = sm.td.vmode == 3u;
+    if (threadIdx.x == 0 && !dexp) build_segments(n, num_pos, sm.seg_start, sm.n_seg);
     __syncthreads();
     const uint32_t j = j0 + threadIdx.x;
+    const float* coef = reinterpret_cast<const float*>(slot + sm.td.off_coef);
     if ((int)j < n)
       P.expand_buf[(size_t)r * P.poly_total + sm.td.poly_off + j] =
-          poly_value(reinterpret_cast<const float*>(slot + sm.td.off_coef), sm.seg_start, sm.n_seg, deg, j);
+          dexp ? dexp_value(coef, num_pos, n, j) : poly_value(coef, sm.seg_start, sm.n_seg, deg, j);
   }
 }
 
@@ -1635,7 +1681,7 @@ DR_D bool wait_flags(const EngineParams& P, uint32_t base, uint32_t aux_base) {
 // value of the p-th shipped coordinate of a sender's tensor under its value codec
 template <bool kFull>
 DR_D float coded_value(const uint32_t* slot, const TensorDesc& td, const float* vals, const float* fitted, uint32_t rp) {
-  if (kFull && td.vmode == 1u) return __ldcg(fitted + load_rank(slot, td, rp));
+  if (kFull && ranked(td.vmode)) return __ldcg(fitted + load_rank(slot, td, rp));
   if (kFull && td.vmode == 2u) {
     const float norm = __ldcg(reinterpret_cast<const float*>(slot + td.off_coef) + (rp >> 9));
     const float lvl = td.rank_u32 ? (float)__ldcg(reinterpret_cast<const int16_t*>(slot + td.off_rankmap) + rp)

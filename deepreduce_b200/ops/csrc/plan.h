@@ -53,8 +53,9 @@ struct TensorDesc {
   uint32_t off_hint;     // 0 = none; else 4 words per tile: bit g set <=> 32-element group g holds a selected element
   // ---- value codec ('both': bloom index + polynomial fit of the values) ----
   uint32_t vmode;        // 0 = fp32 values on the wire, 1 = piece-wise Gram-polynomial fit + rank map,
-                         // 2 = bucketed QSGD (int8 levels, or int16 when rank_u32 is set: quantum_num >= 128)
-  uint32_t off_coef;     // [kMaxSeg * (deg+1)] float coefficients, then {num_pos, n}
+                         // 2 = bucketed QSGD (int8 levels, or int16 when rank_u32 is set: quantum_num >= 128),
+                         // 3 = double-exponential fit of each sign run + rank map
+  uint32_t off_coef;     // [kMaxSeg * (deg+1)] (vmode 3: [kDexpCoefWords]) float coefficients, then {num_pos, n}
   uint32_t off_rankmap;  // rank of the p-th shipped value in the descending sort (u16 if val_cap <= 65536 else u32)
   uint32_t off_selidx;   // scratch (not shipped): element index of the p-th shipped value
   uint32_t off_sorted;   // scratch (not shipped): values in descending order
@@ -75,6 +76,7 @@ constexpr int kDescWords = 32;
 constexpr int kRankBins = 8192;        // 'both': counting-sort bins = sign + 8 exponent + 4 mantissa bits
 constexpr int kMaxSeg = 22;            // codecs/polyfit.py MAX_SEGMENTS
 constexpr int kMaxDeg = 7;
+constexpr uint32_t kDexpCoefWords = 8;  // vmode 3: {a, b, p, q} of the positive run, then of the non-positive run
 
 // payload slot layout (uint32 words):
 //   [0..8)                      : magic, epoch, n_tensors, payload_words, rank, 0,0,0
@@ -132,7 +134,7 @@ enum Phase : int {
   kPhRankScan = 7,   // per-tensor exclusive prefix over the bins
   kPhRankScatter = 8,// group the values by bin
   kPhRankExact = 9,  // exact rank inside the bin -> rank map + sorted values + num_pos
-  kPhFit = 10,       // per-segment Gram-polynomial least squares on the sorted values
+  kPhFit = 10,       // per-segment Gram-polynomial least squares on the sorted values ('dexp': per sign run, fp64)
   kPhFix = 11,       // residual <- value - fitted value (error feedback sees the fit error)
   kPhPush = 12,      // copy the finished slot into every peer's arena (P2P stores over NVLink); the CTA that finishes last
                      // (ticket) releases the flags — no grid barrier between the copy and the signal

@@ -10,6 +10,7 @@ side stream; ``finish()`` makes the optimizer's stream wait on the done events.
 
 CUDA + ('topk' [+ 'index': 'bloom' | plain])  -> fused engine (one kernel/bucket)
 CUDA + 'both' + 'rle' + 'fused_rle_values'    -> fused engine, value codec over the run-length index
+CUDA + 'dexp' values + 'fused_dexp'           -> fused engine, double-exponential values (plain, bloom or rle index)
 CUDA + 'randomk' [+ QSGD values]              -> fused engine, values only on the wire (shared-seed index)
 CUDA + 'none'/'allreduce'                     -> dense NCCL all-reduce of the flat bucket
 anything else (CPU/gloo, other codecs)        -> GRACE-compatible per-tensor path
@@ -50,8 +51,10 @@ def _fused_supported(params: dict) -> bool:
     bitmask over the positives, a different wire from the reference's, where every receiver redraws the pick.
     'both' with the run-length index is fused only with ``'fused_rle_values': True``: without the key that dict keeps
     the per-tensor route it always had (and its checkpoint format).
-    Not fused: 'conflict_sets' without that key (per-tensor GPU kernel), host codecs (Huffman, Deflate, dexp, the
-    integer family), non-512 QSGD buckets."""
+    Double-exponential values ('dexp') are fused only with ``'fused_dexp': True``, for the same reason: 'value', or
+    'both' over the bloom or run-length index.
+    Not fused: 'conflict_sets' without that key (per-tensor GPU kernel), host codecs (Huffman, Deflate, the integer
+    family), dexp without 'fused_dexp', non-512 QSGD buckets."""
     if params.get('compressor') not in ('topk', 'threshold') or params.get('communicator', 'allgather') != 'allgather':
         return False
     dr = params.get('deepreduce', None)
@@ -65,17 +68,21 @@ def _fused_supported(params: dict) -> bool:
     value_ok = (params.get('value', 'polyfit') == 'polyfit'
                 or (params.get('value') == 'qsgd' and 1 <= int(params.get('quantum_num', 127)) <= 32767
                     and int(params.get('bucket_size', 512)) == 512))
+    # the same index rule whether the index is shipped ('both') or not ('value'), as the config check has it
+    index = params.get('index', 'bloom')
+    dexp_ok = (params.get('value') in ('dexp', 'double_exp') and params.get('fused_dexp') is True
+               and ((index == 'bloom' and pol_ok) or (index == 'rle' and policy != 'conflict_sets')))
     if dr == 'index' and params.get('index', 'bloom') == 'bloom':
         return pol_ok
     if dr == 'index' and params.get('index') == 'rle':
         return True                      # lossless tile-local run coding inside the fused kernel
     if dr == 'value':
-        return value_ok                  # coded values + plain indices
+        return value_ok or dexp_ok       # coded values + plain indices
     if dr == 'both' and params.get('index', 'bloom') == 'bloom':
-        return pol_ok and value_ok
+        return pol_ok and (value_ok or dexp_ok)
     if dr == 'both' and params.get('index') == 'rle':
         # the bloom policies do not apply to a lossless index; the fused plan refuses 'conflict_sets' outside bloom
-        return params.get('fused_rle_values') is True and value_ok and policy != 'conflict_sets'
+        return ((params.get('fused_rle_values') is True and value_ok) or dexp_ok) and policy != 'conflict_sets'
     return False
 
 
@@ -133,15 +140,19 @@ def plan_kwargs_from_params(params: dict) -> dict:
     """``params`` dict (the reference's ``--grace_config``) -> BucketPlan keyword arguments."""
     from ..codecs.bloom import canonical_policy
     dr = params.get('deepreduce')
+    v = params.get('value', 'polyfit')
     kw = dict(compress_ratio=params.get('compress_ratio', 0.01),
               index=(params.get('index', 'bloom') if dr in ('index', 'both') else None),
-              value=(params.get('value', 'polyfit') if dr in ('value', 'both') else None),
+              value=({'double_exp': 'dexp'}.get(v, v) if dr in ('value', 'both') else None),
               quantum_num=int(params.get('quantum_num', 127)),
               poly_degree=int(params.get('poly_degree', 5)),
               fpr=params.get('fpr', None),
               policy=canonical_policy(params.get('policy', 'leftmost')),
               min_numel=int(params.get('min_numel', spec.SMALL_TENSOR_NUMEL)),
               hint=bool(params.get('hint', True)))
+    if kw['value'] == 'dexp':
+        from ..codecs.dexp import MIN_NUMEL
+        kw['dexp_min_numel'] = int(params.get('dexp_min_numel', MIN_NUMEL))
     if params.get('compressor') == 'threshold':
         kw.update(sparsifier='threshold', threshold=float(params.get('threshold', 0.0)),
                   capacity_ratio=params.get('threshold_capacity', None))

@@ -33,7 +33,7 @@ import torch.distributed as dist
 from .. import spec
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
 from .plan import update_cta_speeds
-from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID,
+from .plan import (DEXP_COEF_WORDS, DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID,
                    SLOT_HEADER_WORDS, BucketPlan, rle_stream_words)
 
 (PH_ACCUM, PH_FALLBACK, PH_HIST2, PH_INSERT, PH_QUERY, PH_EMIT, PH_RANK_HIST, PH_RANK_SCAN, PH_RANK_SCATTER,
@@ -137,6 +137,41 @@ def conflict_sets_keep_oracle(tp, pos: torch.Tensor, pick_words: np.ndarray) -> 
     return head[torch.from_numpy(keep.astype(bool))]
 
 
+def dexp_runs_fit_oracle(desc: torch.Tensor, num_pos: int) -> torch.Tensor:
+    """'dexp' of the fused engine (vmode 3): the values in descending order split at num_pos (the positives) into two
+    runs, each fitted by ``codecs.dexp.double_exponential_fit`` (fp64) on its own abscissa (i + 1) / length: the
+    positives by ascending value, the rest by ascending magnitude.  Returns the shipped fp32 words
+    (a, b, p, q) of the positive run, then of the rest."""
+    from ..codecs.dexp import double_exponential_fit
+    desc = desc.detach().cpu().double()
+    runs = (desc[:num_pos].flip(0), -desc[num_pos:])
+    return torch.stack([c for y in runs for c in double_exponential_fit(y)]).float()
+
+
+def dexp_runs_eval_oracle(coef: torch.Tensor, num_pos: int, n: int) -> torch.Tensor:
+    """The fitted values of the n ranks (descending order) from the shipped fp32 words: fp64 evaluation
+    (``codecs.dexp.double_exponential_eval``), rounded to fp32, negated on the non-positive run."""
+    from ..codecs.dexp import double_exponential_eval
+    return torch.cat([double_exponential_eval(coef[:4], num_pos).flip(0),
+                      -double_exponential_eval(coef[4:], n - num_pos)])
+
+
+def _write_rank_map(tp, slot: np.ndarray, rank: torch.Tensor):
+    n = int(rank.numel())
+    if tp.rank_u32:
+        slot[tp.off_rankmap:tp.off_rankmap + n] = rank.numpy().astype(np.uint32)
+    else:
+        r16 = np.zeros(((n + 1) // 2) * 2, dtype=np.uint16)
+        r16[:n] = rank.numpy().astype(np.uint16)
+        slot[tp.off_rankmap:tp.off_rankmap + (n + 1) // 2] = r16.view(np.uint32)
+
+
+def _read_rank_map(t, a: np.ndarray, n: int) -> torch.Tensor:
+    if t.rank_u32:
+        return torch.from_numpy(a[t.off_rankmap:t.off_rankmap + n].astype(np.int64))
+    return torch.from_numpy(a[t.off_rankmap:t.off_rankmap + (n + 1) // 2].view(np.uint16)[:n].astype(np.int64))
+
+
 def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, policy: str, seed: int, epoch: int = 1):
     """Encode one tensor into `slot` (uint32 numpy view); returns new residual."""
     if tp.mode == MODE_SHARED:
@@ -208,7 +243,22 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
         slot[tp.off_idx:tp.off_idx + sel.numel()] = sel.cpu().numpy().astype(np.uint32)
         cutoff = int(sel[-1].item()) if n_pos >= limit else 0xFFFFFFFF
     vals = acc[sel].float()
-    if tp.vmode == 1:
+    if tp.vmode == 3:
+        # 'dexp': the same rank map as polyfit; one double-exponential curve per sign run
+        n = int(sel.numel())
+        order = torch.sort(vals, descending=True, stable=True).indices
+        rank = torch.empty(n, dtype=torch.int64)
+        rank[order] = torch.arange(n)
+        num_pos = int((vals > 0).sum())
+        coef = dexp_runs_fit_oracle(vals[order], num_pos)
+        fitted = dexp_runs_eval_oracle(coef, num_pos, n)[rank]
+        slot[tp.off_coef:tp.off_coef + DEXP_COEF_WORDS] = coef.numpy().view(np.uint32)
+        slot[tp.off_coef + DEXP_COEF_WORDS] = num_pos
+        slot[tp.off_coef + DEXP_COEF_WORDS + 1] = n
+        _write_rank_map(tp, slot, rank)
+        resid[sel] = vals - fitted
+        vals = fitted
+    elif tp.vmode == 1:
         # 'both': stable descending sort -> rank map; per-segment Gram fit; fitted values are what is shipped,
         # and the residual keeps (value - fitted)
         from ..codecs.polyfit import MAX_SEGMENTS, get_segments, polyfit_eval_oracle, polyfit_fit_oracle
@@ -224,12 +274,7 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
         slot[tp.off_coef:tp.off_coef + nc] = coef.numpy().view(np.uint32)
         slot[tp.off_coef + nc] = num_pos
         slot[tp.off_coef + nc + 1] = n
-        if tp.rank_u32:
-            slot[tp.off_rankmap:tp.off_rankmap + n] = rank.numpy().astype(np.uint32)
-        else:
-            r16 = np.zeros(((n + 1) // 2) * 2, dtype=np.uint16)
-            r16[:n] = rank.numpy().astype(np.uint16)
-            slot[tp.off_rankmap:tp.off_rankmap + (n + 1) // 2] = r16.view(np.uint32)
+        _write_rank_map(tp, slot, rank)
         resid[sel] = vals - fitted
         vals = fitted
     elif tp.vmode == 2:
@@ -305,11 +350,11 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
             coef = torch.from_numpy(a[t.off_coef:t.off_coef + nc].view(np.float32).copy())
             num_pos, n_fit = int(a[t.off_coef + nc]), int(a[t.off_coef + nc + 1])
             curve = polyfit_eval_oracle(coef, get_segments(n_fit, num_pos), t.poly_degree)
-            if t.rank_u32:
-                rank = a[t.off_rankmap:t.off_rankmap + n].astype(np.int64)
-            else:
-                rank = a[t.off_rankmap:t.off_rankmap + (n + 1) // 2].view(np.uint16)[:n].astype(np.int64)
-            vals = curve[torch.from_numpy(rank)]
+            vals = curve[_read_rank_map(t, a, n)]
+        elif t.vmode == 3:
+            coef = torch.from_numpy(a[t.off_coef:t.off_coef + DEXP_COEF_WORDS].view(np.float32).copy())
+            num_pos, n_fit = int(a[t.off_coef + DEXP_COEF_WORDS]), int(a[t.off_coef + DEXP_COEF_WORDS + 1])
+            vals = dexp_runs_eval_oracle(coef, num_pos, n_fit)[_read_rank_map(t, a, n)]
         elif t.vmode == 2:
             from ..codecs.qsgd import qsgd_decode_oracle
             norms = torch.from_numpy(a[t.off_coef:t.off_coef + (n + 511) // 512].view(np.float32).copy())
@@ -391,6 +436,8 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
         thr = float(np.array([thr_bits], dtype=np.uint32).view(np.float32)[0])
         if t.vmode == 1:
             vbytes = 4 * (22 * (t.poly_degree + 1) + 2) + (4 if t.rank_u32 else 2) * t.val_cap
+        elif t.vmode == 3:
+            vbytes = 4 * (DEXP_COEF_WORDS + 2) + (4 if t.rank_u32 else 2) * t.val_cap
         elif t.vmode == 2:
             vbytes = 4 * ((t.val_cap + 511) // 512) + t.val_cap * (2 if t.rank_u32 else 1)
         else:

@@ -17,6 +17,7 @@ import numpy as np
 import torch
 
 from .. import spec
+from ..codecs.dexp import MIN_NUMEL as DEXP_MIN_NUMEL
 
 MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED = 0, 1, 2, 3
 KEY_SPAN = 1 << 31                    # select keys are 31-bit
@@ -50,6 +51,7 @@ def update_cta_speeds(speeds, dur, gain: float = 0.8):
     out = np.clip(speeds * rel ** gain, 0.5, 2.0)
     return out / out.mean()
 MAX_POLY_K = 1 << 17      # the all-pairs rank pass is O(K^2): larger tensors keep fp32 values
+DEXP_COEF_WORDS = 8       # 'dexp': {a, b, p, q} of the positive run, then of the non-positive run (ops/csrc/plan.h)
 DESC_WORDS = 32
 RANK_BINS = 8192
 
@@ -178,10 +180,12 @@ class BucketPlan:
     max_hash: int = 16
     ks: Optional[Sequence[int]] = None    # explicit per-tensor K (overrides compress_ratio)
     hint: bool = True                     # ship the 1-bit-per-32-elements occupancy hint next to each bloom filter
-    value: Optional[str] = None           # None (fp32 values), 'polyfit' or 'qsgd' ('both': bloom or rle index + value codec)
+    value: Optional[str] = None           # None (fp32 values), 'polyfit', 'qsgd' or 'dexp' ('both': bloom or rle index +
+                                          # value codec)
     quantum_num: int = 127                # QSGD levels (int8 on the wire)
     poly_degree: int = 5
     poly_min_k: int = 512                 # tensors shipping fewer values keep them as fp32 (the fit header would be larger)
+    dexp_min_numel: int = DEXP_MIN_NUMEL  # 'dexp' fits tensors of more elements than this (the per-tensor codec's rule)
     sparsifier: str = "topk"              # 'topk' (radix select of the K largest) | 'threshold' (|x| > threshold, variable K)
                                           # | 'randomk' (seeded index draw every rank repeats: only values are shipped)
     threshold: float = 0.0
@@ -193,16 +197,16 @@ class BucketPlan:
     def __post_init__(self):
         if self.index not in (None, "bloom", "rle"):
             raise ValueError(f"fused engine index codecs: None, 'bloom', 'rle'; got {self.index!r}")
-        if self.value not in (None, "polyfit", "qsgd"):
-            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd'; got {self.value!r}")
+        if self.value not in (None, "polyfit", "qsgd", "dexp"):
+            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp'; got {self.value!r}")
         if self.sparsifier not in ("topk", "threshold", "randomk"):
             raise ValueError(f"fused engine sparsifiers: 'topk', 'threshold', 'randomk'; got {self.sparsifier!r}")
         shared = self.sparsifier == "randomk"
         if shared and self.index is not None:
             raise ValueError("'randomk' ships no index (every rank draws the same set): pass index=None")
-        if shared and self.value == "polyfit":
+        if shared and self.value in ("polyfit", "dexp"):
             # rank_bin centres the value bins on the selection threshold, which here is a hash, not a magnitude
-            raise NotImplementedError("'randomk' is fused with fp32 or QSGD values, not with 'polyfit'")
+            raise NotImplementedError(f"'randomk' is fused with fp32 or QSGD values, not with {self.value!r}")
         if self.value == "qsgd" and not (1 <= int(self.quantum_num) <= 32767):
             raise ValueError("quantum_num must be in [1, 32767]")
         fixed_thr = 0
@@ -311,11 +315,14 @@ class BucketPlan:
 
     def _value_region(self, tp: TensorPlan, word: int, scratch: list) -> int:
         """Lay out the value side of a tensor's slot region (fp32 values, or a value codec + sender-local scratch)."""
-        if self.value == "polyfit" and tp.k >= self.poly_min_k and tp.val_cap <= MAX_POLY_K:
-            tp.vmode = 1
+        poly = self.value == "polyfit" and tp.k >= self.poly_min_k
+        dexp = self.value == "dexp" and tp.numel > self.dexp_min_numel
+        if (poly or dexp) and tp.val_cap <= MAX_POLY_K:
+            # curve coefficients + {num_pos, n} | rank map of the shipped values in their descending order
+            tp.vmode = 1 if poly else 3
             tp.rank_u32 = int(tp.val_cap > 65536)
             tp.off_coef = word
-            word = _align(word + MAX_SEGMENTS * (tp.poly_degree + 1) + 2, 4)
+            word = _align(word + (MAX_SEGMENTS * (tp.poly_degree + 1) if poly else DEXP_COEF_WORDS) + 2, 4)
             tp.off_rankmap = word
             word = _align(word + (tp.val_cap if tp.rank_u32 else (tp.val_cap + 1) // 2), 4)
             scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap), (tp, "off_sorted", tp.val_cap)]
@@ -336,8 +343,9 @@ class BucketPlan:
         return word
 
     def poly_tables(self):
-        """(tensor ids with vmode==1, largest K first ; rank-phase tasks {tensor, first value of a 512-chunk})."""
-        ids = sorted([i for i, t in enumerate(self.tensors) if t.vmode == 1], key=lambda i: -self.tensors[i].val_cap)
+        """(tensor ids with a rank map (vmode 1 or 3), largest K first ; rank-phase tasks {tensor, first value of a
+        512-chunk})."""
+        ids = sorted([i for i, t in enumerate(self.tensors) if t.vmode in (1, 3)], key=lambda i: -self.tensors[i].val_cap)
         off = 0
         for o, i in enumerate(ids):
             self.tensors[i].poly_off, self.tensors[i].poly_ord = off, o
