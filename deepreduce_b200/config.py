@@ -18,7 +18,7 @@ from typing import Optional
 
 COMPRESSORS = ("none", "topk", "threshold", "randomk")
 OUT_OF_SCOPE_COMPRESSORS = ("SKCompressCPU", "SKCompressGPU", "sketch")        # comparison baselines of a GRACE fork
-MEMORIES = ("none", "residual")
+MEMORIES = ("none", "residual", "dgc")
 COMMUNICATORS = ("allgather", "allreduce")
 MODES = (None, "value", "index", "both")
 POLICIES = ("leftmost", "leftmostK", "random", "randomK", "p0", "policy_zero", "conflict_sets", "p2")
@@ -30,7 +30,7 @@ KNOWN_KEYS = frozenset({
     "policy", "sort", "poly_degree", "quantum_num", "bucket_size", "micro-benchmark", "world_size", "average",
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
-    "p2_pick_mask", "fused_rle_values", "fused_dexp",
+    "p2_pick_mask", "fused_rle_values", "fused_dexp", "momentum", "gradient_clipping",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -93,6 +93,23 @@ class DeepReduceConfig:
             world_size=None if g("world_size", None) is None else int(g("world_size")),
             hint=bool(g("hint", True)), min_numel=int(g("min_numel", 1000)))
         cfg.validate()
+        # 'dgc' memory (momentum correction + momentum factor masking, Lin et al. 2018): the momentum factor rides in
+        # 'momentum'; it replaces the optimizer's momentum, and the residual it keeps is the plain one (beta = gamma = 1)
+        if "momentum" in params:
+            m = params["momentum"]
+            if cfg.memory != "dgc":
+                raise ConfigError(f"'momentum' applies to 'memory': 'dgc' (got memory={cfg.memory!r})")
+            if isinstance(m, bool) or not isinstance(m, (int, float)) or not 0.0 <= float(m) < 1.0:
+                raise ConfigError(f"'momentum' must be a number in [0, 1) (got {m!r})")
+        if cfg.memory == "dgc":
+            if cfg.compressor == "none":
+                raise ConfigError("'memory': 'dgc' needs a sparsifier: set 'compressor' to topk/threshold/randomk")
+            if cfg.beta != 1.0 or cfg.gamma != 1.0:
+                raise ConfigError(f"'memory': 'dgc' keeps the residual with beta = gamma = 1 (got beta={cfg.beta}, "
+                                  f"gamma={cfg.gamma})")
+        # GRACE's DGC clips each gradient by a norm reduced across ranks; not supported
+        if g("gradient_clipping", False) not in (False, None):
+            raise ConfigError("'gradient_clipping' is not supported; clip the gradients before the exchange instead")
         # opt-in wire of the fused engine's conflict_sets policy: the sender ships its pick as a bitmask over the positives
         p2 = g("p2_pick_mask", False)
         if not isinstance(p2, bool):

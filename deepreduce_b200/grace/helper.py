@@ -7,7 +7,7 @@ from typing import Iterable
 import torch
 
 from .communicators import Allgather, Allreduce
-from .memory import NoneMemory, ResidualMemory
+from .memory import DgcMemory, NoneMemory, ResidualMemory
 from .sparsifiers import NoneCompressor, RandomKCompressor, ThresholdCompressor, TopKCompressor
 
 _BITS = {torch.float64: 64, torch.int64: 64, torch.float32: 32, torch.int32: 32,
@@ -52,6 +52,8 @@ def grace_from_params(params: dict):
 
     if mem == 'residual':
         memory = ResidualMemory(params.get('beta', 1.0), params.get('gamma', 1.0))
+    elif mem == 'dgc':
+        memory = DgcMemory(params.get('momentum', 0.9))
     elif mem in ('none', None):
         memory = NoneMemory()
     else:

@@ -4,6 +4,11 @@
 ``update: r <- g - decompress(compress(g))`` (SURVEY §2.5; TF twin in
 reference tensorflow/deepreduce.py:31-52).  Unlike GRACE the residual state is
 checkpointable (``state_dict``), see SURVEY §5.
+
+``DgcMemory``: momentum correction and momentum factor masking of Deep Gradient
+Compression (Lin et al., ICLR 2018; GRACE's DGC memory without its gradient
+clipping).  The momentum is accumulated locally, before the selection, and cleared
+wherever this rank's own decoded contribution is non-zero.
 """
 from __future__ import annotations
 
@@ -44,5 +49,52 @@ class ResidualMemory(Memory):
     def load_state_dict(self, state, device=None):
         self.beta = state.get("beta", self.beta)
         self.gamma = state.get("gamma", self.gamma)
+        self.residuals = {k: (v.to(device) if device is not None else v.clone())
+                          for k, v in state.get("residuals", {}).items()}
+
+
+class DgcMemory(Memory):
+    """Per tensor, with ``m = momentum``::
+
+        u <- fl(fl(m * u) + g)          # two roundings, never a fused multiply-add
+        v <- fl(v + u)                  # v: the residual, as ResidualMemory with beta = gamma = 1
+        ... v is selected, encoded and shipped ...
+        v <- v - own(v)                 # own(v): what the receivers rebuild from this rank's message
+        u[i] <- 0 where own(v)[i] != 0  # momentum factor masking (-0.0 counts as zero)
+
+    A tensor not seen before starts with ``u = v = g`` (no additions, so ``-0.0`` stays intact).  With ``m = 0`` and
+    finite gradients it computes bit for bit what ``ResidualMemory()`` computes.  The momentum lives here, so the
+    optimizer that follows must not add its own (e.g. ``SGD(momentum=0)``)."""
+
+    def __init__(self, momentum: float = 0.9):
+        self.momentum = float(momentum)
+        self.momenta: dict[str, torch.Tensor] = {}
+        self.residuals: dict[str, torch.Tensor] = {}
+
+    def compensate(self, tensor, name):
+        if name in self.momenta:
+            u = self.momentum * self.momenta[name] + tensor
+            tensor = self.residuals[name] + u
+        else:
+            u = tensor
+        self.momenta[name] = u
+        return tensor
+
+    def update(self, tensor, name, compressor, tensor_compressed, ctx):
+        own = compressor.decompress(tensor_compressed, ctx).view_as(tensor)
+        self.residuals[name] = tensor - own
+        u = self.momenta[name]
+        self.momenta[name] = torch.where(own != 0, torch.zeros_like(u), u)
+
+    def state_dict(self):
+        return {"momentum": self.momentum,
+                "momenta": {k: v.detach().cpu().clone() for k, v in self.momenta.items()},
+                "residuals": {k: v.detach().cpu().clone() for k, v in self.residuals.items()}}
+
+    def load_state_dict(self, state, device=None):
+        if "momenta" not in state:
+            raise ValueError("not a 'dgc' memory state (no 'momenta'): it was saved with another memory")
+        self.momentum = state.get("momentum", self.momentum)
+        self.momenta = {k: (v.to(device) if device is not None else v.clone()) for k, v in state["momenta"].items()}
         self.residuals = {k: (v.to(device) if device is not None else v.clone())
                           for k, v in state.get("residuals", {}).items()}

@@ -624,6 +624,12 @@ struct Engine {
     P.grad = reinterpret_cast<float*>(grad); P.resid = reinterpret_cast<float*>(resid);
   }
 
+  // 'dgc' memory: the fp32 momentum buffer (same element layout as the residual) and the momentum factor; 0 = none
+  // (the residual memory's kernels)
+  void set_momentum(int64_t mom, double momentum) {
+    P.mom = reinterpret_cast<float*>(mom); P.momentum = (float)momentum;
+  }
+
   int get_grid() {
     if (grid == 0) grid = dr::engine_max_grid(blocks_per_sm, dyn_smem);
     return grid;
@@ -849,6 +855,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                     int64_t, int64_t, int64_t, std::vector<int64_t>, int, int>())
       .def("configure", &Engine::configure)
       .def("set_buffers", &Engine::set_buffers)
+      .def("set_momentum", &Engine::set_momentum)
       .def("set_bf16", &Engine::set_bf16)
       .def("set_poly", &Engine::set_poly)
       .def("set_shard", &Engine::set_shard)

@@ -385,7 +385,12 @@ DR_D uint32_t round16(uint32_t bytes) { return (bytes + 15u) & ~15u; }
 // kB = true    : bf16 bucket.  The g half of a stage holds the bf16 half-tile (4 KB, the rest of its 8 KB unused, so the
 //               ring arithmetic is the same), each thread widens its 8 bytes in registers and zero-fills its 8 bytes of
 //               the bf16 output; the rows of acc32 that the apply of this step adds into are zeroed here too.
-template <bool kTma, bool kFull, bool kB>
+// kDgc = true  : 'dgc' memory.  Each thread reads its float4 of the momentum u with a direct streaming load, issued
+//               before it waits for the ring so that the load overlaps the wait, and writes u back the same way.  u
+//               is not staged through the ring: the stage size, the ring depth and the shared-memory budget stay
+//               the same as the existing variants', so u costs no ring space and no extra TMA bookkeeping, and each
+//               element of u is read by exactly the thread that uses it.
+template <bool kTma, bool kFull, bool kB, bool kDgc>
 DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t parity_slot = P.epoch & 1u;
@@ -506,6 +511,11 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
         const uint32_t off = (uint32_t)h * kHalf;
         uint32_t key4[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};   // 0xFFFFFFFF = not an element
         if (off < ti.n) {                                                  // CTA-uniform
+          float4 u_old = zero4;
+          if constexpr (kDgc) {
+            const uint32_t e0 = off + tid * 4u;
+            if (e0 < ti.n) u_old = __ldcs(reinterpret_cast<const float4*>(P.mom + ti.base + e0));
+          }
           if (kTma) {
             // refill first: the stage consumed one item ago is free as soon as every warp released it
             if (tid == kProducer && !first_item && p_tile < t_end) {
@@ -532,7 +542,15 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
             if constexpr (kB) g = widen_bf16x4(reinterpret_cast<const uint2*>(sg)[tid]);
             else g = sg[tid];
             float4 a;
-            if (has_resid) {
+            if constexpr (kDgc) {                                          // two roundings each: no contracted FMA
+              const float mu = P.momentum;
+              float4 u;
+              u.x = __fadd_rn(__fmul_rn(mu, u_old.x), g.x); u.y = __fadd_rn(__fmul_rn(mu, u_old.y), g.y);
+              u.z = __fadd_rn(__fmul_rn(mu, u_old.z), g.z); u.w = __fadd_rn(__fmul_rn(mu, u_old.w), g.w);
+              __stcs(reinterpret_cast<float4*>(P.mom + ti.base + e0), u);
+              const float4 r = sr[tid];
+              a.x = __fadd_rn(r.x, u.x); a.y = __fadd_rn(r.y, u.y); a.z = __fadd_rn(r.z, u.z); a.w = __fadd_rn(r.w, u.w);
+            } else if (has_resid) {
               const float4 r = sr[tid];
               a.x = beta * r.x + gamma * g.x; a.y = beta * r.y + gamma * g.y;
               a.z = beta * r.z + gamma * g.z; a.w = beta * r.w + gamma * g.w;
@@ -1103,7 +1121,7 @@ DR_D void policy_filter(const EngineParams& P, Smem& sm) {
   }
 }
 
-template <bool kFull, bool kB>
+template <bool kFull, bool kB, bool kDgc>
 DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t parity = P.epoch & 1u;
@@ -1213,6 +1231,8 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
             const uint32_t rp = excl + base + q;
             vals[rp] = v;
             P.resid[gi] = 0.0f;                                            // residual is exactly 0 on the shipped set
+            // momentum factor masking where the own decoded value is this fp32 value (coded values: phase_fix)
+            if constexpr (kDgc) { if (vmode == 0u && v != 0.0f) P.mom[gi] = 0.0f; }
             if (scatter) put_out<kB>(P, gi, v * P.scale);
             if (mode == (uint32_t)kModeRaw) idxs[rp] = ti.local0 + e;
             else if (kFull && mode == (uint32_t)kModeRle) rle_put(idxs, rp, e);
@@ -1524,6 +1544,8 @@ DR_D void phase_fit(const EngineParams& P, Smem& sm) {
 }
 
 // phase 11: error feedback sees the fit error: resid[idx_p] = value_p - fitted_p
+// (kDgc: and the momentum of idx_p is cleared when the decoded value, the one every receiver rebuilds, is non-zero)
+template <bool kDgc>
 DR_D void phase_fix(const EngineParams& P, Smem& sm) {
   const uint32_t parity = P.epoch & 1u;
   uint32_t* my_slot = slot_ptr(P.arena[P.rank], P, parity, P.rank);
@@ -1558,6 +1580,7 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
         if (sm.td.rank_u32) reinterpret_cast<int16_t*>(my_slot + sm.td.off_rankmap)[p] = (int16_t)l;   // quantum_num >= 128
         else reinterpret_cast<int8_t*>(my_slot + sm.td.off_rankmap)[p] = (int8_t)l;
         P.resid[__ldcg(my_slot + sm.td.off_selidx + p)] = v - norm / q * l;
+        if constexpr (kDgc) { if (__fmul_rn(norm / q, l) != 0.0f) P.mom[__ldcg(my_slot + sm.td.off_selidx + p)] = 0.0f; }
       }
       continue;
     }
@@ -1575,6 +1598,7 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
       const float fitted = dexp ? dexp_value(coef, num_pos, n, rank) : poly_value(coef, sm.seg_start, sm.n_seg, deg, rank);
       const float v = __ldcg(reinterpret_cast<const float*>(my_slot + sm.td.off_vals) + p);
       P.resid[__ldcg(my_slot + sm.td.off_selidx + p)] = v - fitted;
+      if constexpr (kDgc) { if (fitted != 0.0f) P.mom[__ldcg(my_slot + sm.td.off_selidx + p)] = 0.0f; }
     }
   }
 }
@@ -2187,7 +2211,7 @@ DR_D bool phase_active(const EngineParams& P, int ph) {
   }
 }
 
-template <int kMinBlocks, bool kFull, bool kB>
+template <int kMinBlocks, bool kFull, bool kB, bool kDgc = false>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const __grid_constant__ EngineParams P) {
   __shared__ Smem sm;
   if (threadIdx.x == 0) {
@@ -2218,18 +2242,18 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
       }
     }
     switch (ph) {
-      case kPhAccum: if (P.use_tma) phase_accum<true, kFull, kB>(P, sm); else phase_accum<false, kFull, kB>(P, sm); break;
+      case kPhAccum: if (P.use_tma) phase_accum<true, kFull, kB, kDgc>(P, sm); else phase_accum<false, kFull, kB, kDgc>(P, sm); break;
       case kPhFallback: phase_fallback<kFull>(P, sm); break;
       case kPhHist2: phase_hist2(P, sm); break;
       case kPhInsert: phase_insert(P, sm); break;
       case kPhQuery: phase_query(P, sm); break;
-      case kPhEmit: phase_emit<kFull, kB>(P, sm, bar_epoch); break;
+      case kPhEmit: phase_emit<kFull, kB, kDgc>(P, sm, bar_epoch); break;
       case kPhRankHist: if constexpr (kFull) phase_rank_hist(P, sm); break;
       case kPhRankScan: if constexpr (kFull) phase_rank_scan(P, sm); break;
       case kPhRankScatter: if constexpr (kFull) phase_rank_scatter(P, sm); break;
       case kPhRankExact: if constexpr (kFull) phase_rank_exact(P, sm); break;
       case kPhFit: if constexpr (kFull) phase_fit(P, sm); break;
-      case kPhFix: if constexpr (kFull) phase_fix(P, sm); break;
+      case kPhFix: if constexpr (kFull) phase_fix<kDgc>(P, sm); break;
       case kPhExpand: if constexpr (kFull) phase_expand(P, sm); break;
       case kPhPush: phase_push(P, sm); break;
       case kPhSignal: if (!wait_flags<kB>(P, 0u, 0u)) return; break;
@@ -2269,6 +2293,13 @@ static const void* kernel_for(int blocks_per_sm, bool full, bool bf16) {
   return full ? (const void*)dr_engine_kernel<1, true, false> : (const void*)dr_engine_kernel<1, false, false>;
 }
 
+// ... and the 'dgc' memory (momentum correction + factor masking): the full feature set only, fp32 or bf16 buckets, a
+// separate instantiation again, so that the eight kernels above are compiled from unchanged code
+static const void* dgc_kernel_for(int blocks_per_sm, bool bf16) {
+  if (blocks_per_sm >= 2) return bf16 ? (const void*)dr_engine_kernel<2, true, true, true> : (const void*)dr_engine_kernel<2, true, false, true>;
+  return bf16 ? (const void*)dr_engine_kernel<1, true, true, true> : (const void*)dr_engine_kernel<1, true, false, true>;
+}
+
 static void ensure_attr() {
   if (!g_attr_set) {
     for (int bf16 = 0; bf16 < 2; ++bf16) {
@@ -2276,6 +2307,8 @@ static void ensure_attr() {
         cudaFuncSetAttribute(kernel_for(1, full, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         cudaFuncSetAttribute(kernel_for(2, full, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
       }
+      cudaFuncSetAttribute(dgc_kernel_for(1, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+      cudaFuncSetAttribute(dgc_kernel_for(2, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
     }
     g_attr_set = true;
   }
@@ -2292,6 +2325,11 @@ int engine_max_grid(int blocks_per_sm, int dyn_smem_bytes) {
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kernel_for(blocks_per_sm, v & 1, v >> 1), kThreads, (size_t)dyn_smem_bytes);
     if (o < occ) occ = o;
   }
+  for (int bf16 = 0; bf16 < 2; ++bf16) {
+    int o = 0;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, dgc_kernel_for(blocks_per_sm, bf16), kThreads, (size_t)dyn_smem_bytes);
+    if (o < occ) occ = o;
+  }
   if (occ < 1) occ = 1;
   if (blocks_per_sm > 0 && blocks_per_sm < occ) occ = blocks_per_sm;
   return occ * sms;
@@ -2306,8 +2344,9 @@ cudaError_t engine_launch(const EngineParams& P, int grid, int blocks_per_sm, in
   void* args[] = {const_cast<EngineParams*>(&P)};
   count_launch(1);
   const bool full = P.n_poly != 0 || P.n_poly_tasks != 0 || P.has_rle != 0 || P.has_shared != 0;
-  return cudaLaunchCooperativeKernel(kernel_for(blocks_per_sm, full, P.bf16 != 0), dim3(grid), dim3(kThreads), args,
-                                     (size_t)dyn_smem_bytes, stream);
+  const void* kernel = P.mom != nullptr ? dgc_kernel_for(blocks_per_sm, P.bf16 != 0)
+                                        : kernel_for(blocks_per_sm, full, P.bf16 != 0);
+  return cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kThreads), args, (size_t)dyn_smem_bytes, stream);
 }
 
 }  // namespace dr

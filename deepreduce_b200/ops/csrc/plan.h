@@ -122,7 +122,7 @@ constexpr uint32_t kArenaHdrWords = 128;
 // and the same 22-bit rule applies to it: a superset of the K smallest hashes, plus ~numel / 2^22 elements sharing the
 // threshold's prefix.  The set depends on (numel, K, epoch, salt) only, so every rank computes the same one.
 enum Phase : int {
-  kPhAccum = 0,      // r = beta*r + gamma*g ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
+  kPhAccum = 0,      // r = beta*r + gamma*g (dgc: u = m*u + g, r = r + u) ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
   kPhFallback = 1,   // (only if some bound was unsafe) digit 1 redone without the bound, candidate lists rebuilt in full
   kPhHist2 = 2,      // digit 2 of the candidate keys in the threshold bin
   kPhInsert = 3,     // selected candidates -> bloom filter + occupancy hint (bloom) / positive masks (raw, rle)
@@ -229,6 +229,11 @@ struct EngineParams {
                                  // in the accumulate phase for the bloom tiles that are applied
   uint32_t acc_tiles;            // rows of acc32 (0: no tensor needs the apply)
   int bf16;
+  // 'dgc' memory (mom != nullptr, the <.., true, .., true> kernels; beta = gamma = 1): momentum correction before the
+  // select, u = fl(fl(momentum * u) + g) and r = fl(r + u), and momentum factor masking, u = 0 wherever this rank's
+  // own decoded contribution is non-zero (emit for fp32 values, fix for coded values)
+  float* mom;                    // [total elements] fp32 momentum u (persists across steps)
+  float momentum;
 };
 
 // Slot and slice layout, shared by the kernel and the host that launches it (binding.cpp)

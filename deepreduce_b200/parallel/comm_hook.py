@@ -17,7 +17,8 @@ DDP packs a bucket's gradients back to back, unpadded, at arbitrary offsets; the
 segment table, built the first time the hook meets it; ``bucket_pack`` / ``bucket_unpack`` (``ops/csrc/repack.cu``)
 move the whole bucket in one launch each way.  DDP rebuilds its buckets after the first iteration, so a run meets two
 layouts: the residual of every parameter is carried from the old engine into the new one (DESIGN.md, "DDP
-communication hook").
+communication hook"), and with ``'memory': 'dgc'`` its momentum too.  That memory holds the momentum, so the optimizer
+stepping the DDP model must run without one (e.g. ``torch.optim.SGD(..., momentum=0)``).
 """
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -80,6 +81,11 @@ class _Layout:
         i = self.slot[id(p)]
         return self.engine.resid[self.eng_off[i]:self.eng_off[i] + self.segments[i][1]]
 
+    def mom_of(self, p) -> torch.Tensor:
+        """The parameter's 'dgc' momentum in this engine (same place as its residual)."""
+        i = self.slot[id(p)]
+        return self.engine.mom[self.eng_off[i]:self.eng_off[i] + self.segments[i][1]]
+
 
 # ---------------------------------------------------------------------------
 # state + hook
@@ -111,6 +117,8 @@ class DeepReduceHookState:
         self._by_index: Dict[int, _Layout] = {}      # the layout a bucket index had last
         self._owner: Dict[int, _Layout] = {}         # id(parameter) -> the layout holding its residual
         self._pending: Dict[str, torch.Tensor] = {}  # loaded residuals of parameters no engine holds yet
+        self._pending_mom: Dict[str, torch.Tensor] = {}  # ... and their loaded 'dgc' momenta
+        self.dgc = self.params.get('memory') == 'dgc'
         self._pending_epoch = 0
         self._stream: Optional[torch.cuda.Stream] = None
         self.grc = None
@@ -232,11 +240,16 @@ class DeepReduceHookState:
             old = self._owner.get(id(p))
             if old is not None:
                 dst.copy_(old.resid_of(p))
+                if self.dgc:
+                    lay.mom_of(p).copy_(old.mom_of(p))
                 old.live -= 1
                 if old.live == 0:
                     self._close_layout(old)
-            elif n in self._pending:
-                dst.copy_(self._pending.pop(n).to(dst.device, torch.float32).reshape(-1))
+            else:
+                if n in self._pending:
+                    dst.copy_(self._pending.pop(n).to(dst.device, torch.float32).reshape(-1))
+                if self.dgc and n in self._pending_mom:
+                    lay.mom_of(p).copy_(self._pending_mom.pop(n).to(dst.device, torch.float32).reshape(-1))
             self._owner[id(p)] = lay
         eng.epoch = max(eng.epoch, self._pending_epoch)
         self._by_index[index] = lay
@@ -311,16 +324,22 @@ class DeepReduceHookState:
     # ---- checkpoint / resume ----------------------------------------------------------
     def state_dict(self) -> dict:
         """Keyed by parameter name, so that a checkpoint loads into a run with other buckets: the residual of every
-        parameter (fused path, flat in storage order) or the GRACE memory (per-tensor path)."""
+        parameter (fused path, flat in storage order; with 'dgc' its momentum too, under ``"momentum"``) or the GRACE
+        memory (per-tensor path)."""
         if self._layouts:
             torch.cuda.synchronize(self._layouts[0].engine.device)
         resid = {n: t.clone() for n, t in self._pending.items()}
+        mom = {n: t.clone() for n, t in self._pending_mom.items()}
         for lay in self._layouts:
             for p, n in zip(lay.params, lay.names):
                 if self._owner.get(id(p)) is lay:
                     resid[n] = lay.resid_of(p).detach().cpu().clone()
+                    if self.dgc:
+                        mom[n] = lay.mom_of(p).detach().cpu().clone()
         out = {"step": self.step_count, "residuals": resid,
                "epoch": max([self._pending_epoch] + [e.epoch for e in self.engines])}
+        if self.dgc:
+            out["momentum"] = mom
         if self.grc is not None:
             out["memory"] = self.grc.memory.state_dict()
         return out
@@ -336,14 +355,18 @@ class DeepReduceHookState:
             for p, n in zip(lay.params, lay.names):
                 if self._owner.get(id(p)) is lay:
                     by_name[n] = lay
-        self._pending = {}
-        for n, t in state.get("residuals", {}).items():
-            lay = by_name.get(n)
-            if lay is None:
-                self._pending[n] = t.detach().cpu().clone()
-            else:
-                p = next(q for q, m in zip(lay.params, lay.names) if m == n)
-                lay.resid_of(p).copy_(t.to(lay.engine.device, torch.float32).reshape(-1))
+        if self.dgc != ("momentum" in state) and state.get("residuals"):
+            raise ValueError("hook state of another memory: 'dgc' states carry a 'momentum' map, other states do not")
+        self._pending, self._pending_mom = {}, {}
+        for key, pending, view in (("residuals", self._pending, _Layout.resid_of),
+                                   ("momentum", self._pending_mom, _Layout.mom_of)):
+            for n, t in state.get(key, {}).items():
+                lay = by_name.get(n)
+                if lay is None:
+                    pending[n] = t.detach().cpu().clone()
+                else:
+                    p = next(q for q, m in zip(lay.params, lay.names) if m == n)
+                    view(lay, p).copy_(t.to(lay.engine.device, torch.float32).reshape(-1))
         if "memory" in state:
             if self.grc is None:
                 from ..wrappers import deepreduce_from_params

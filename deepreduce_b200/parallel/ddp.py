@@ -176,13 +176,14 @@ def engine_split_numel(params: dict, blocks_per_sm: int) -> int:
 
 def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: bool, blocks_per_sm: int,
                 grad_dtype: torch.dtype) -> BucketEngine:
-    """The ``BucketEngine`` of one bucket for ``params`` (residual memory, beta / gamma, averaging), with its tile
-    partitions calibrated unless ``'calibrate_partition': False``.  Collective at W > 1."""
-    residual = params.get('memory', 'none') == 'residual'
+    """The ``BucketEngine`` of one bucket for ``params`` (residual or 'dgc' memory, beta / gamma, momentum, averaging),
+    with its tile partitions calibrated unless ``'calibrate_partition': False``.  Collective at W > 1."""
+    memory = params.get('memory', 'none')
     eng = BucketEngine(plan, device=device, group=group,
-                       beta=float(params.get('beta', 1.0)) if residual else 0.0,
+                       beta=float(params.get('beta', 1.0)) if memory in ('residual', 'dgc') else 0.0,
                        gamma=float(params.get('gamma', 1.0)), average=params.get('average', True),
-                       use_history=use_history, blocks_per_sm=blocks_per_sm, grad_dtype=grad_dtype)
+                       use_history=use_history, blocks_per_sm=blocks_per_sm, grad_dtype=grad_dtype,
+                       momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None)
     # re-cut the kernel's tile partitions from measured per-CTA phase times (collective; ~12 exchange steps
     # on synthetic gradients, state reset afterwards) — 'calibrate_partition': False keeps the static cut
     if params.get('calibrate_partition', True) and eng.cuts is not None:
@@ -194,6 +195,8 @@ def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: b
             eng.cta_speeds = None
             eng._set_cuts()
             eng.resid.zero_(); eng.sel.zero_(); eng.grad.zero_()
+            if eng.mom is not None:
+                eng.mom.zero_()
     return eng
 
 

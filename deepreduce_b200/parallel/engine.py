@@ -306,16 +306,27 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
 
 
 def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Sequence[torch.Tensor], *, beta=1.0,
-                  gamma=1.0, average=True, seed=spec.DEFAULT_SEED, epoch=1):
+                  gamma=1.0, average=True, seed=spec.DEFAULT_SEED, epoch=1, momentum=None, moms=None):
     """One bucket step for W ranks on the CPU.  grads/resids: per-rank flat
-    buffers (plan.total_elems).  Returns (dense_out, new_resids, slots)."""
+    buffers (plan.total_elems).  Returns (dense_out, new_resids, slots).
+
+    ``momentum`` set ('dgc' memory, beta = gamma = 1): ``moms`` are the per-rank momenta u, the step is
+    u = momentum * u + g, r = r + u (each a separately rounded fp32 op) before the select, and u is cleared wherever
+    the rank's own decoded value is non-zero; returns (dense_out, new_resids, slots, new_moms)."""
     W = len(grads)
+    dgc = momentum is not None
+    if dgc and (beta != 1.0 or gamma != 1.0 or moms is None or len(moms) != W):
+        raise ValueError("engine_oracle: momentum needs beta = gamma = 1 and one momentum buffer per rank")
     out = torch.zeros(plan.total_elems, dtype=torch.float32)
-    new_resids, slots = [], []
+    new_resids, slots, new_moms = [], [], []
     for r in range(W):
         g = grads[r].detach().cpu().float()
         res = resids[r].detach().cpu().float()
-        acc_flat = beta * res + gamma * g if beta != 0.0 else gamma * g
+        if dgc:
+            u = float(momentum) * moms[r].detach().cpu().float() + g
+            acc_flat = res + u
+        else:
+            acc_flat = beta * res + gamma * g if beta != 0.0 else gamma * g
         slot = np.zeros(plan.payload_words, dtype=np.uint32)
         slot[0:5] = [MAGIC, epoch, len(plan.tensors), plan.payload_words, r]
         nres = acc_flat.clone()
@@ -324,10 +335,16 @@ def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Seque
             resid_t, sel, vals = encode_tensor_oracle(tp, acc_flat[seg], slot, ti, plan.policy, seed, epoch)
             nres[seg] = resid_t
             out[seg].index_add_(0, sel, vals)
+            if dgc:                                  # momentum factor masking on the own decoded contribution
+                u[seg][sel[vals != 0]] = 0.0
         new_resids.append(nres)
         slots.append(slot)
+        if dgc:
+            new_moms.append(u)
     if average:
         out = out / W
+    if dgc:
+        return out, new_resids, slots, new_moms
     return out, new_resids, slots
 
 
@@ -486,13 +503,20 @@ class BucketEngine:
                  seed: int = spec.DEFAULT_SEED, spin_limit: int = 20_000_000, world: Optional[int] = None,
                  rank: Optional[int] = None, filter_smem_bytes: Optional[int] = None, use_tma: bool = True,
                  hist_shift: int = 22, shard: Optional[bool] = None, transport: Optional[str] = None,
-                 peer_timeout_ms: Optional[int] = None, fault: int = 0, grad_dtype: torch.dtype = torch.float32):
+                 peer_timeout_ms: Optional[int] = None, fault: int = 0, grad_dtype: torch.dtype = torch.float32,
+                 momentum: Optional[float] = None):
         # grad_dtype=torch.bfloat16: the flat gradient (in: local, out: aggregate) is bf16.  The residual, the select,
         # the codecs and the wire stay fp32 (widening bf16 is exact), so the engine computes exactly what an fp32 engine
         # fed the widened gradient computes, and rounds the aggregate once (to nearest even) where it is final.  The
         # rounding error is not fed back into the residual, as torch's bf16 DDP does with its reduced sum.
         if grad_dtype not in (torch.float32, torch.bfloat16):
             raise ValueError(f"grad_dtype must be torch.float32 or torch.bfloat16 (got {grad_dtype})")
+        # momentum=m: the 'dgc' memory.  An fp32 momentum buffer ``mom`` next to the residual: u = m*u + g, r = r + u
+        # before the select, u cleared wherever this rank's own decoded value is non-zero (engine_oracle)
+        if momentum is not None and (float(beta) != 1.0 or float(gamma) != 1.0 or not 0.0 <= float(momentum) < 1.0):
+            raise ValueError(f"momentum needs beta = gamma = 1 and a value in [0, 1) (got beta={beta}, gamma={gamma}, "
+                             f"momentum={momentum})")
+        self.momentum = None if momentum is None else float(momentum)
         from .. import ops
         self.mod = ops.cuda_module()
         self.plan = plan
@@ -519,6 +543,8 @@ class BucketEngine:
         with torch.cuda.device(dev):
             self.grad = torch.zeros(plan.total_elems, dtype=grad_dtype, device=dev)
             self.resid = torch.zeros(plan.total_elems, dtype=torch.float32, device=dev)
+            self.mom = (torch.zeros(plan.total_elems, dtype=torch.float32, device=dev) if self.momentum is not None
+                        else None)
             self.tensor_table = plan.tensor_table().to(dev)
             self.tile_table = plan.tile_table().to(dev)
             self.hist = torch.zeros(NUM_HIST * nT * HIST_BINS, dtype=torch.int32, device=dev)
@@ -554,6 +580,8 @@ class BucketEngine:
             self.cuts = None
             self.ctx.set_scratch(self.pos_mask.data_ptr(), self.dec_mask.data_ptr(), self.cand.data_ptr(),
                                  self.cand_cnt.data_ptr())
+            if self.mom is not None:
+                self.ctx.set_momentum(self.mom.data_ptr(), self.momentum)
             if grad_dtype == torch.bfloat16:
                 # fp32 sums of the bloom apply (every sender of a tile is added before the one rounding): one 4096-float
                 # row per tile this rank decodes; not needed when every bloom tensor is scattered by emit (W = 1, fp32
@@ -624,7 +652,7 @@ class BucketEngine:
         slower in accumulate and query), and every phase ends at a grid barrier, i.e. lasts
         as long as its slowest CTA.  Collective at W > 1 (runs ``(rounds + 1) * (steps + 1)`` exchange steps).  Resets
         residual / select history / gradient afterwards; the step counter keeps running (flags are epoch-valued).
-        Returns the per-round phase maxima / medians."""
+        Resets the momentum of a 'dgc' engine too.  Returns the per-round phase maxima / medians."""
         G = self.grid()
         dbg = torch.zeros((PH_END + 1) * G * 2, dtype=torch.int64, device=self.device)
         self.ctx.set_debug_times(dbg.data_ptr())
@@ -658,6 +686,8 @@ class BucketEngine:
         finally:
             self.ctx.set_debug_times(0)
         self.resid.zero_(); self.sel.zero_(); self.grad.zero_()
+        if self.mom is not None:
+            self.mom.zero_()
         return log
 
     # ---- arena -------------------------------------------------------------
@@ -819,11 +849,19 @@ class BucketEngine:
 
     # ---- state (checkpoint / resume; SURVEY §5) ----------------------------
     def state_dict(self):
-        return {"resid": self.resid.detach().cpu().clone(), "epoch": self.epoch,
-                "sel": self.sel.detach().cpu().clone()}
+        out = {"resid": self.resid.detach().cpu().clone(), "epoch": self.epoch,
+               "sel": self.sel.detach().cpu().clone()}
+        if self.mom is not None:
+            out["mom"] = self.mom.detach().cpu().clone()
+        return out
 
     def load_state_dict(self, state):
+        if ("mom" in state) != (self.mom is not None):
+            raise ValueError("engine state of another memory: a 'dgc' engine loads only 'dgc' states (with 'mom'), "
+                             "any other engine only states without it")
         self.resid.copy_(state["resid"].to(self.device))
+        if self.mom is not None:
+            self.mom.copy_(state["mom"].to(self.device))
         self.sel.copy_(state["sel"].to(self.device))
         # never move the step counter backwards inside a live process group: the peers' flags in the arena carry
         # epochs this engine has already used (e.g. during calibrate_partition)

@@ -38,6 +38,10 @@ class Trainer:
                                  background_thread=background_thread, blocks_per_sm=blocks_per_sm,
                                  overlap_grid=overlap_grid)
         if optimizer is None:
+            # 'memory': 'dgc' accumulates the momentum before the exchange (momentum correction): the optimizer then
+            # runs without one, whatever ``momentum`` says.  A user optimizer must do the same.
+            if params.get('memory') == 'dgc':
+                momentum = 0.0
             kw = dict(lr=lr, momentum=momentum, weight_decay=weight_decay)
             if self.is_cuda:
                 kw["fused"] = True
