@@ -1,6 +1,7 @@
 """Sparse codecs + registry (reference pytorch/deepreduce.py:913-922)."""
 from .base import SparseCompressor, compressor, register
 from . import bitpack
+from .bf16 import BF16
 from .bloom import Bloom, Bloomfilter, get_BFconfig
 from .bloom_cpu import BloomCPU, bloom_compress_blob, bloom_decompress_blob
 from .dexp import DoubleExp
@@ -10,6 +11,6 @@ from .polyfit import PolyFit, PolyFitCPU, get_segments
 from .qsgd import QSGD
 from .rle import RunLength
 
-__all__ = ["SparseCompressor", "compressor", "register", "bitpack", "Bloom", "Bloomfilter", "get_BFconfig",
+__all__ = ["SparseCompressor", "compressor", "register", "bitpack", "BF16", "Bloom", "Bloomfilter", "get_BFconfig",
            "BloomCPU", "bloom_compress_blob", "bloom_decompress_blob", "DoubleExp", "IntegerIndex", "Gzip",
            "Huffman", "PolyFit", "PolyFitCPU", "get_segments", "QSGD", "RunLength"]

@@ -554,7 +554,7 @@ struct Engine {
     P.spin_limit = 20u * 1000u * 1000u;
     P.filter_smem_words = (uint32_t)(dyn_smem / 4);
     P.use_tma = 1; P.hist_shift = 23;
-    P.shard = 0; P.s2_words = 0; P.s2_cap = 0; P.has_rle = 0; P.has_shared = 0; P.mc_arena = nullptr;
+    P.shard = 0; P.s2_words = 0; P.s2_cap = 0; P.has_rle = 0; P.has_shared = 0; P.has_bf16_values = 0; P.mc_arena = nullptr;
     P.peer_timeout_ms = 120000u; P.fault = 0; P.debug_times = nullptr; P.cost_prefix = nullptr; P.deterministic = 0; P.cuts = nullptr; P.cuts_grid = 0;
     cudaGetDevice(&device);
   }
@@ -592,6 +592,7 @@ struct Engine {
 
   void set_has_rle(int v) { P.has_rle = v; }
   void set_has_shared(int v) { P.has_shared = v; }
+  void set_has_bf16_values(int v) { P.has_bf16_values = v; }
   // scratch of the candidate / bitmask pipeline (see engine.cu): masks [n_tiles*128] u32 x2, candidate keys
   // entries [n_tiles*4096] x {u32 key, u32 offset}, counts [n_tiles*16] u32
   void set_scratch(int64_t pos_mask, int64_t dec_mask, int64_t cand, int64_t cand_cnt) {
@@ -862,6 +863,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("set_has_rle", &Engine::set_has_rle)
       .def("set_p2", &Engine::set_p2)
       .def("set_has_shared", &Engine::set_has_shared)
+      .def("set_has_bf16_values", &Engine::set_has_bf16_values)
       .def("set_scratch", &Engine::set_scratch)
       .def("set_peer_timeout_ms", &Engine::set_peer_timeout_ms)
       .def("set_fault", &Engine::set_fault)

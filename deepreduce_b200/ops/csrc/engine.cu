@@ -129,8 +129,14 @@ DR_D float4 widen_bf16x4(uint2 h) {
                      __uint_as_float(h.y & 0xFFFF0000u));
 }
 
+// round to nearest even (a finite value past the largest bf16 becomes +-inf), every NaN to the quiet NaN 0x7FC0
+DR_D uint32_t bf16_rne_bits(float v) {
+  const uint32_t u = __float_as_uint(v);
+  return (u & 0x7FFFFFFFu) > 0x7F800000u ? 0x7FC0u : (u + 0x7FFFu + ((u >> 16) & 1u)) >> 16;
+}
+
 // bf16 buckets whose bloom tensor is applied by phase_compact (every sender added into acc32, then rounded): all of them
-// except where emit already scattered the rank's own values (W == 1, fp32 values)
+// except where emit already scattered the rank's own values (W == 1, fp32 values; bf16 values too, see phase_accum)
 DR_D bool bloom_applied(const EngineParams& P, uint32_t mode, uint32_t vmode) {
   return mode == (uint32_t)kModeBloom && !(P.world == 1 && vmode == 0u);
 }
@@ -483,6 +489,9 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
     const uint32_t mode = __ldg(&tdp->mode), fixed = __ldg(&tdp->fixed_thr);
     bool zero_acc = false;                                                 // bf16: this tensor's rows of acc32 start from 0
     if constexpr (kB) zero_acc = bloom_applied(P, mode, __ldg(&tdp->vmode));
+    // bf16 values at W == 1: emit scatters them, as it does fp32 values, and decode and compact do not run (they run at
+    // W == 1 only for the fix phase's value codecs), so no acc32 row is applied
+    if constexpr (kFull && kB) zero_acc = zero_acc && !(P.world == 1 && __ldg(&tdp->vmode) == kVmodeBf16);
     // 'randomk' (full kernel only): the keys are hashes of the element index (CTA-uniform per tensor), the candidate
     // bound is static
     const bool shared = kFull && (mode == (uint32_t)kModeShared);
@@ -1229,6 +1238,23 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           auto put = [&](bool have, uint32_t q, uint32_t e, size_t gi, float v) {
             if (!have) return;
             const uint32_t rp = excl + base + q;
+            if constexpr (kFull) {
+              if (vmode == kVmodeBf16) {
+                // bf16 values: v rounded goes on the wire and its rounding error, exact, stays in the residual (0
+                // where the rounded value is not finite, as for fp32 values).  dec is what every receiver adds into
+                // its zero-filled output, so a value that rounds to -0.0 lands as +0.0 here too.
+                const uint32_t h = bf16_rne_bits(v);
+                reinterpret_cast<uint16_t*>(vals)[rp] = (uint16_t)h;
+                const float w = __uint_as_float(h << 16), dec = __fadd_rn(w, 0.0f);
+                P.resid[gi] = isfinite(w) ? __fsub_rn(v, w) : 0.0f;
+                if constexpr (kDgc) { if (dec != 0.0f) P.mom[gi] = 0.0f; }
+                if (P.world == 1) put_out<kB>(P, gi, dec * P.scale);
+                if (mode == (uint32_t)kModeRaw) idxs[rp] = ti.local0 + e;
+                else if (mode == (uint32_t)kModeRle) rle_put(idxs, rp, e);
+                if (rp == limit - 1u) dyn->cutoff = ti.local0 + e;
+                return;
+              }
+            }
             vals[rp] = v;
             P.resid[gi] = 0.0f;                                            // residual is exactly 0 on the shipped set
             // momentum factor masking where the own decoded value is this fp32 value (coded values: phase_fix)
@@ -1706,6 +1732,9 @@ DR_D bool wait_flags(const EngineParams& P, uint32_t base, uint32_t aux_base) {
 template <bool kFull>
 DR_D float coded_value(const uint32_t* slot, const TensorDesc& td, const float* vals, const float* fitted, uint32_t rp) {
   if (kFull && ranked(td.vmode)) return __ldcg(fitted + load_rank(slot, td, rp));
+  if constexpr (kFull) {
+    if (td.vmode == kVmodeBf16) return __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const uint16_t*>(vals) + rp) << 16);
+  }
   if (kFull && td.vmode == 2u) {
     const float norm = __ldcg(reinterpret_cast<const float*>(slot + td.off_coef) + (rp >> 9));
     const float lvl = td.rank_u32 ? (float)__ldcg(reinterpret_cast<const int16_t*>(slot + td.off_rankmap) + rp)
@@ -2281,9 +2310,10 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
 // filter staging; <2> = 64 regs, two CTAs per SM, up to 88 KB each.
 static bool g_attr_set = false;
 
-// ... x two feature sets: <.., false, ..> index-only (plain pairs / bloom), <.., true, ..> + value codecs, run-length
-// index and the shared 'randomk' index; ... x the gradient type: <.., .., false> fp32 buckets, <.., .., true> bf16 buckets
-// (a separate instantiation, so the fp32 kernels are compiled from exactly the code they had before bf16 existed)
+// ... x two feature sets: <.., false, ..> index-only (plain pairs / bloom), <.., true, ..> + value codecs (bf16 values
+// included), run-length index and the shared 'randomk' index; ... x the gradient type: <.., .., false> fp32 buckets,
+// <.., .., true> bf16 buckets (a separate instantiation, so the fp32 kernels are compiled from exactly the code they had
+// before bf16 existed)
 static const void* kernel_for(int blocks_per_sm, bool full, bool bf16) {
   if (bf16) {
     if (blocks_per_sm >= 2) return full ? (const void*)dr_engine_kernel<2, true, true> : (const void*)dr_engine_kernel<2, false, true>;
@@ -2343,7 +2373,7 @@ cudaError_t engine_launch(const EngineParams& P, int grid, int blocks_per_sm, in
   if (e != cudaSuccess) return e;
   void* args[] = {const_cast<EngineParams*>(&P)};
   count_launch(1);
-  const bool full = P.n_poly != 0 || P.n_poly_tasks != 0 || P.has_rle != 0 || P.has_shared != 0;
+  const bool full = P.n_poly != 0 || P.n_poly_tasks != 0 || P.has_rle != 0 || P.has_shared != 0 || P.has_bf16_values != 0;
   const void* kernel = P.mom != nullptr ? dgc_kernel_for(blocks_per_sm, P.bf16 != 0)
                                         : kernel_for(blocks_per_sm, full, P.bf16 != 0);
   return cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kThreads), args, (size_t)dyn_smem_bytes, stream);

@@ -54,7 +54,9 @@ struct TensorDesc {
   // ---- value codec ('both': bloom index + polynomial fit of the values) ----
   uint32_t vmode;        // 0 = fp32 values on the wire, 1 = piece-wise Gram-polynomial fit + rank map,
                          // 2 = bucketed QSGD (int8 levels, or int16 when rank_u32 is set: quantum_num >= 128),
-                         // 3 = double-exponential fit of each sign run + rank map
+                         // 3 = double-exponential fit of each sign run + rank map,
+                         // 4 = bf16 values: the p-th value's bits in half p % 2 (low half first) of word off_vals + p / 2,
+                         //     rounded by emit, which also writes the residual (no scratch, no rank / fit / fix phase)
   uint32_t off_coef;     // [kMaxSeg * (deg+1)] (vmode 3: [kDexpCoefWords]) float coefficients, then {num_pos, n}
   uint32_t off_rankmap;  // rank of the p-th shipped value in the descending sort (u16 if val_cap <= 65536 else u32)
   uint32_t off_selidx;   // scratch (not shipped): element index of the p-th shipped value
@@ -77,6 +79,7 @@ constexpr int kRankBins = 8192;        // 'both': counting-sort bins = sign + 8 
 constexpr int kMaxSeg = 22;            // codecs/polyfit.py MAX_SEGMENTS
 constexpr int kMaxDeg = 7;
 constexpr uint32_t kDexpCoefWords = 8;  // vmode 3: {a, b, p, q} of the positive run, then of the non-positive run
+constexpr uint32_t kVmodeBf16 = 4;      // TensorDesc::vmode of bf16 values
 
 // payload slot layout (uint32 words):
 //   [0..8)                      : magic, epoch, n_tensors, payload_words, rank, 0,0,0
@@ -234,6 +237,7 @@ struct EngineParams {
   // own decoded contribution is non-zero (emit for fp32 values, fix for coded values)
   float* mom;                    // [total elements] fp32 momentum u (persists across steps)
   float momentum;
+  int has_bf16_values;           // some tensor ships bf16 values (vmode 4: only the <.., true> kernels carry that path)
 };
 
 // Slot and slice layout, shared by the kernel and the host that launches it (binding.cpp)

@@ -33,8 +33,8 @@ import torch.distributed as dist
 from .. import spec
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
 from .plan import update_cta_speeds
-from .plan import (DEXP_COEF_WORDS, DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID,
-                   SLOT_HEADER_WORDS, BucketPlan, rle_stream_words)
+from .plan import (DEXP_COEF_WORDS, DYN_WORDS, EMIT_DECODES, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST,
+                   POLICY_ID, SLOT_HEADER_WORDS, BucketPlan, rle_stream_words)
 
 (PH_ACCUM, PH_FALLBACK, PH_HIST2, PH_INSERT, PH_QUERY, PH_EMIT, PH_RANK_HIST, PH_RANK_SCAN, PH_RANK_SCATTER,
  PH_RANK_EXACT, PH_FIT, PH_FIX, PH_PUSH, PH_SIGNAL, PH_EXPAND, PH_DECODE, PH_COMPACT, PH_PUSH2, PH_SIGNAL2,
@@ -295,6 +295,18 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
             slot[tp.off_rankmap:tp.off_rankmap + (n + 3) // 4] = l8.view(np.uint32)
         resid[sel] = vals - dec
         vals = dec
+    elif tp.vmode == 4:
+        # bf16 values (round to nearest even, NaN -> 0x7FC0), two per word; the residual keeps the exact rounding error
+        # where the widened value is finite, and is 0 (as for fp32 values) where it is not
+        from ..codecs.bf16 import bf16_bits_oracle, bf16_widen_oracle
+        n = int(sel.numel())
+        q = np.zeros(((n + 1) // 2) * 2, dtype=np.uint16)
+        bits = bf16_bits_oracle(vals)
+        q[:n] = bits.numpy().astype(np.uint16)
+        slot[tp.off_vals:tp.off_vals + (n + 1) // 2] = q.view(np.uint32)
+        dec = bf16_widen_oracle(bits)
+        resid[sel] = torch.where(torch.isfinite(dec), vals - dec, torch.zeros_like(dec))
+        vals = dec
     else:
         slot[tp.off_vals:tp.off_vals + sel.numel()] = vals.cpu().numpy().view(np.uint32)
         resid[sel] = 0
@@ -380,6 +392,10 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
             else:
                 lvl = torch.from_numpy(a[t.off_rankmap:t.off_rankmap + (n + 3) // 4].view(np.int8)[:n].astype(np.int64))
             vals = qsgd_decode_oracle(lvl, norms, int(t.poly_degree), 512)
+        elif t.vmode == 4:
+            from ..codecs.bf16 import bf16_widen_oracle
+            bits = a[t.off_vals:t.off_vals + (n + 1) // 2].view(np.uint16)[:n].astype(np.int64)
+            vals = bf16_widen_oracle(torch.from_numpy(bits))
         else:
             vals = torch.from_numpy(a[t.off_vals:t.off_vals + n].view(np.float32).copy())
         out[t.elem_off:t.elem_off + t.numel].index_add_(0, idx, vals.float())
@@ -457,6 +473,8 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
             vbytes = 4 * (DEXP_COEF_WORDS + 2) + (4 if t.rank_u32 else 2) * t.val_cap
         elif t.vmode == 2:
             vbytes = 4 * ((t.val_cap + 511) // 512) + t.val_cap * (2 if t.rank_u32 else 1)
+        elif t.vmode == 4:
+            vbytes = 2 * t.val_cap
         else:
             vbytes = 4 * t.val_cap
         if t.mode == MODE_BLOOM:
@@ -585,8 +603,9 @@ class BucketEngine:
             if grad_dtype == torch.bfloat16:
                 # fp32 sums of the bloom apply (every sender of a tile is added before the one rounding): one 4096-float
                 # row per tile this rank decodes; not needed when every bloom tensor is scattered by emit (W = 1, fp32
-                # values on the wire)
-                applied = any(t.mode == MODE_BLOOM and not (self.world == 1 and t.vmode == 0) for t in plan.tensors)
+                # or bf16 values on the wire: emit knows the decoded value)
+                applied = any(t.mode == MODE_BLOOM and not (self.world == 1 and t.vmode in EMIT_DECODES)
+                              for t in plan.tensors)
                 acc_tiles = span_max if applied else 0
                 self.acc32 = torch.zeros(max(acc_tiles, 1) * 4096, dtype=torch.float32, device=dev)
                 self.ctx.set_bf16(self.grad.data_ptr(), self.acc32.data_ptr(), acc_tiles)
@@ -619,6 +638,7 @@ class BucketEngine:
             if n_p2:
                 self.ctx.set_p2(self.p2_table.data_ptr(), n_p2, self.p2_scratch.data_ptr(), p2_cap)
             self.ctx.set_has_shared(int(any(t.mode == MODE_SHARED for t in plan.tensors)))
+            self.ctx.set_has_bf16_values(int(any(t.vmode == 4 for t in plan.tensors)))
             ids, n_poly, tasks, n_tasks = plan.poly_tables()
             self.poly_ids, self.poly_tasks = ids.to(dev), tasks.to(dev)
             from .plan import RANK_BINS

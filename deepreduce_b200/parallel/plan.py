@@ -52,6 +52,7 @@ def update_cta_speeds(speeds, dur, gain: float = 0.8):
     return out / out.mean()
 MAX_POLY_K = 1 << 17      # the all-pairs rank pass is O(K^2): larger tensors keep fp32 values
 DEXP_COEF_WORDS = 8       # 'dexp': {a, b, p, q} of the positive run, then of the non-positive run (ops/csrc/plan.h)
+EMIT_DECODES = (0, 4)     # vmodes whose decoded value emit knows (fp32, bf16): at W = 1 it scatters them itself
 DESC_WORDS = 32
 RANK_BINS = 8192
 
@@ -180,8 +181,8 @@ class BucketPlan:
     max_hash: int = 16
     ks: Optional[Sequence[int]] = None    # explicit per-tensor K (overrides compress_ratio)
     hint: bool = True                     # ship the 1-bit-per-32-elements occupancy hint next to each bloom filter
-    value: Optional[str] = None           # None (fp32 values), 'polyfit', 'qsgd' or 'dexp' ('both': bloom or rle index +
-                                          # value codec)
+    value: Optional[str] = None           # None (fp32 values), 'polyfit', 'qsgd', 'dexp' or 'bf16' ('both': bloom or rle
+                                          # index + value codec)
     quantum_num: int = 127                # QSGD levels (int8 on the wire)
     poly_degree: int = 5
     poly_min_k: int = 512                 # tensors shipping fewer values keep them as fp32 (the fit header would be larger)
@@ -197,8 +198,8 @@ class BucketPlan:
     def __post_init__(self):
         if self.index not in (None, "bloom", "rle"):
             raise ValueError(f"fused engine index codecs: None, 'bloom', 'rle'; got {self.index!r}")
-        if self.value not in (None, "polyfit", "qsgd", "dexp"):
-            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp'; got {self.value!r}")
+        if self.value not in (None, "polyfit", "qsgd", "dexp", "bf16"):
+            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp', 'bf16'; got {self.value!r}")
         if self.sparsifier not in ("topk", "threshold", "randomk"):
             raise ValueError(f"fused engine sparsifiers: 'topk', 'threshold', 'randomk'; got {self.sparsifier!r}")
         shared = self.sparsifier == "randomk"
@@ -206,7 +207,7 @@ class BucketPlan:
             raise ValueError("'randomk' ships no index (every rank draws the same set): pass index=None")
         if shared and self.value in ("polyfit", "dexp"):
             # rank_bin centres the value bins on the selection threshold, which here is a hash, not a magnitude
-            raise NotImplementedError(f"'randomk' is fused with fp32 or QSGD values, not with {self.value!r}")
+            raise NotImplementedError(f"'randomk' is fused with fp32, QSGD or bf16 values, not with {self.value!r}")
         if self.value == "qsgd" and not (1 <= int(self.quantum_num) <= 32767):
             raise ValueError("quantum_num must be in [1, 32767]")
         fixed_thr = 0
@@ -337,6 +338,12 @@ class BucketPlan:
             tp.off_rankmap = word                        # levels
             word = _align(word + ((tp.val_cap + 1) // 2 if tp.rank_u32 else (tp.val_cap + 3) // 4), 4)
             scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap)]
+        elif self.value == "bf16":
+            # bf16 values, two per word (the p-th value in the low half of word p // 2): emit rounds them as it gathers
+            # and knows the decoded value, so there is no sender scratch and no later phase
+            tp.vmode = 4
+            tp.off_vals = word
+            word = _align(word + (tp.val_cap + 1) // 2, 4)
         else:
             tp.off_vals = word
             word = _align(word + tp.val_cap, 4)
@@ -351,8 +358,10 @@ class BucketPlan:
             self.tensors[i].poly_off, self.tensors[i].poly_ord = off, o
             off += self.tensors[i].val_cap
         self.poly_total = off
-        coded = sorted([i for i, t in enumerate(self.tensors) if t.vmode != 0], key=lambda i: -self.tensors[i].val_cap)
-        tasks = [(i, c) for i in coded for c in range(0, self.tensors[i].val_cap, 512)]      # all value-coded tensors
+        # the fix phase's tensors: every value codec but bf16 (vmode 4), whose residual emit writes
+        coded = sorted([i for i, t in enumerate(self.tensors) if t.vmode in (1, 2, 3)],
+                       key=lambda i: -self.tensors[i].val_cap)
+        tasks = [(i, c) for i in coded for c in range(0, self.tensors[i].val_cap, 512)]
         ids_t = torch.tensor(ids if ids else [0], dtype=torch.int32)
         tasks_t = torch.tensor(tasks if tasks else [(0, 0)], dtype=torch.int32).reshape(-1)
         return ids_t, len(ids), tasks_t, len(tasks)

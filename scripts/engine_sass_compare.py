@@ -74,12 +74,14 @@ def main() -> int:
         head = kernels(os.path.join(ROOT, CSRC), work, "head")
     ok = True
     for args, code in sorted(base.items()):
-        match = [c for a, c in head.items() if a[:3] == args and all(x == "false" for x in a[3:])]
+        n = len(args)                # 3 or 4 template arguments, depending on the base
+        match = [c for a, c in head.items() if a[:n] == args and all(x == "false" for x in a[n:])]
         same = bool(match) and match[0] == code
         ok &= same
         print(f"dr_engine_kernel<{', '.join(args)}>: {code.count(chr(10)) + 1} lines, "
               f"{'identical' if same else 'DIFFERENT' if match else 'MISSING in the working tree'}")
-    for args in sorted(a for a in head if a[:3] not in base or any(x != "false" for x in a[3:])):
+    n = len(next(iter(base))) if base else 3
+    for args in sorted(a for a in head if a[:n] not in base or any(x != "false" for x in a[n:])):
         print(f"dr_engine_kernel<{', '.join(args)}>: new variant ({head[args].count(chr(10)) + 1} lines)")
     print("all base variants identical" if ok else "SASS differs")
     return 0 if ok else 1
