@@ -560,9 +560,14 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
               const float4 r = sr[tid];
               a.x = __fadd_rn(r.x, u.x); a.y = __fadd_rn(r.y, u.y); a.z = __fadd_rn(r.z, u.z); a.w = __fadd_rn(r.w, u.w);
             } else if (has_resid) {
+              // fl(fl(beta * r) + fl(gamma * g)): three roundings, as ResidualMemory and engine_oracle make them in
+              // torch.  Left to itself nvcc fuses one product into an FFMA (here gamma * g), which changes a and the
+              // residual wherever that factor is not 0 or a power of two
               const float4 r = sr[tid];
-              a.x = beta * r.x + gamma * g.x; a.y = beta * r.y + gamma * g.y;
-              a.z = beta * r.z + gamma * g.z; a.w = beta * r.w + gamma * g.w;
+              a.x = __fadd_rn(__fmul_rn(beta, r.x), __fmul_rn(gamma, g.x));
+              a.y = __fadd_rn(__fmul_rn(beta, r.y), __fmul_rn(gamma, g.y));
+              a.z = __fadd_rn(__fmul_rn(beta, r.z), __fmul_rn(gamma, g.z));
+              a.w = __fadd_rn(__fmul_rn(beta, r.w), __fmul_rn(gamma, g.w));
             } else {
               a.x = gamma * g.x; a.y = gamma * g.y; a.z = gamma * g.z; a.w = gamma * g.w;
             }

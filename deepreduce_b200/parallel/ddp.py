@@ -179,16 +179,23 @@ def engine_split_numel(params: dict, blocks_per_sm: int) -> int:
     return int(sn or 0)
 
 
+def engine_kwargs(params: dict) -> dict:
+    """The ``BucketEngine`` memory arguments for ``params``: beta, gamma, momentum and averaging.  They follow the
+    per-tensor memory GRACE builds for the same dict: only ``ResidualMemory`` scales the gradient by gamma, so
+    'none' and 'dgc' memory run with gamma = 1 ('dgc' accepts no other), and without a residual beta is 0."""
+    memory = params.get('memory', 'none')
+    return dict(beta=float(params.get('beta', 1.0)) if memory in ('residual', 'dgc') else 0.0,
+                gamma=float(params.get('gamma', 1.0)) if memory == 'residual' else 1.0,
+                average=params.get('average', True),
+                momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None)
+
+
 def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: bool, blocks_per_sm: int,
                 grad_dtype: torch.dtype) -> BucketEngine:
-    """The ``BucketEngine`` of one bucket for ``params`` (residual or 'dgc' memory, beta / gamma, momentum, averaging),
-    with its tile partitions calibrated unless ``'calibrate_partition': False``.  Collective at W > 1."""
-    memory = params.get('memory', 'none')
-    eng = BucketEngine(plan, device=device, group=group,
-                       beta=float(params.get('beta', 1.0)) if memory in ('residual', 'dgc') else 0.0,
-                       gamma=float(params.get('gamma', 1.0)), average=params.get('average', True),
-                       use_history=use_history, blocks_per_sm=blocks_per_sm, grad_dtype=grad_dtype,
-                       momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None)
+    """The ``BucketEngine`` of one bucket for ``params`` (memory arguments from ``engine_kwargs``), with its tile
+    partitions calibrated unless ``'calibrate_partition': False``.  Collective at W > 1."""
+    eng = BucketEngine(plan, device=device, group=group, use_history=use_history, blocks_per_sm=blocks_per_sm,
+                       grad_dtype=grad_dtype, **engine_kwargs(params))
     # re-cut the kernel's tile partitions from measured per-CTA phase times (collective; ~12 exchange steps
     # on synthetic gradients, state reset afterwards) — 'calibrate_partition': False keeps the static cut
     if params.get('calibrate_partition', True) and eng.cuts is not None:
