@@ -6,7 +6,7 @@ within half a bf16 ulp of fp32's largest finite value, and the relative error of
 (8 significant bits).  With a residual or 'dgc' memory the rounding error is not lost: ``v - widen(bf16(v))`` is
 exact in fp32, and the memories already keep ``v - decompress(compress(v))``.
 
-Wire: ``bfloat16[K]``.  The fused engine ships the same 16-bit words (``parallel/plan.py``, vmode 4); its kernel
+Wire: ``bfloat16[K]``.  The fused engine ships the same 16-bit words (``parallel/plan.py``, ``VMODE_BF16``); its kernel
 rounds a NaN to the quiet NaN 0x7FC0 (``bf16_bits_oracle``), where torch's own cast may give another NaN pattern.
 """
 from __future__ import annotations

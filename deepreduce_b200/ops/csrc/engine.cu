@@ -135,10 +135,13 @@ DR_D uint32_t bf16_rne_bits(float v) {
   return (u & 0x7FFFFFFFu) > 0x7F800000u ? 0x7FC0u : (u + 0x7FFFu + ((u >> 16) & 1u)) >> 16;
 }
 
-// bf16 buckets whose bloom tensor is applied by phase_compact (every sender added into acc32, then rounded): all of them
-// except where emit already scattered the rank's own values (W == 1, fp32 values; bf16 values too, see phase_accum)
+// at W == 1 emit has already scattered the tensor's decoded fp32 values into the output (bf16 values too: phase_accum).
+// phase_compact writes it out in its two skip tests, where the vmode load stays behind the short-circuit.
+DR_D bool emit_scatters(const EngineParams& P, uint32_t vmode) { return P.world == 1 && vmode == kVmodeFp32; }
+
+// bf16 buckets' bloom tensors that phase_compact applies (every sender added into acc32, then rounded once)
 DR_D bool bloom_applied(const EngineParams& P, uint32_t mode, uint32_t vmode) {
-  return mode == (uint32_t)kModeBloom && !(P.world == 1 && vmode == 0u);
+  return mode == (uint32_t)kModeBloom && !emit_scatters(P, vmode);
 }
 
 DR_D void load_tensor(const EngineParams& P, uint32_t t, Smem& sm) {
@@ -1194,7 +1197,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
     // ---- one warp per tile, tiles handed out dynamically (a tile's cost follows its number of positives)
     uint32_t cur = kNoTensor;
     uint32_t mode = 0, k = 0, val_cap = 0, off_vals = 0, off_idx = 0, off_prefix = 0, tile_begin = 0, n_tiles = 0,
-             vmode = 0, off_selidx = 0, thr = 0;
+             vmode = kVmodeFp32, off_selidx = 0, thr = 0;
     const uint32_t* hint = nullptr;
     uint16_t* list = reinterpret_cast<uint16_t*>(g_filter_smem) + warp * kListCap;
     while (true) {
@@ -1226,7 +1229,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
       DynHeader* dyn = reinterpret_cast<DynHeader*>(my_slot + kSlotHeaderWords) + cur;
       float* vals = reinterpret_cast<float*>(my_slot + off_vals);
       uint32_t* idxs = my_slot + off_idx;
-      const bool scatter = (P.world == 1) && (vmode == 0u);
+      const bool scatter = emit_scatters(P, vmode);
       const uint32_t n_emit = excl < limit ? min(total, limit - excl) : 0u;      // elements of this tile that are shipped
       for (uint32_t base = 0; base < n_emit; base += kListCap) {
         fill_list(list, mm, incl - c, base, lane);
@@ -1263,11 +1266,11 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
             vals[rp] = v;
             P.resid[gi] = 0.0f;                                            // residual is exactly 0 on the shipped set
             // momentum factor masking where the own decoded value is this fp32 value (coded values: phase_fix)
-            if constexpr (kDgc) { if (vmode == 0u && v != 0.0f) P.mom[gi] = 0.0f; }
+            if constexpr (kDgc) { if (vmode == kVmodeFp32 && v != 0.0f) P.mom[gi] = 0.0f; }
             if (scatter) put_out<kB>(P, gi, v * P.scale);
             if (mode == (uint32_t)kModeRaw) idxs[rp] = ti.local0 + e;
             else if (kFull && mode == (uint32_t)kModeRle) rle_put(idxs, rp, e);
-            if (kFull && vmode) my_slot[off_selidx + rp] = (uint32_t)gi;
+            if (kFull && vmode != kVmodeFp32) my_slot[off_selidx + rp] = (uint32_t)gi;
             if (rp == limit - 1u) dyn->cutoff = ti.local0 + e;
           };
           put(ha, qa, ea, ga, va);
@@ -1334,13 +1337,13 @@ DR_D float poly_value(const float* __restrict__ coef, const int* start, int n_se
   return acc;
 }
 
-// 'dexp' (vmode 3): two double-exponential curves per tensor, over the rank map's two sign runs.  Coefficient words
+// 'dexp' (kVmodeDexp): two double-exponential curves per tensor, over the rank map's two sign runs.  Coefficient words
 // (fp32): {a, b, p, q} of the positive run by ascending value, then {a, b, p, q} of the magnitudes of the rest (the
 // values <= 0) by ascending |v|; each on its own abscissa x_i = (i + 1) / run length.
-DR_D bool ranked(uint32_t vmode) { return vmode == 1u || vmode == 3u; }
+DR_D bool ranked(uint32_t vmode) { return vmode == kVmodePolyfit || vmode == kVmodeDexp; }
 
 // words before the {num_pos, n} tail of a ranked tensor's header
-DR_D uint32_t coef_words(uint32_t vmode, uint32_t deg) { return vmode == 3u ? kDexpCoefWords : kMaxSeg * (deg + 1u); }
+DR_D uint32_t coef_words(uint32_t vmode, uint32_t deg) { return vmode == kVmodeDexp ? kDexpCoefWords : kMaxSeg * (deg + 1u); }
 
 // fitted value of rank j (descending order) from the shipped fp32 words: the sender's residual and every receiver's
 // decode go through this one evaluation, in fp64 without contraction (the oracle's torch order), rounded once
@@ -1497,7 +1500,7 @@ DR_D void phase_fit(const EngineParams& P, Smem& sm) {
   for (uint32_t task = gw; task < P.n_poly * kMaxSeg; task += nw) {
     const uint32_t t = __ldg(P.poly_tensors + task / kMaxSeg), s = task % kMaxSeg;
     const TensorDesc* td = P.tensors + t;
-    if (__ldg(&td->vmode) != 1u) continue;
+    if (__ldg(&td->vmode) != kVmodePolyfit) continue;
     const uint32_t off_coef = __ldg(&td->off_coef), off_sorted = __ldg(&td->off_sorted);
     const int deg = (int)__ldg(&td->poly_degree);
     const uint32_t* tail = my_slot + off_coef + kMaxSeg * (deg + 1);
@@ -1558,7 +1561,7 @@ DR_D void phase_fit(const EngineParams& P, Smem& sm) {
   for (uint32_t task = blockIdx.x; task < 2u * P.n_poly; task += gridDim.x) {
     const uint32_t t = __ldg(P.poly_tensors + task / 2u), neg = task & 1u;
     const TensorDesc* td = P.tensors + t;
-    if (__ldg(&td->vmode) != 3u) continue;
+    if (__ldg(&td->vmode) != kVmodeDexp) continue;
     float* coef = reinterpret_cast<float*>(my_slot + __ldg(&td->off_coef));
     const uint32_t* tail = my_slot + __ldg(&td->off_coef) + kDexpCoefWords;
     const uint32_t num_pos = __ldcg(tail), n = __ldcg(tail + 1);
@@ -1583,7 +1586,7 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
   for (uint32_t task = blockIdx.x; task < P.n_poly_tasks; task += gridDim.x) {
     const uint32_t t = __ldg(P.poly_tasks + 2 * task), p0 = __ldg(P.poly_tasks + 2 * task + 1);
     load_tensor(P, t, sm);
-    if (sm.td.vmode == 2) {
+    if (sm.td.vmode == kVmodeQsgd) {
       // bucketed QSGD (reference QSGD, pytorch/deepreduce.py:849-907, which syncs the host once per bucket):
       // this CTA owns one 512-value bucket: L2 norm, stochastic rounding with a counter-based RNG, int8 level
       const DynHeader* dyn = reinterpret_cast<const DynHeader*>(my_slot + kSlotHeaderWords) + t;
@@ -1619,7 +1622,7 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
     const uint32_t* tail = my_slot + sm.td.off_coef + coef_words(sm.td.vmode, deg);
     const int num_pos = (int)__ldcg(tail), n = (int)__ldcg(tail + 1);
     if ((int)p0 >= n) continue;
-    const bool dexp = sm.td.vmode == 3u;
+    const bool dexp = sm.td.vmode == kVmodeDexp;
     if (threadIdx.x == 0 && !dexp) build_segments(n, num_pos, sm.seg_start, sm.n_seg);
     __syncthreads();
     const uint32_t p = p0 + threadIdx.x;
@@ -1648,7 +1651,7 @@ DR_D void phase_expand(const EngineParams& P, Smem& sm) {
     const uint32_t* tail = slot + sm.td.off_coef + coef_words(sm.td.vmode, deg);
     const int num_pos = (int)__ldcg(tail), n = (int)__ldcg(tail + 1);
     if ((int)j0 >= n) continue;
-    const bool dexp = sm.td.vmode == 3u;
+    const bool dexp = sm.td.vmode == kVmodeDexp;
     if (threadIdx.x == 0 && !dexp) build_segments(n, num_pos, sm.seg_start, sm.n_seg);
     __syncthreads();
     const uint32_t j = j0 + threadIdx.x;
@@ -1740,7 +1743,7 @@ DR_D float coded_value(const uint32_t* slot, const TensorDesc& td, const float* 
   if constexpr (kFull) {
     if (td.vmode == kVmodeBf16) return __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const uint16_t*>(vals) + rp) << 16);
   }
-  if (kFull && td.vmode == 2u) {
+  if (kFull && td.vmode == kVmodeQsgd) {
     const float norm = __ldcg(reinterpret_cast<const float*>(slot + td.off_coef) + (rp >> 9));
     const float lvl = td.rank_u32 ? (float)__ldcg(reinterpret_cast<const int16_t*>(slot + td.off_rankmap) + rp)
                                   : (float)__ldcg(reinterpret_cast<const int8_t*>(slot + td.off_rankmap) + rp);
@@ -1827,7 +1830,7 @@ DR_D void phase_decode(const EngineParams& P, Smem& sm) {
 
 constexpr uint32_t kS2Stage = 256;             // per-warp stage of the slice list: entries (index | value), flushed at > 128
 
-// debug timeline: sub-step stamps of the apply/compact phase go to the (otherwise unused at vmode 0) slots 6..9
+// debug timeline: sub-step stamps of the apply/compact phase go to the (otherwise unused at kVmodeFp32) slots 6..9
 DR_D void dbg_stamp(const EngineParams& P, int slot, int which) {
   if (P.debug_times && threadIdx.x == 0) P.debug_times[((size_t)slot * gridDim.x + blockIdx.x) * 2 + which] = globaltimer_ns();
 }
@@ -1915,7 +1918,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
     {  // filter-coded tensors (and everything emit already scattered at W == 1) are skipped without a CTA barrier
       const TensorDesc* tdp = P.tensors + t;
       const uint32_t seg_end0 = min(t_last, __ldg(&tdp->tile_begin) + __ldg(&tdp->n_tiles));
-      if (__ldg(&tdp->mode) == (uint32_t)kModeBloom || (P.world == 1 && __ldg(&tdp->vmode) == 0u)) { tile = seg_end0; continue; }
+      if (__ldg(&tdp->mode) == (uint32_t)kModeBloom || (P.world == 1 && __ldg(&tdp->vmode) == kVmodeFp32)) { tile = seg_end0; continue; }
     }
     load_tensor(P, t, sm);
     const uint32_t seg_end = min(t_last, sm.td.tile_begin + sm.td.n_tiles);
@@ -2111,7 +2114,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
   for (uint32_t tl = t_first + warp; tl < t_last; tl += kWarps) {
     const Tile ti = load_tile(P.tiles, tl);
     if (ti.tensor != cur) warp_tensor(ti.tensor);
-    const bool apply = !fast && td.mode == (uint32_t)kModeBloom && !(P.world == 1 && td.vmode == 0u);
+    const bool apply = !fast && td.mode == (uint32_t)kModeBloom && !(P.world == 1 && td.vmode == kVmodeFp32);
     if (apply) {
       const uint32_t tile_local = tl - td.tile_begin;
       for (int r = 0; r < P.world; ++r) {

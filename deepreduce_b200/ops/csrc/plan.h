@@ -29,6 +29,15 @@ enum TensorMode : uint32_t {
                     // only the values travel; off_prefix is sender-local scratch (per-tile exclusive prefix)
 };
 
+enum ValueMode : uint32_t {  // TensorDesc::vmode: how a tensor's values travel in the slot (parallel/plan.py VMODE_*)
+  kVmodeFp32 = 0,     // fp32 values
+  kVmodePolyfit = 1,  // piece-wise Gram-polynomial fit + rank map
+  kVmodeQsgd = 2,     // bucketed QSGD (int8 levels, or int16 when rank_u32 is set: quantum_num >= 128)
+  kVmodeDexp = 3,     // double-exponential fit of each sign run + rank map
+  kVmodeBf16 = 4,     // bf16 values: the p-th value's bits in half p % 2 (low half first) of word off_vals + p / 2,
+                      // rounded by emit, which also writes the residual (no scratch, no rank / fit / fix phase)
+};
+
 // kPolicyP2 ('conflict_sets', opt-in): the sender draws the pick over its positives and ships it as a bitmask (p2.cu);
 // the engine kernel itself treats it as leftmost on the thinned positives
 enum Policy : int { kPolicyLeftmost = 0, kPolicyRandom = 1, kPolicyP0 = 2, kPolicyP2 = 3 };
@@ -52,19 +61,15 @@ struct TensorDesc {
   uint32_t n_filter_words;
   uint32_t off_hint;     // 0 = none; else 4 words per tile: bit g set <=> 32-element group g holds a selected element
   // ---- value codec ('both': bloom index + polynomial fit of the values) ----
-  uint32_t vmode;        // 0 = fp32 values on the wire, 1 = piece-wise Gram-polynomial fit + rank map,
-                         // 2 = bucketed QSGD (int8 levels, or int16 when rank_u32 is set: quantum_num >= 128),
-                         // 3 = double-exponential fit of each sign run + rank map,
-                         // 4 = bf16 values: the p-th value's bits in half p % 2 (low half first) of word off_vals + p / 2,
-                         //     rounded by emit, which also writes the residual (no scratch, no rank / fit / fix phase)
-  uint32_t off_coef;     // [kMaxSeg * (deg+1)] (vmode 3: [kDexpCoefWords]) float coefficients, then {num_pos, n}
+  uint32_t vmode;        // ValueMode
+  uint32_t off_coef;     // [kMaxSeg * (deg+1)] (kVmodeDexp: [kDexpCoefWords]) float coefficients, then {num_pos, n}
   uint32_t off_rankmap;  // rank of the p-th shipped value in the descending sort (u16 if val_cap <= 65536 else u32)
   uint32_t off_selidx;   // scratch (not shipped): element index of the p-th shipped value
   uint32_t off_sorted;   // scratch (not shipped): values in descending order
   uint32_t poly_degree;
   uint32_t rank_u32;     // 1: rank map entries are 32-bit
   uint32_t poly_off;     // offset of this tensor's values in the engine's per-value scratch arrays
-  uint32_t poly_ord;     // ordinal among the vmode==1 tensors (selects its bin table)
+  uint32_t poly_ord;     // ordinal among the ranked (kVmodePolyfit, kVmodeDexp) tensors (selects its bin table)
   uint32_t fixed_thr;    // != 0: 'threshold' sparsifier — select key >= fixed_thr (31-bit |x| pattern), no radix select, variable K
   uint32_t shared_lb;    // kModeShared: static candidate bound on the hash key (multiple of 512; replaces the history bound)
   // ---- P2 ('conflict_sets') bloom tensors; 0 otherwise ----
@@ -78,8 +83,7 @@ constexpr int kDescWords = 32;
 constexpr int kRankBins = 8192;        // 'both': counting-sort bins = sign + 8 exponent + 4 mantissa bits
 constexpr int kMaxSeg = 22;            // codecs/polyfit.py MAX_SEGMENTS
 constexpr int kMaxDeg = 7;
-constexpr uint32_t kDexpCoefWords = 8;  // vmode 3: {a, b, p, q} of the positive run, then of the non-positive run
-constexpr uint32_t kVmodeBf16 = 4;      // TensorDesc::vmode of bf16 values
+constexpr uint32_t kDexpCoefWords = 8;  // kVmodeDexp: {a, b, p, q} of the positive run, then of the non-positive run
 
 // payload slot layout (uint32 words):
 //   [0..8)                      : magic, epoch, n_tensors, payload_words, rank, 0,0,0
@@ -198,7 +202,7 @@ struct EngineParams {
   uint32_t filter_smem_words;    // capacity of the dynamic-SMEM buffer (filter staging / TMA tile ring)
   int use_tma;                   // streaming phases fetch tiles with cp.async.bulk into an SMEM ring
   uint32_t hist_shift;           // history bound = prev_thr - (1 << hist_shift): 23 -> x0.5, 22 -> ~x0.7
-  const uint32_t* poly_tensors;  // ids of the tensors with vmode == 1 (largest K first)
+  const uint32_t* poly_tensors;  // ids of the ranked (kVmodePolyfit, kVmodeDexp) tensors (largest K first)
   uint32_t n_poly;
   const uint32_t* poly_tasks;    // per-value tasks: {tensor id, first value of a 512-value chunk}
   uint32_t n_poly_tasks;
@@ -206,7 +210,7 @@ struct EngineParams {
   float* bucket_val;             // [sum K] values grouped by bin
   uint32_t* bucket_pos;          // [sum K] original position p of the grouped values
   float* expand_buf;             // [world][sum K] fitted curves of every rank
-  uint32_t poly_total;           // sum K over the vmode==1 tensors
+  uint32_t poly_total;           // sum K over the ranked tensors
   unsigned long long* debug_times;  // optional [kPhEnd + 1][grid][2] globaltimer ns at phase entry / exit of every CTA (nullptr: off);
                                     // row kPhEnd: {%smid of the CTA, 0}
   const uint32_t* cuts;          // optional per-phase-class tile partitions [kNumParts][cuts_grid + 1] (first tile of every CTA,
@@ -237,7 +241,7 @@ struct EngineParams {
   // own decoded contribution is non-zero (emit for fp32 values, fix for coded values)
   float* mom;                    // [total elements] fp32 momentum u (persists across steps)
   float momentum;
-  int has_bf16_values;           // some tensor ships bf16 values (vmode 4: only the <.., true> kernels carry that path)
+  int has_bf16_values;           // some tensor ships bf16 values (kVmodeBf16: only the <.., true> kernels carry that path)
 };
 
 // Slot and slice layout, shared by the kernel and the host that launches it (binding.cpp)

@@ -31,10 +31,13 @@ import torch
 import torch.distributed as dist
 
 from .. import spec
+from ..codecs.bf16 import bf16_bits_oracle, bf16_widen_oracle
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
+from ..codecs.polyfit import get_segments, polyfit_eval_oracle, polyfit_fit_oracle
+from ..codecs.qsgd import qsgd_decode_oracle, qsgd_encode_oracle
 from .plan import update_cta_speeds
-from .plan import (DEXP_COEF_WORDS, DYN_WORDS, EMIT_DECODES, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST,
-                   POLICY_ID, SLOT_HEADER_WORDS, BucketPlan, rle_stream_words)
+from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID, SLOT_HEADER_WORDS,
+                   VMODE_BF16, VMODE_DEXP, VMODE_QSGD, BucketPlan, rle_stream_words)
 
 (PH_ACCUM, PH_FALLBACK, PH_HIST2, PH_INSERT, PH_QUERY, PH_EMIT, PH_RANK_HIST, PH_RANK_SCAN, PH_RANK_SCATTER,
  PH_RANK_EXACT, PH_FIT, PH_FIX, PH_PUSH, PH_SIGNAL, PH_EXPAND, PH_DECODE, PH_COMPACT, PH_PUSH2, PH_SIGNAL2,
@@ -138,7 +141,7 @@ def conflict_sets_keep_oracle(tp, pos: torch.Tensor, pick_words: np.ndarray) -> 
 
 
 def dexp_runs_fit_oracle(desc: torch.Tensor, num_pos: int) -> torch.Tensor:
-    """'dexp' of the fused engine (vmode 3): the values in descending order split at num_pos (the positives) into two
+    """'dexp' of the fused engine (VMODE_DEXP): the values in descending order split at num_pos (the positives) into two
     runs, each fitted by ``codecs.dexp.double_exponential_fit`` (fp64) on its own abscissa (i + 1) / length: the
     positives by ascending value, the rest by ascending magnitude.  Returns the shipped fp32 words
     (a, b, p, q) of the positive run, then of the rest."""
@@ -154,6 +157,17 @@ def dexp_runs_eval_oracle(coef: torch.Tensor, num_pos: int, n: int) -> torch.Ten
     from ..codecs.dexp import double_exponential_eval
     return torch.cat([double_exponential_eval(coef[:4], num_pos).flip(0),
                       -double_exponential_eval(coef[4:], n - num_pos)])
+
+
+def _ranked_curve(t, a: np.ndarray) -> torch.Tensor:
+    """The fitted values of a ranked tensor's ranks (descending order), from the curve words and the {num_pos, n} tail
+    in its slot region: the sender's residual and every receiver's decode go through this one evaluation."""
+    nc = t.coef_words
+    coef = torch.from_numpy(a[t.off_coef:t.off_coef + nc].view(np.float32).copy())
+    num_pos, n = int(a[t.off_coef + nc]), int(a[t.off_coef + nc + 1])
+    if t.vmode == VMODE_DEXP:
+        return dexp_runs_eval_oracle(coef, num_pos, n)
+    return polyfit_eval_oracle(coef, get_segments(n, num_pos), t.poly_degree)
 
 
 def _write_rank_map(tp, slot: np.ndarray, rank: torch.Tensor):
@@ -243,43 +257,26 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
         slot[tp.off_idx:tp.off_idx + sel.numel()] = sel.cpu().numpy().astype(np.uint32)
         cutoff = int(sel[-1].item()) if n_pos >= limit else 0xFFFFFFFF
     vals = acc[sel].float()
-    if tp.vmode == 3:
-        # 'dexp': the same rank map as polyfit; one double-exponential curve per sign run
-        n = int(sel.numel())
+    n = int(sel.numel())
+    if tp.ranked:
+        # 'both': stable descending sort -> rank map; the fitted curve is shipped, the residual keeps value - fitted
         order = torch.sort(vals, descending=True, stable=True).indices
         rank = torch.empty(n, dtype=torch.int64)
         rank[order] = torch.arange(n)
         num_pos = int((vals > 0).sum())
-        coef = dexp_runs_fit_oracle(vals[order], num_pos)
-        fitted = dexp_runs_eval_oracle(coef, num_pos, n)[rank]
-        slot[tp.off_coef:tp.off_coef + DEXP_COEF_WORDS] = coef.numpy().view(np.uint32)
-        slot[tp.off_coef + DEXP_COEF_WORDS] = num_pos
-        slot[tp.off_coef + DEXP_COEF_WORDS + 1] = n
-        _write_rank_map(tp, slot, rank)
-        resid[sel] = vals - fitted
-        vals = fitted
-    elif tp.vmode == 1:
-        # 'both': stable descending sort -> rank map; per-segment Gram fit; fitted values are what is shipped,
-        # and the residual keeps (value - fitted)
-        from ..codecs.polyfit import MAX_SEGMENTS, get_segments, polyfit_eval_oracle, polyfit_fit_oracle
-        n = int(sel.numel())
-        order = torch.sort(vals, descending=True, stable=True).indices
-        rank = torch.empty(n, dtype=torch.int64)
-        rank[order] = torch.arange(n)
-        num_pos = int((vals > 0).sum())
-        segs = get_segments(n, num_pos)
-        coef = polyfit_fit_oracle(vals[order], segs, tp.poly_degree)
-        fitted = polyfit_eval_oracle(coef, segs, tp.poly_degree)[rank] if n else vals
-        nc = MAX_SEGMENTS * (tp.poly_degree + 1)
+        if tp.vmode == VMODE_DEXP:
+            coef = dexp_runs_fit_oracle(vals[order], num_pos)
+        else:
+            coef = polyfit_fit_oracle(vals[order], get_segments(n, num_pos), tp.poly_degree)
+        nc = tp.coef_words
         slot[tp.off_coef:tp.off_coef + nc] = coef.numpy().view(np.uint32)
         slot[tp.off_coef + nc] = num_pos
         slot[tp.off_coef + nc + 1] = n
         _write_rank_map(tp, slot, rank)
+        fitted = _ranked_curve(tp, slot)[rank]
         resid[sel] = vals - fitted
         vals = fitted
-    elif tp.vmode == 2:
-        from ..codecs.qsgd import qsgd_decode_oracle, qsgd_encode_oracle
-        n = int(sel.numel())
+    elif tp.vmode == VMODE_QSGD:
         q = int(tp.poly_degree)
         lvl, norms = qsgd_encode_oracle(vals, q, 512, 0x51ED + epoch)
         dec = qsgd_decode_oracle(lvl, norms, q, 512) if n else vals
@@ -295,11 +292,9 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
             slot[tp.off_rankmap:tp.off_rankmap + (n + 3) // 4] = l8.view(np.uint32)
         resid[sel] = vals - dec
         vals = dec
-    elif tp.vmode == 4:
+    elif tp.vmode == VMODE_BF16:
         # bf16 values (round to nearest even, NaN -> 0x7FC0), two per word; the residual keeps the exact rounding error
         # where the widened value is finite, and is 0 (as for fp32 values) where it is not
-        from ..codecs.bf16 import bf16_bits_oracle, bf16_widen_oracle
-        n = int(sel.numel())
         q = np.zeros(((n + 1) // 2) * 2, dtype=np.uint16)
         bits = bf16_bits_oracle(vals)
         q[:n] = bits.numpy().astype(np.uint16)
@@ -373,27 +368,16 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
         n = int(idx.numel())
         if n == 0:
             continue
-        if t.vmode == 1:
-            from ..codecs.polyfit import MAX_SEGMENTS, get_segments, polyfit_eval_oracle
-            nc = MAX_SEGMENTS * (t.poly_degree + 1)
-            coef = torch.from_numpy(a[t.off_coef:t.off_coef + nc].view(np.float32).copy())
-            num_pos, n_fit = int(a[t.off_coef + nc]), int(a[t.off_coef + nc + 1])
-            curve = polyfit_eval_oracle(coef, get_segments(n_fit, num_pos), t.poly_degree)
-            vals = curve[_read_rank_map(t, a, n)]
-        elif t.vmode == 3:
-            coef = torch.from_numpy(a[t.off_coef:t.off_coef + DEXP_COEF_WORDS].view(np.float32).copy())
-            num_pos, n_fit = int(a[t.off_coef + DEXP_COEF_WORDS]), int(a[t.off_coef + DEXP_COEF_WORDS + 1])
-            vals = dexp_runs_eval_oracle(coef, num_pos, n_fit)[_read_rank_map(t, a, n)]
-        elif t.vmode == 2:
-            from ..codecs.qsgd import qsgd_decode_oracle
+        if t.ranked:
+            vals = _ranked_curve(t, a)[_read_rank_map(t, a, n)]
+        elif t.vmode == VMODE_QSGD:
             norms = torch.from_numpy(a[t.off_coef:t.off_coef + (n + 511) // 512].view(np.float32).copy())
             if t.rank_u32:
                 lvl = torch.from_numpy(a[t.off_rankmap:t.off_rankmap + (n + 1) // 2].view(np.int16)[:n].astype(np.int64))
             else:
                 lvl = torch.from_numpy(a[t.off_rankmap:t.off_rankmap + (n + 3) // 4].view(np.int8)[:n].astype(np.int64))
             vals = qsgd_decode_oracle(lvl, norms, int(t.poly_degree), 512)
-        elif t.vmode == 4:
-            from ..codecs.bf16 import bf16_widen_oracle
+        elif t.vmode == VMODE_BF16:
             bits = a[t.off_vals:t.off_vals + (n + 1) // 2].view(np.uint16)[:n].astype(np.int64)
             vals = bf16_widen_oracle(torch.from_numpy(bits))
         else:
@@ -467,31 +451,11 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
         d0 = SLOT_HEADER_WORDS + DYN_WORDS * ti
         n_sel, cutoff, thr_bits, n_pos = (int(x) for x in a[d0:d0 + 4])
         thr = float(np.array([thr_bits], dtype=np.uint32).view(np.float32)[0])
-        if t.vmode == 1:
-            vbytes = 4 * (22 * (t.poly_degree + 1) + 2) + (4 if t.rank_u32 else 2) * t.val_cap
-        elif t.vmode == 3:
-            vbytes = 4 * (DEXP_COEF_WORDS + 2) + (4 if t.rank_u32 else 2) * t.val_cap
-        elif t.vmode == 2:
-            vbytes = 4 * ((t.val_cap + 511) // 512) + t.val_cap * (2 if t.rank_u32 else 1)
-        elif t.vmode == 4:
-            vbytes = 2 * t.val_cap
-        else:
-            vbytes = 4 * t.val_cap
-        if t.mode == MODE_BLOOM:
-            ibytes = 4 * (t.n_filter_words + t.n_tiles + (4 * t.n_tiles if t.off_hint else 0))
-            if t.pos_cap:                                    # P2: positives per tile + the pick bitmask
-                ibytes += 4 * (t.n_tiles + (t.pos_cap + 31) // 32)
-            false_pos = max(0, n_pos - min(t.k, n_pos))      # positives beyond the K inserted (upper bound under 22-bit ties)
-        elif t.mode == MODE_RLE:
-            ibytes = 4 * ((t.n_tiles + 1) // 2 + rle_stream_words(t.val_cap))
-            false_pos = 0
-        elif t.mode == MODE_SHARED:
-            ibytes, false_pos = 0, 0                         # every rank draws the index set itself
-        else:
-            ibytes, false_pos = 4 * t.val_cap, 0
+        # bloom: positives beyond the K inserted (upper bound under 22-bit ties)
+        false_pos = max(0, n_pos - min(t.k, n_pos)) if t.mode == MODE_BLOOM else 0
         row = {"name": t.name, "numel": t.numel, "k": t.k, "n_sel": n_sel, "n_pos": n_pos, "false_pos": false_pos,
                "threshold": thr, "cutoff": None if cutoff == 0xFFFFFFFF else cutoff,
-               "value_bytes": vbytes, "index_bytes": ibytes}
+               "value_bytes": t.value_bytes, "index_bytes": t.index_bytes}
         if plan.policy == "random" and t.mode == MODE_BLOOM:   # header word 2 is the policy's acceptance threshold here
             row["threshold"] = None
             row["accept_rate"] = 1.0 if thr_bits == 0xFFFFFFFF else thr_bits / 2.0 ** 32
@@ -604,8 +568,7 @@ class BucketEngine:
                 # fp32 sums of the bloom apply (every sender of a tile is added before the one rounding): one 4096-float
                 # row per tile this rank decodes; not needed when every bloom tensor is scattered by emit (W = 1, fp32
                 # or bf16 values on the wire: emit knows the decoded value)
-                applied = any(t.mode == MODE_BLOOM and not (self.world == 1 and t.vmode in EMIT_DECODES)
-                              for t in plan.tensors)
+                applied = any(t.mode == MODE_BLOOM and (self.world > 1 or t.coded) for t in plan.tensors)
                 acc_tiles = span_max if applied else 0
                 self.acc32 = torch.zeros(max(acc_tiles, 1) * 4096, dtype=torch.float32, device=dev)
                 self.ctx.set_bf16(self.grad.data_ptr(), self.acc32.data_ptr(), acc_tiles)
@@ -638,7 +601,7 @@ class BucketEngine:
             if n_p2:
                 self.ctx.set_p2(self.p2_table.data_ptr(), n_p2, self.p2_scratch.data_ptr(), p2_cap)
             self.ctx.set_has_shared(int(any(t.mode == MODE_SHARED for t in plan.tensors)))
-            self.ctx.set_has_bf16_values(int(any(t.vmode == 4 for t in plan.tensors)))
+            self.ctx.set_has_bf16_values(int(any(t.vmode == VMODE_BF16 for t in plan.tensors)))
             ids, n_poly, tasks, n_tasks = plan.poly_tables()
             self.poly_ids, self.poly_tasks = ids.to(dev), tasks.to(dev)
             from .plan import RANK_BINS

@@ -20,6 +20,7 @@ from .. import spec
 from ..codecs.dexp import MIN_NUMEL as DEXP_MIN_NUMEL
 
 MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED = 0, 1, 2, 3
+VMODE_FP32, VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_BF16 = 0, 1, 2, 3, 4   # TensorDesc.vmode (plan.h ValueMode)
 KEY_SPAN = 1 << 31                    # select keys are 31-bit
 POLICY_ID = {"leftmost": 0, "random": 1, "p0": 2, "conflict_sets": 3}
 P2_MAX_POS_CAP = 1 << 20              # P2: the draw keeps one chosen bit per positive in shared memory (128 KB)
@@ -52,7 +53,6 @@ def update_cta_speeds(speeds, dur, gain: float = 0.8):
     return out / out.mean()
 MAX_POLY_K = 1 << 17      # the all-pairs rank pass is O(K^2): larger tensors keep fp32 values
 DEXP_COEF_WORDS = 8       # 'dexp': {a, b, p, q} of the positive run, then of the non-positive run (ops/csrc/plan.h)
-EMIT_DECODES = (0, 4)     # vmodes whose decoded value emit knows (fp32, bf16): at W = 1 it scatters them itself
 DESC_WORDS = 32
 RANK_BINS = 8192
 
@@ -166,6 +166,40 @@ class TensorPlan:
                 self.salt, self.n_filter_words, self.off_hint, self.vmode, self.off_coef, self.off_rankmap,
                 self.off_selidx, self.off_sorted, self.poly_degree, self.rank_u32, self.poly_off, self.poly_ord,
                 self.fixed_thr, self.shared_lb, self.pos_cap, self.off_pos_prefix, self.off_pick, 0, 0]
+
+    @property
+    def ranked(self) -> bool:
+        """The values travel as a fitted curve + the rank map of the shipped values (polyfit, dexp)."""
+        return self.vmode in (VMODE_POLYFIT, VMODE_DEXP)
+
+    @property
+    def coded(self) -> bool:
+        """A fix phase writes the residual (polyfit, QSGD, dexp); emit knows the other modes' decoded values."""
+        return self.vmode in (VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP)
+
+    @property
+    def coef_words(self) -> int:
+        """Words of a ranked tensor's curve, before its {num_pos, n} tail."""
+        return DEXP_COEF_WORDS if self.vmode == VMODE_DEXP else MAX_SEGMENTS * (self.poly_degree + 1)
+
+    @property
+    def value_bytes(self) -> int:
+        """Shipped bytes of the values (unpadded)."""
+        if self.ranked:
+            return 4 * (self.coef_words + 2) + (4 if self.rank_u32 else 2) * self.val_cap
+        if self.vmode == VMODE_QSGD:
+            return 4 * ((self.val_cap + 511) // 512) + self.val_cap * (2 if self.rank_u32 else 1)
+        return (2 if self.vmode == VMODE_BF16 else 4) * self.val_cap
+
+    @property
+    def index_bytes(self) -> int:
+        """Shipped bytes of the index (unpadded); 'randomk' ships none, every rank draws the index set itself."""
+        if self.mode == MODE_BLOOM:                    # filter, per-tile prefix, hint; P2: positives per tile + the pick
+            return 4 * (self.n_filter_words + self.n_tiles + (4 * self.n_tiles if self.off_hint else 0) +
+                        (self.n_tiles + (self.pos_cap + 31) // 32 if self.pos_cap else 0))
+        if self.mode == MODE_RLE:
+            return 4 * ((self.n_tiles + 1) // 2 + rle_stream_words(self.val_cap))
+        return 0 if self.mode == MODE_SHARED else 4 * self.val_cap
 
 
 @dataclass
@@ -320,17 +354,17 @@ class BucketPlan:
         dexp = self.value == "dexp" and tp.numel > self.dexp_min_numel
         if (poly or dexp) and tp.val_cap <= MAX_POLY_K:
             # curve coefficients + {num_pos, n} | rank map of the shipped values in their descending order
-            tp.vmode = 1 if poly else 3
+            tp.vmode = VMODE_POLYFIT if poly else VMODE_DEXP
             tp.rank_u32 = int(tp.val_cap > 65536)
             tp.off_coef = word
-            word = _align(word + (MAX_SEGMENTS * (tp.poly_degree + 1) if poly else DEXP_COEF_WORDS) + 2, 4)
+            word = _align(word + tp.coef_words + 2, 4)
             tp.off_rankmap = word
             word = _align(word + (tp.val_cap if tp.rank_u32 else (tp.val_cap + 1) // 2), 4)
             scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap), (tp, "off_sorted", tp.val_cap)]
         elif self.value == "qsgd":
             # bucketed QSGD (512 values per bucket): int8 levels (int16 when quantum_num >= 128, reference
             # pytorch/deepreduce.py:873) + one fp32 norm per bucket
-            tp.vmode = 2
+            tp.vmode = VMODE_QSGD
             tp.poly_degree = int(self.quantum_num)      # field re-used: quantum_num
             tp.rank_u32 = int(self.quantum_num >= 128)  # field re-used: 16-bit levels
             tp.off_coef = word                           # norms
@@ -338,29 +372,24 @@ class BucketPlan:
             tp.off_rankmap = word                        # levels
             word = _align(word + ((tp.val_cap + 1) // 2 if tp.rank_u32 else (tp.val_cap + 3) // 4), 4)
             scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap)]
-        elif self.value == "bf16":
-            # bf16 values, two per word (the p-th value in the low half of word p // 2): emit rounds them as it gathers
-            # and knows the decoded value, so there is no sender scratch and no later phase
-            tp.vmode = 4
-            tp.off_vals = word
-            word = _align(word + (tp.val_cap + 1) // 2, 4)
         else:
+            # fp32 values, or bf16 values two per word (the p-th value in the low half of word p // 2): emit rounds them
+            # as it gathers and knows the decoded value, so there is no sender scratch and no later phase
+            tp.vmode = VMODE_BF16 if self.value == "bf16" else VMODE_FP32
             tp.off_vals = word
-            word = _align(word + tp.val_cap, 4)
+            word = _align(word + (tp.value_bytes + 3) // 4, 4)
         return word
 
     def poly_tables(self):
-        """(tensor ids with a rank map (vmode 1 or 3), largest K first ; rank-phase tasks {tensor, first value of a
+        """(ranked tensor ids, largest K first ; per-value tasks of the coded tensors {tensor, first value of a
         512-chunk})."""
-        ids = sorted([i for i, t in enumerate(self.tensors) if t.vmode in (1, 3)], key=lambda i: -self.tensors[i].val_cap)
+        ids = sorted([i for i, t in enumerate(self.tensors) if t.ranked], key=lambda i: -self.tensors[i].val_cap)
         off = 0
         for o, i in enumerate(ids):
             self.tensors[i].poly_off, self.tensors[i].poly_ord = off, o
             off += self.tensors[i].val_cap
         self.poly_total = off
-        # the fix phase's tensors: every value codec but bf16 (vmode 4), whose residual emit writes
-        coded = sorted([i for i, t in enumerate(self.tensors) if t.vmode in (1, 2, 3)],
-                       key=lambda i: -self.tensors[i].val_cap)
+        coded = sorted([i for i, t in enumerate(self.tensors) if t.coded], key=lambda i: -self.tensors[i].val_cap)
         tasks = [(i, c) for i in coded for c in range(0, self.tensors[i].val_cap, 512)]
         ids_t = torch.tensor(ids if ids else [0], dtype=torch.int32)
         tasks_t = torch.tensor(tasks if tasks else [(0, 0)], dtype=torch.int32).reshape(-1)

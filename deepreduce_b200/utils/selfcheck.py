@@ -24,7 +24,7 @@ import torch.distributed as dist
 
 from .. import spec
 from ..codecs.bloom import bloom_query_oracle
-from ..parallel.plan import DYN_WORDS, MODE_BLOOM, MODE_RAW, MODE_SHARED, SLOT_HEADER_WORDS
+from ..parallel.plan import DYN_WORDS, MODE_BLOOM, MODE_RAW, MODE_SHARED, SLOT_HEADER_WORDS, VMODE_FP32
 
 
 def decode_slot_torch(plan, slot: torch.Tensor, seed: int = spec.DEFAULT_SEED):
@@ -36,7 +36,7 @@ def decode_slot_torch(plan, slot: torch.Tensor, seed: int = spec.DEFAULT_SEED):
     hdr = slot[:SLOT_HEADER_WORDS + DYN_WORDS * len(plan.tensors)].to(torch.int64).cpu() & 0xFFFFFFFF
     out = torch.zeros(plan.total_elems, dtype=torch.float32, device=dev)
     for ti, t in enumerate(plan.tensors):
-        if t.vmode != 0 or t.mode not in (MODE_BLOOM, MODE_RAW, MODE_SHARED):
+        if t.vmode != VMODE_FP32 or t.mode not in (MODE_BLOOM, MODE_RAW, MODE_SHARED):
             return None
         d0 = SLOT_HEADER_WORDS + DYN_WORDS * ti
         n_sel, cutoff = int(hdr[d0]), int(hdr[d0 + 1])
