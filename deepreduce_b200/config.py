@@ -12,6 +12,7 @@ written back into the user's dict.  Unknown keys are reported (typos such as
 """
 from __future__ import annotations
 
+import math
 import warnings
 from dataclasses import asdict, dataclass
 from typing import Optional
@@ -30,7 +31,7 @@ KNOWN_KEYS = frozenset({
     "policy", "sort", "poly_degree", "quantum_num", "bucket_size", "micro-benchmark", "world_size", "average",
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
-    "p2_pick_mask", "fused_rle_values", "fused_dexp", "momentum", "gradient_clipping",
+    "p2_pick_mask", "fused_rle_values", "fused_dexp", "momentum", "gradient_clipping", "weight_decay",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -101,6 +102,15 @@ class DeepReduceConfig:
                 raise ConfigError(f"'momentum' applies to 'memory': 'dgc' (got memory={cfg.memory!r})")
             if isinstance(m, bool) or not isinstance(m, (int, float)) or not 0.0 <= float(m) < 1.0:
                 raise ConfigError(f"'momentum' must be a number in [0, 1) (got {m!r})")
+        # ... and weight decay, added to the gradient ahead of that momentum as momentum SGD adds it: 'weight_decay' then
+        # replaces the optimizer's weight decay too
+        if "weight_decay" in params:
+            wd = params["weight_decay"]
+            if cfg.memory != "dgc":
+                raise ConfigError(f"'weight_decay' applies to 'memory': 'dgc' (got memory={cfg.memory!r})")
+            if (isinstance(wd, bool) or not isinstance(wd, (int, float)) or not math.isfinite(float(wd))
+                    or float(wd) < 0.0):
+                raise ConfigError(f"'weight_decay' must be a finite number >= 0 (got {wd!r})")
         if cfg.memory == "dgc":
             if cfg.compressor == "none":
                 raise ConfigError("'memory': 'dgc' needs a sparsifier: set 'compressor' to topk/threshold/randomk")

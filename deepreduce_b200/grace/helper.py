@@ -53,7 +53,7 @@ def grace_from_params(params: dict):
     if mem == 'residual':
         memory = ResidualMemory(params.get('beta', 1.0), params.get('gamma', 1.0))
     elif mem == 'dgc':
-        memory = DgcMemory(params.get('momentum', 0.9))
+        memory = DgcMemory(params.get('momentum', 0.9), params.get('weight_decay', 0.0))
     elif mem in ('none', None):
         memory = NoneMemory()
     else:

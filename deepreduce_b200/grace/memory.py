@@ -17,6 +17,19 @@ import torch
 from .base import Memory
 
 
+def _dense(t: torch.Tensor) -> bool:
+    """True if t's strides describe a permutation of a contiguous layout (contiguous, channels_last, ...): the layouts
+    in which DDP keeps a parameter's gradient with the parameter's strides."""
+    expect = 1
+    for st, sz in sorted(zip(t.stride(), t.size())):
+        if sz == 1:
+            continue
+        if st != expect:
+            return False
+        expect *= sz
+    return True
+
+
 class NoneMemory(Memory):
     def compensate(self, tensor, name):
         return tensor
@@ -64,14 +77,52 @@ class DgcMemory(Memory):
 
     A tensor not seen before starts with ``u = v = g`` (no additions, so ``-0.0`` stays intact).  With ``m = 0`` and
     finite gradients it computes bit for bit what ``ResidualMemory()`` computes.  The momentum lives here, so the
-    optimizer that follows must not add its own (e.g. ``SGD(momentum=0)``)."""
+    optimizer that follows must not add its own (e.g. ``SGD(momentum=0)``).
 
-    def __init__(self, momentum: float = 0.9):
+    ``weight_decay = wd > 0``: g is first replaced by ``fl(g + fl(wd * w))``, w the parameter ``bind_parameters`` bound
+    to the tensor's name, as torch's momentum SGD puts the decay through its momentum buffer; the optimizer then runs
+    without weight decay too.  With ``wd = 0`` nothing is read or added."""
+
+    def __init__(self, momentum: float = 0.9, weight_decay: float = 0.0):
         self.momentum = float(momentum)
+        self.weight_decay = float(weight_decay)
         self.momenta: dict[str, torch.Tensor] = {}
         self.residuals: dict[str, torch.Tensor] = {}
+        self.parameters: dict[str, torch.Tensor] = {}
+        self._storage_layout: dict[str, tuple] = {}   # storage-order names -> the parameter's strides when bound
+
+    def bind_parameters(self, named_parameters, storage_order: bool = False):
+        """``(name, parameter)`` pairs: the values the weight decay reads for the gradient of that name.
+
+        ``storage_order=True``: the gradients of these names arrive as plain reshapes of a flat buffer that holds
+        them in their parameters' storage order, as torch DDP's gradient buckets do (a dense parameter's gradient is
+        laid out with the parameter's strides, e.g. channels_last).  w is then read in storage order too, so that
+        element i of w belongs to element i of the gradient.  The parameter's layout must stay the one it had when it
+        was bound: a change of strides raises."""
+        for n, p in named_parameters:
+            self.parameters[n] = p
+            if storage_order:
+                self._storage_layout[n] = tuple(p.stride())
+            else:
+                self._storage_layout.pop(n, None)
+
+    def _weights(self, name, shape, dtype):
+        w = self.parameters.get(name)
+        if w is None:
+            raise KeyError(f"'dgc' weight decay: no parameter is bound to {name!r} (bind_parameters)")
+        w = w.detach()
+        layout = self._storage_layout.get(name)
+        if layout is not None:
+            if tuple(w.stride()) != layout:
+                raise ValueError(f"'dgc' weight decay: parameter {name!r} changed its layout from strides {layout} "
+                                 f"to {tuple(w.stride())} after it was bound; its gradient keeps the old order")
+            if _dense(w):
+                w = w.as_strided((w.numel(),), (1,))              # storage order
+        return w.reshape(shape).to(dtype)
 
     def compensate(self, tensor, name):
+        if self.weight_decay != 0.0:
+            tensor = tensor + (self.weight_decay * self._weights(name, tensor.shape, tensor.dtype))
         if name in self.momenta:
             u = self.momentum * self.momenta[name] + tensor
             tensor = self.residuals[name] + u

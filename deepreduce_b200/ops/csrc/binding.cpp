@@ -631,6 +631,13 @@ struct Engine {
     P.mom = reinterpret_cast<float*>(mom); P.momentum = (float)momentum;
   }
 
+  // 'dgc' weight decay: the device table of parameter addresses, one per plan tensor (EngineParams::wparams), and the
+  // factor; 0 = none (nothing is read)
+  void set_weight_decay(int64_t table, double weight_decay) {
+    TORCH_CHECK(weight_decay == 0.0 || table != 0, "set_weight_decay: weight decay needs the parameter table");
+    P.wparams = reinterpret_cast<const unsigned long long*>(table); P.weight_decay = (float)weight_decay;
+  }
+
   int get_grid() {
     if (grid == 0) grid = dr::engine_max_grid(blocks_per_sm, dyn_smem);
     return grid;
@@ -857,6 +864,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("configure", &Engine::configure)
       .def("set_buffers", &Engine::set_buffers)
       .def("set_momentum", &Engine::set_momentum)
+      .def("set_weight_decay", &Engine::set_weight_decay)
       .def("set_bf16", &Engine::set_bf16)
       .def("set_poly", &Engine::set_poly)
       .def("set_shard", &Engine::set_shard)

@@ -386,6 +386,29 @@ DR_D void append_candidates(Smem& sm, uint32_t m, const uint32_t (&key)[4], uint
 
 DR_D uint32_t round16(uint32_t bytes) { return (bytes + 15u) & ~15u; }
 
+// 'dgc' weight decay: the four parameter values of plan tensor t at in-tensor elements e .. e + 3, of which the first n
+// (>= 1) lie inside the tensor; the others are padding of the engine's buffers, which the parameter does not have, and
+// read as 0.  One vector load when the address is aligned and all four are inside, else element by element.  A bf16
+// bucket's parameters stay packed (low half first, as widen_bf16x4 takes them) until they are used: two registers
+// instead of four across the ring wait.
+DR_D float4 load_weights(const EngineParams& P, uint32_t t, uint32_t e, uint32_t n) {
+  const float* w = reinterpret_cast<const float*>(__ldg(P.wparams + t)) + e;
+  if (n >= 4u && (reinterpret_cast<uintptr_t>(w) & 15u) == 0u) return __ldg(reinterpret_cast<const float4*>(w));
+  float v[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (uint32_t j = 0; j < 4u; ++j) if (j < n) v[j] = __ldg(w + j);
+  return make_float4(v[0], v[1], v[2], v[3]);
+}
+
+DR_D uint2 load_weights_bf16(const EngineParams& P, uint32_t t, uint32_t e, uint32_t n) {
+  const uint16_t* w = reinterpret_cast<const uint16_t*>(__ldg(P.wparams + t)) + e;
+  if (n >= 4u && (reinterpret_cast<uintptr_t>(w) & 7u) == 0u) return __ldg(reinterpret_cast<const uint2*>(w));
+  uint32_t h[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+  for (uint32_t j = 0; j < 4u; ++j) if (j < n) h[j] = __ldg(w + j);
+  return make_uint2(h[0] | (h[1] << 16), h[2] | (h[3] << 16));
+}
+
 // kTma = true : g / r half-tiles arrive through a CTA-wide TMA ring (cp.async.bulk + full/empty mbarriers, one producer
 //               thread); kTma = false: every THREAD copies its own float4 of g and r with cp.async (LDGSTS) into a
 //               private slot of the ring and reads it back itself — no mbarriers, no producer, warps never wait for
@@ -398,7 +421,9 @@ DR_D uint32_t round16(uint32_t bytes) { return (bytes + 15u) & ~15u; }
 //               before it waits for the ring so that the load overlaps the wait, and writes u back the same way.  u
 //               is not staged through the ring: the stage size, the ring depth and the shared-memory budget stay
 //               the same as the existing variants', so u costs no ring space and no extra TMA bookkeeping, and each
-//               element of u is read by exactly the thread that uses it.
+//               element of u is read by exactly the thread that uses it.  With weight decay (P.weight_decay != 0,
+//               CTA-uniform) the thread reads its four elements of the parameter w the same way, next to u, and adds
+//               fl(weight_decay * w) to g before the momentum; with weight_decay == 0 nothing is read or added.
 template <bool kTma, bool kFull, bool kB, bool kDgc>
 DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
@@ -523,10 +548,17 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
         const uint32_t off = (uint32_t)h * kHalf;
         uint32_t key4[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};   // 0xFFFFFFFF = not an element
         if (off < ti.n) {                                                  // CTA-uniform
-          float4 u_old = zero4;
+          float4 u_old = zero4, w = zero4;
+          uint2 w_bf16 = make_uint2(0u, 0u);
           if constexpr (kDgc) {
             const uint32_t e0 = off + tid * 4u;
-            if (e0 < ti.n) u_old = __ldcs(reinterpret_cast<const float4*>(P.mom + ti.base + e0));
+            if (e0 < ti.n) {
+              u_old = __ldcs(reinterpret_cast<const float4*>(P.mom + ti.base + e0));
+              if (P.weight_decay != 0.0f) {
+                if constexpr (kB) w_bf16 = load_weights_bf16(P, cur, ti.local0 + e0, ti.n - e0);
+                else w = load_weights(P, cur, ti.local0 + e0, ti.n - e0);
+              }
+            }
           }
           if (kTma) {
             // refill first: the stage consumed one item ago is free as soon as every warp released it
@@ -555,7 +587,12 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
             else g = sg[tid];
             float4 a;
             if constexpr (kDgc) {                                          // two roundings each: no contracted FMA
-              const float mu = P.momentum;
+              const float mu = P.momentum, wd = P.weight_decay;
+              if (wd != 0.0f) {                                            // d = fl(g + fl(wd * w)) replaces g
+                if constexpr (kB) w = widen_bf16x4(w_bf16);
+                g.x = __fadd_rn(g.x, __fmul_rn(wd, w.x)); g.y = __fadd_rn(g.y, __fmul_rn(wd, w.y));
+                g.z = __fadd_rn(g.z, __fmul_rn(wd, w.z)); g.w = __fadd_rn(g.w, __fmul_rn(wd, w.w));
+              }
               float4 u;
               u.x = __fadd_rn(__fmul_rn(mu, u_old.x), g.x); u.y = __fadd_rn(__fmul_rn(mu, u_old.y), g.y);
               u.z = __fadd_rn(__fmul_rn(mu, u_old.z), g.z); u.w = __fadd_rn(__fmul_rn(mu, u_old.w), g.w);

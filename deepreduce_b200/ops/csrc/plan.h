@@ -129,7 +129,7 @@ constexpr uint32_t kArenaHdrWords = 128;
 // and the same 22-bit rule applies to it: a superset of the K smallest hashes, plus ~numel / 2^22 elements sharing the
 // threshold's prefix.  The set depends on (numel, K, epoch, salt) only, so every rank computes the same one.
 enum Phase : int {
-  kPhAccum = 0,      // r = beta*r + gamma*g (dgc: u = m*u + g, r = r + u) ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
+  kPhAccum = 0,      // r = beta*r + gamma*g (dgc: u = m*u + g [+ wd*w], r = r + u) ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
   kPhFallback = 1,   // (only if some bound was unsafe) digit 1 redone without the bound, candidate lists rebuilt in full
   kPhHist2 = 2,      // digit 2 of the candidate keys in the threshold bin
   kPhInsert = 3,     // selected candidates -> bloom filter + occupancy hint (bloom) / positive masks (raw, rle)
@@ -242,6 +242,12 @@ struct EngineParams {
   float* mom;                    // [total elements] fp32 momentum u (persists across steps)
   float momentum;
   int has_bf16_values;           // some tensor ships bf16 values (kVmodeBf16: only the <.., true> kernels carry that path)
+  // 'dgc' weight decay (weight_decay != 0, the dgc kernels only): the accumulate phase adds weight_decay * w to the
+  // gradient ahead of the momentum, d = fl(g + fl(weight_decay * w)), with w read from the parameter itself.
+  // wparams[t]: address of plan tensor t's first element in its parameter's storage (the bucket's dtype; a chunk of a
+  // split parameter points at its offset).  Only the tensor's numel elements are read: the padding takes w = 0.
+  const unsigned long long* wparams;  // [n_tensors]
+  float weight_decay;
 };
 
 // Slot and slice layout, shared by the kernel and the host that launches it (binding.cpp)

@@ -18,7 +18,10 @@ segment table, built the first time the hook meets it; ``bucket_pack`` / ``bucke
 move the whole bucket in one launch each way.  DDP rebuilds its buckets after the first iteration, so a run meets two
 layouts: the residual of every parameter is carried from the old engine into the new one (DESIGN.md, "DDP
 communication hook"), and with ``'memory': 'dgc'`` its momentum too.  That memory holds the momentum, so the optimizer
-stepping the DDP model must run without one (e.g. ``torch.optim.SGD(..., momentum=0)``).
+stepping the DDP model must run without one (e.g. ``torch.optim.SGD(..., momentum=0)``).  With ``'weight_decay'`` in
+the dict the memory adds the decay ahead of its momentum, reading the parameters of each bucket, so that optimizer also
+runs with ``weight_decay=0``.  The parameters are read in the order of their gradients in the bucket, i.e. in their
+storage order, which DDP gives a dense parameter's gradient; their layouts must not change after DDP built its buckets.
 """
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -163,10 +166,17 @@ class DeepReduceHookState:
         work = dist.all_reduce(buf, group=self.group, async_op=True)
         return work.get_future().then(lambda f: f.value()[0])
 
+    def _make_grc(self):
+        from ..wrappers import deepreduce_from_params
+        self.grc = deepreduce_from_params(self.params)
+        if hasattr(self.grc.memory, "bind_parameters"):           # 'dgc' weight decay reads the parameters
+            # bucket.gradients() are plain reshapes of the flat bucket, which holds every gradient in its
+            # parameter's storage order: the memory reads the parameters in that order too
+            self.grc.memory.bind_parameters(self.module.named_parameters(), storage_order=True)
+
     def _grace(self, bucket, buf):
         if self.grc is None:
-            from ..wrappers import deepreduce_from_params
-            self.grc = deepreduce_from_params(self.params)
+            self._make_grc()
         for p, g in zip(bucket.parameters(), bucket.gradients()):
             out = self.grc.step(g, self._name(p))
             g.copy_(out.view_as(g))
@@ -227,9 +237,12 @@ class DeepReduceHookState:
         numels, pnames, shapes, owner = split_large(numels, names, shapes,
                                                      engine_split_numel(self.params, self.blocks_per_sm))
         plan = BucketPlan(numels, pnames, shapes, **plan_kwargs_from_params(self.params))
+        # 'weight_decay': the engine reads every parameter in storage order, where the bucket holds its gradient (DDP
+        # lays a dense parameter's gradient out with the parameter's strides; bind_parameters refuses any other).  The
+        # parameters' layouts are recorded here and must stay as DDP found them: a later change raises at the next step
         # calibration (inside make_engine) resets the residual: it runs before the carry below
         eng = make_engine(plan, self.params, device=buf.device, group=self.group, use_history=self.use_history,
-                          blocks_per_sm=self.blocks_per_sm, grad_dtype=buf.dtype)
+                          blocks_per_sm=self.blocks_per_sm, grad_dtype=buf.dtype, parameters=list(params), owner=owner)
         table = segment_table(segments, plan, owner)
         repack = ops.cuda_module().Repack(table, buf.numel(), plan.total_elems, eng.grad)
         lay = _Layout(key, index, list(params), names, list(segments), plan, eng, table, repack)
@@ -369,8 +382,7 @@ class DeepReduceHookState:
                     view(lay, p).copy_(t.to(lay.engine.device, torch.float32).reshape(-1))
         if "memory" in state:
             if self.grc is None:
-                from ..wrappers import deepreduce_from_params
-                self.grc = deepreduce_from_params(self.params)
+                self._make_grc()
             dev = next(self.module.parameters()).device
             self.grc.memory.load_state_dict(state["memory"], device=dev)
 

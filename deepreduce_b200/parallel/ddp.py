@@ -180,22 +180,28 @@ def engine_split_numel(params: dict, blocks_per_sm: int) -> int:
 
 
 def engine_kwargs(params: dict) -> dict:
-    """The ``BucketEngine`` memory arguments for ``params``: beta, gamma, momentum and averaging.  They follow the
-    per-tensor memory GRACE builds for the same dict: only ``ResidualMemory`` scales the gradient by gamma, so
-    'none' and 'dgc' memory run with gamma = 1 ('dgc' accepts no other), and without a residual beta is 0."""
+    """The ``BucketEngine`` memory arguments for ``params``: beta, gamma, momentum, weight decay and averaging.  They
+    follow the per-tensor memory GRACE builds for the same dict: only ``ResidualMemory`` scales the gradient by gamma,
+    so 'none' and 'dgc' memory run with gamma = 1 ('dgc' accepts no other), and without a residual beta is 0."""
     memory = params.get('memory', 'none')
     return dict(beta=float(params.get('beta', 1.0)) if memory in ('residual', 'dgc') else 0.0,
                 gamma=float(params.get('gamma', 1.0)) if memory == 'residual' else 1.0,
                 average=params.get('average', True),
-                momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None)
+                momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None,
+                weight_decay=float(params.get('weight_decay', 0.0)) if memory == 'dgc' else 0.0)
 
 
 def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: bool, blocks_per_sm: int,
-                grad_dtype: torch.dtype) -> BucketEngine:
+                grad_dtype: torch.dtype, parameters=None, owner=None) -> BucketEngine:
     """The ``BucketEngine`` of one bucket for ``params`` (memory arguments from ``engine_kwargs``), with its tile
-    partitions calibrated unless ``'calibrate_partition': False``.  Collective at W > 1."""
+    partitions calibrated unless ``'calibrate_partition': False``.  ``parameters`` / ``owner``: the bucket's parameters
+    and the plan tensors' owners (``split_large``), bound when the engine applies weight decay.  Collective at W > 1."""
     eng = BucketEngine(plan, device=device, group=group, use_history=use_history, blocks_per_sm=blocks_per_sm,
                        grad_dtype=grad_dtype, **engine_kwargs(params))
+    if eng.weight_decay != 0.0:
+        if parameters is None:
+            raise ValueError("'weight_decay' reads the parameters: make_engine needs the bucket's parameters")
+        eng.bind_parameters(parameters, owner)
     # re-cut the kernel's tile partitions from measured per-CTA phase times (collective; ~12 exchange steps
     # on synthetic gradients, state reset afterwards) — 'calibrate_partition': False keeps the static cut
     if params.get('calibrate_partition', True) and eng.cuts is not None:
@@ -255,6 +261,8 @@ class DeepReduceDDP:
                 self._install_hooks()
         else:
             self.grc = deepreduce_from_params(self.params)
+            if hasattr(self.grc.memory, "bind_parameters"):       # 'dgc' weight decay reads the parameters
+                self.grc.memory.bind_parameters(self.named)
 
     # ---- bucket construction ------------------------------------------------
     def _build_buckets(self, cap_mb, blocks_per_sm, use_history):
@@ -273,7 +281,8 @@ class DeepReduceDDP:
             if self.fused:
                 plan = BucketPlan(numels, names, shapes, **plan_kwargs_from_params(self.params))
                 eng = make_engine(plan, self.params, device=self.device, group=self.group, use_history=use_history,
-                                  blocks_per_sm=blocks_per_sm, grad_dtype=dtype)
+                                  blocks_per_sm=blocks_per_sm, grad_dtype=dtype, parameters=[p for _, p in items],
+                                  owner=owner)
                 self.engines.append(eng)
                 flat, views = eng.grad, eng.grad_views
             else:
@@ -322,6 +331,7 @@ class DeepReduceDDP:
         self._launched[b] = True
         if self.fused:
             eng = self.engines[b]
+            eng.refresh_parameters()          # weight decay: follow a parameter whose storage moved (p.data = ...)
             # the engine's own step counter, never reset: peer flags carry the epoch, so an epoch that was already used
             # (e.g. by calibrate_partition's synthetic steps, or by a self-check step between training steps) would
             # let the flag waits pass before the peers have written their slots

@@ -21,6 +21,7 @@ Parity with the reference (hangxu0304/DeepReduce), per tensor of the bucket:
 """
 from __future__ import annotations
 
+import math
 import os
 
 from collections import OrderedDict
@@ -313,22 +314,30 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
 
 
 def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Sequence[torch.Tensor], *, beta=1.0,
-                  gamma=1.0, average=True, seed=spec.DEFAULT_SEED, epoch=1, momentum=None, moms=None):
+                  gamma=1.0, average=True, seed=spec.DEFAULT_SEED, epoch=1, momentum=None, moms=None,
+                  weight_decay=0.0, weights=None):
     """One bucket step for W ranks on the CPU.  grads/resids: per-rank flat
     buffers (plan.total_elems).  Returns (dense_out, new_resids, slots).
 
     ``momentum`` set ('dgc' memory, beta = gamma = 1): ``moms`` are the per-rank momenta u, the step is
     u = momentum * u + g, r = r + u (each a separately rounded fp32 op) before the select, and u is cleared wherever
-    the rank's own decoded value is non-zero; returns (dense_out, new_resids, slots, new_moms)."""
+    the rank's own decoded value is non-zero; returns (dense_out, new_resids, slots, new_moms).
+
+    ``weight_decay`` wd != 0 (with ``momentum``): ``weights`` are the per-rank parameters, flat in plan layout (zeros in
+    the padding), and g is replaced by d = g + (wd * w), two roundings, before the momentum."""
     W = len(grads)
     dgc = momentum is not None
     if dgc and (beta != 1.0 or gamma != 1.0 or moms is None or len(moms) != W):
         raise ValueError("engine_oracle: momentum needs beta = gamma = 1 and one momentum buffer per rank")
+    if weight_decay != 0.0 and (not dgc or weights is None or len(weights) != W):
+        raise ValueError("engine_oracle: weight_decay needs momentum and one parameter buffer per rank")
     out = torch.zeros(plan.total_elems, dtype=torch.float32)
     new_resids, slots, new_moms = [], [], []
     for r in range(W):
         g = grads[r].detach().cpu().float()
         res = resids[r].detach().cpu().float()
+        if weight_decay != 0.0:
+            g = g + (float(weight_decay) * weights[r].detach().cpu().float())
         if dgc:
             u = float(momentum) * moms[r].detach().cpu().float() + g
             acc_flat = res + u
@@ -486,7 +495,7 @@ class BucketEngine:
                  rank: Optional[int] = None, filter_smem_bytes: Optional[int] = None, use_tma: bool = True,
                  hist_shift: int = 22, shard: Optional[bool] = None, transport: Optional[str] = None,
                  peer_timeout_ms: Optional[int] = None, fault: int = 0, grad_dtype: torch.dtype = torch.float32,
-                 momentum: Optional[float] = None):
+                 momentum: Optional[float] = None, weight_decay: float = 0.0):
         # grad_dtype=torch.bfloat16: the flat gradient (in: local, out: aggregate) is bf16.  The residual, the select,
         # the codecs and the wire stay fp32 (widening bf16 is exact), so the engine computes exactly what an fp32 engine
         # fed the widened gradient computes, and rounds the aggregate once (to nearest even) where it is final.  The
@@ -499,6 +508,15 @@ class BucketEngine:
             raise ValueError(f"momentum needs beta = gamma = 1 and a value in [0, 1) (got beta={beta}, gamma={gamma}, "
                              f"momentum={momentum})")
         self.momentum = None if momentum is None else float(momentum)
+        # weight_decay=wd ('dgc' only): d = g + wd*w ahead of the momentum, w read from the parameters that
+        # ``bind_parameters`` points the kernel at (engine_oracle(weight_decay=..., weights=...))
+        wd = weight_decay
+        if isinstance(wd, bool) or not isinstance(wd, (int, float)) or not math.isfinite(wd) or wd < 0:
+            raise ValueError(f"weight_decay must be a finite number >= 0 (got {wd!r})")
+        if wd != 0 and momentum is None:
+            raise ValueError("weight_decay is added inside the 'dgc' memory: it needs momentum")
+        self.weight_decay = float(wd)
+        self._bound = None                       # (parameters, owner, data_ptrs, strides) of the last bind_parameters
         from .. import ops
         self.mod = ops.cuda_module()
         self.plan = plan
@@ -564,6 +582,8 @@ class BucketEngine:
                                  self.cand_cnt.data_ptr())
             if self.mom is not None:
                 self.ctx.set_momentum(self.mom.data_ptr(), self.momentum)
+            # one parameter address per plan tensor (bind_parameters); the kernel reads it only when weight_decay != 0
+            self.wparams = torch.zeros(nT, dtype=torch.int64, device=dev)
             if grad_dtype == torch.bfloat16:
                 # fp32 sums of the bloom apply (every sender of a tile is added before the one rounding): one 4096-float
                 # row per tile this rank decodes; not needed when every bloom tensor is scattered by emit (W = 1, fp32
@@ -768,10 +788,78 @@ class BucketEngine:
             self.mod.arena_free(self._arena_ptr)
             self._ipc = False
 
+    # ---- parameters ('dgc' weight decay) --------------------------------------
+    def bind_parameters(self, parameters: Sequence[torch.Tensor], owner: Optional[Sequence[int]] = None):
+        """Point the kernel at the parameters whose values the weight decay reads: ``parameters`` in plan order, one per
+        original tensor, and ``owner[j]`` the parameter plan tensor j belongs to (``split_large``; default: one plan
+        tensor each).  A chunk reads its parameter from the chunk's offset on.  Every parameter must be on this
+        engine's device, of the bucket's dtype, and dense, so that its storage order is the order of its gradient in
+        the bucket.  The table is uploaded on the current stream; call it again (or ``refresh_parameters``) when a
+        parameter's storage moves."""
+        from .ddp import _is_dense
+        params = list(parameters)
+        owner = list(range(len(params))) if owner is None else [int(o) for o in owner]
+        tensors = self.plan.tensors
+        if len(owner) != len(tensors) or sorted(set(owner)) != list(range(len(params))):
+            raise ValueError(f"bind_parameters: {len(params)} parameters and owner {owner} do not cover the plan's "
+                             f"{len(tensors)} tensors")
+        done = [0] * len(params)                 # elements of each parameter covered by its earlier chunks
+        ptrs = []
+        for j, t in enumerate(tensors):
+            i = owner[j]
+            p = params[i]
+            if p.device != self.device or p.dtype != self.grad_dtype:
+                raise ValueError(f"bind_parameters: parameter {i} ({t.name}) is {p.dtype} on {p.device}; the engine's "
+                                 f"bucket is {self.grad_dtype} on {self.device}")
+            if not _is_dense(p):
+                raise ValueError(f"bind_parameters: parameter {i} ({t.name}) is not dense in memory: its storage order "
+                                 f"is not the order of its gradient in the bucket")
+            ptrs.append(p.data_ptr() + done[i] * p.element_size())
+            done[i] += t.numel
+        for i, p in enumerate(params):
+            if done[i] != p.numel():
+                raise ValueError(f"bind_parameters: parameter {i} has {p.numel()} elements, the plan {done[i]}")
+        self.wparams.copy_(torch.tensor(ptrs, dtype=torch.int64))
+        self._bound = (params, owner, [p.data_ptr() for p in params], [tuple(p.stride()) for p in params])
+        self.ctx.set_weight_decay(self.wparams.data_ptr(), self.weight_decay)
+
+    def refresh_parameters(self):
+        """Before a launch: rebuild the parameter table if a bound parameter's storage moved (``p.data = ...``).  The
+        check is a host-side comparison of data pointers; it raises if weight decay is on and nothing is bound.  A moved
+        parameter must keep the strides it was bound with: the bucket holds its gradient in that storage order (e.g.
+        ``model.to(memory_format=...)`` after the buckets were built raises here)."""
+        if self.weight_decay == 0.0:
+            return
+        if self._bound is None:
+            raise RuntimeError("weight_decay > 0 reads the parameters: call bind_parameters() before the first step")
+        params, owner, ptrs, layouts = self._bound
+        if any(p.data_ptr() != q for p, q in zip(params, ptrs)):
+            changed = [i for i, (p, l) in enumerate(zip(params, layouts)) if tuple(p.stride()) != l]
+            if changed:
+                raise ValueError(f"weight decay: parameters {changed} of the bucket changed their layout since they "
+                                 f"were bound; the bucket keeps their gradients in the old storage order")
+            self.bind_parameters(params, owner)
+
+    def parameter_buffer(self) -> torch.Tensor:
+        """The bound parameters as one flat fp32 buffer in plan layout (zeros in the padding), what the kernel reads:
+        the ``weights`` of ``engine_oracle``."""
+        if self._bound is None:
+            raise RuntimeError("no parameters are bound (bind_parameters)")
+        params, owner, _, _ = self._bound
+        out = torch.zeros(self.plan.total_elems, dtype=torch.float32, device=self.device)
+        done = [0] * len(params)
+        for j, t in enumerate(self.plan.tensors):
+            p = params[owner[j]].detach()
+            flat = p.as_strided((p.numel(),), (1,))                  # storage order
+            out[t.elem_off:t.elem_off + t.numel] = flat[done[owner[j]]:done[owner[j]] + t.numel].float()
+            done[owner[j]] += t.numel
+        return out
+
     # ---- run ---------------------------------------------------------------
     def step(self, epoch: Optional[int] = None):
         """Launch the fused kernel on the current stream.  In: ``self.grad``
         (local dense grads).  Out: ``self.grad`` (aggregated), ``self.resid``."""
+        self.refresh_parameters()
         self.epoch = self.epoch + 1 if epoch is None else int(epoch)
         if self.transport == "nccl" and self.world > 1:
             self._step_nccl()

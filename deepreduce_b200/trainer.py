@@ -39,9 +39,13 @@ class Trainer:
                                  overlap_grid=overlap_grid)
         if optimizer is None:
             # 'memory': 'dgc' accumulates the momentum before the exchange (momentum correction): the optimizer then
-            # runs without one, whatever ``momentum`` says.  A user optimizer must do the same.
+            # runs without one, whatever ``momentum`` says.  A user optimizer must do the same.  With 'weight_decay'
+            # in the dict the memory adds the decay ahead of that momentum, and the dict's value replaces
+            # ``weight_decay`` here: the optimizer runs without it.
             if params.get('memory') == 'dgc':
                 momentum = 0.0
+                if 'weight_decay' in params:
+                    weight_decay = 0.0
             kw = dict(lr=lr, momentum=momentum, weight_decay=weight_decay)
             if self.is_cuda:
                 kw["fused"] = True

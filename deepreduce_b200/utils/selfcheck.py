@@ -94,7 +94,8 @@ def multi_gpu_check(engine, seed: int = 4242) -> dict:
         v.copy_(torch.randn(v.shape, device=dev, generator=gen) * 1e-2)
     g = g.to(engine.grad.dtype).float()         # bf16 engine: the widened bf16 gradient is what the engine accumulates
     if engine.mom is not None:                  # 'dgc': the momentum is compensated, then added to the residual
-        acc = engine.resid + (engine.momentum * engine.mom + g)
+        d = g + (engine.weight_decay * engine.parameter_buffer()) if engine.weight_decay != 0.0 else g
+        acc = engine.resid + (engine.momentum * engine.mom + d)
     else:
         acc = engine.beta * engine.resid + engine.gamma * g if engine.beta != 0.0 else engine.gamma * g
     engine.grad.copy_(g)

@@ -1,13 +1,18 @@
-"""Cost of the 'dgc' memory (momentum correction + momentum factor masking) on ResNet-50, bf16 buckets, bloom at 1 %.
+"""Cost of the 'dgc' memory (momentum correction + momentum factor masking) on ResNet-50, bf16 buckets, bloom at 1 %,
+and of its weight decay.
 
-Two measurements on one GPU, each alternating its two arms round by round:
+Two measurements on one GPU, each alternating its three arms round by round:
 
-* exchange kernel: one bf16 ``BucketEngine`` over every ResNet-50 parameter with the residual memory, and the same
-  engine with ``momentum=0.9`` (phase 0 also streams the fp32 momentum in and out: 8 B per element);
+* exchange kernel: one bf16 ``BucketEngine`` over every ResNet-50 parameter with the residual memory, the same
+  engine with ``momentum=0.9`` (phase 0 also streams the fp32 momentum in and out: 8 B per element), and with
+  ``momentum=0.9, weight_decay=1e-4`` (phase 0 also reads the bf16 parameters: 2 B more per element), once with
+  random parameters and once with all-zero parameters ("w = 0": d = g exactly, so that arm computes what the plain
+  'dgc' arm computes and differs from it only by the parameter read); every arm exchanges the same gradients;
   ms per launch from CUDA events over ``--launches`` launches;
 * whole training step: ResNet-50 with bf16 conv / linear weights and fp32 BatchNorm (batch ``--batch``, 224 x 224,
-  channels_last, so one bf16 and one fp32 bucket) under ``DeepReduceDDP`` with
-  residual + SGD(momentum 0.9) against dgc + SGD(momentum 0), img/s from CUDA events over ``--steps`` steps.
+  channels_last, so one bf16 and one fp32 bucket) under ``DeepReduceDDP`` with residual + SGD(momentum 0.9),
+  dgc + SGD(momentum 0), and dgc with 'weight_decay' + SGD(momentum 0, weight_decay 0), img/s from CUDA events over
+  ``--steps`` steps.
 
 Prints one JSON line with the card's name and power limit read in the same process.
 
@@ -29,7 +34,8 @@ from randomk_step import card, events_ms  # noqa: E402
 BLOOM = {'compressor': 'topk', 'communicator': 'allgather', 'compress_ratio': 0.01, 'deepreduce': 'index',
          'index': 'bloom', 'calibrate_partition': False}
 ARMS = {"residual": ({**BLOOM, 'memory': 'residual'}, 0.9),
-        "dgc": ({**BLOOM, 'memory': 'dgc', 'momentum': 0.9}, 0.0)}
+        "dgc": ({**BLOOM, 'memory': 'dgc', 'momentum': 0.9}, 0.0),
+        "dgc_weight_decay": ({**BLOOM, 'memory': 'dgc', 'momentum': 0.9, 'weight_decay': 1e-4}, 0.0)}
 
 
 def exchange_kernel(launches, rounds):
@@ -39,14 +45,24 @@ def exchange_kernel(launches, rounds):
     from deepreduce_b200.parallel.ddp import make_engine, plan_kwargs_from_params
     numels = [p.numel() for p in reversed(list(models.resnet50().parameters()))]
     gen = torch.Generator(device="cuda:0").manual_seed(7)
+    weights = [torch.randn(n, device="cuda:0", generator=gen).to(torch.bfloat16) for n in numels]
+    g = (torch.randn(sum(numels), device="cuda:0", generator=gen) * 1e-3).to(torch.bfloat16)
+    zeros = [torch.zeros_like(w) for w in weights]
+    arms = {name: (params, weights) for name, (params, _) in ARMS.items()}
+    arms["dgc_weight_decay_w0"] = (ARMS["dgc_weight_decay"][0], zeros)
     engs, res = {}, {}
-    for name, (params, _) in ARMS.items():
+    for name, (params, ws) in arms.items():
         plan = BucketPlan(numels, **plan_kwargs_from_params(params))
         eng = make_engine(plan, params, device=torch.device("cuda:0"), group=None, use_history=True, blocks_per_sm=2,
-                          grad_dtype=torch.bfloat16)
-        g = (torch.randn(plan.total_elems, device="cuda:0", generator=gen) * 1e-3).to(torch.bfloat16)
-        engs[name] = (eng, g)
-        res[name] = {"elements": int(plan.total_elems), "momentum_buffer": eng.mom is not None, "ms": []}
+                          grad_dtype=torch.bfloat16, parameters=ws)
+        flat = torch.zeros(plan.total_elems, dtype=torch.bfloat16, device="cuda:0")
+        off = 0
+        for v in plan.views(flat):       # every arm exchanges the same gradients: only the memory differs
+            v.copy_(g[off:off + v.numel()].view(v.shape))
+            off += v.numel()
+        engs[name] = (eng, flat)
+        res[name] = {"elements": int(plan.total_elems), "momentum_buffer": eng.mom is not None,
+                     "weight_decay": eng.weight_decay, "ms": []}
 
     def launch(name):
         eng, g = engs[name]
@@ -118,7 +134,8 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("dgc_step.py measures on a GPU; no CUDA device is visible")
     torch.cuda.set_device(0)
-    out = {"what": "ResNet-50, bf16 buckets, top-k 1 % + bloom index, W = 1: residual vs dgc memory",
+    out = {"what": "ResNet-50, bf16 buckets, top-k 1 % + bloom index, W = 1: residual vs dgc memory vs dgc memory "
+                   "with weight decay",
            "card": card(), "exchange_kernel": exchange_kernel(args.launches, args.rounds),
            "train_step": train_step(args.steps, args.rounds, args.batch)}
     line = json.dumps(out)
