@@ -32,6 +32,7 @@ KNOWN_KEYS = frozenset({
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
     "p2_pick_mask", "fused_rle_values", "fused_dexp", "momentum", "gradient_clipping", "weight_decay",
+    "clip_norm",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -111,15 +112,25 @@ class DeepReduceConfig:
             if (isinstance(wd, bool) or not isinstance(wd, (int, float)) or not math.isfinite(float(wd))
                     or float(wd) < 0.0):
                 raise ConfigError(f"'weight_decay' must be a finite number >= 0 (got {wd!r})")
+        # ... and DGC's local gradient clipping: each tensor's gradient is scaled down to norm c / sqrt(W) before it
+        # enters the momentum, inside the memory, because no user code runs between backward and the exchange
+        if "clip_norm" in params:
+            c = params["clip_norm"]
+            if cfg.memory != "dgc":
+                raise ConfigError(f"'clip_norm' applies to 'memory': 'dgc' (got memory={cfg.memory!r})")
+            if (isinstance(c, bool) or not isinstance(c, (int, float)) or not math.isfinite(float(c))
+                    or float(c) <= 0.0):
+                raise ConfigError(f"'clip_norm' must be a finite number > 0 (got {c!r})")
         if cfg.memory == "dgc":
             if cfg.compressor == "none":
                 raise ConfigError("'memory': 'dgc' needs a sparsifier: set 'compressor' to topk/threshold/randomk")
             if cfg.beta != 1.0 or cfg.gamma != 1.0:
                 raise ConfigError(f"'memory': 'dgc' keeps the residual with beta = gamma = 1 (got beta={cfg.beta}, "
                                   f"gamma={cfg.gamma})")
-        # GRACE's DGC clips each gradient by a norm reduced across ranks; not supported
+        # GRACE's DGC clamps each gradient element-wise to a norm reduced across ranks; not supported
         if g("gradient_clipping", False) not in (False, None):
-            raise ConfigError("'gradient_clipping' is not supported; clip the gradients before the exchange instead")
+            raise ConfigError("'gradient_clipping' (GRACE's element-wise clamp to the norm reduced across ranks) is not "
+                              "supported; for DGC's per-tensor norm clipping use 'memory': 'dgc' with 'clip_norm': c")
         # opt-in wire of the fused engine's conflict_sets policy: the sender ships its pick as a bitmask over the positives
         p2 = g("p2_pick_mask", False)
         if not isinstance(p2, bool):

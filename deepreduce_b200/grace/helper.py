@@ -53,7 +53,9 @@ def grace_from_params(params: dict):
     if mem == 'residual':
         memory = ResidualMemory(params.get('beta', 1.0), params.get('gamma', 1.0))
     elif mem == 'dgc':
-        memory = DgcMemory(params.get('momentum', 0.9), params.get('weight_decay', 0.0))
+        import torch.distributed as dist
+        memory = DgcMemory(params.get('momentum', 0.9), params.get('weight_decay', 0.0), params.get('clip_norm'),
+                           dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1)
     elif mem in ('none', None):
         memory = NoneMemory()
     else:

@@ -5,12 +5,14 @@
 reference tensorflow/deepreduce.py:31-52).  Unlike GRACE the residual state is
 checkpointable (``state_dict``), see SURVEY §5.
 
-``DgcMemory``: momentum correction and momentum factor masking of Deep Gradient
-Compression (Lin et al., ICLR 2018; GRACE's DGC memory without its gradient
-clipping).  The momentum is accumulated locally, before the selection, and cleared
-wherever this rank's own decoded contribution is non-zero.
+``DgcMemory``: momentum correction, momentum factor masking and local gradient
+clipping of Deep Gradient Compression (Lin et al., ICLR 2018).  The momentum is
+accumulated locally, before the selection, and cleared wherever this rank's own
+decoded contribution is non-zero.
 """
 from __future__ import annotations
+
+import math
 
 import torch
 
@@ -28,6 +30,30 @@ def _dense(t: torch.Tensor) -> bool:
             return False
         expect *= sz
     return True
+
+
+def pairwise_sumsq(flat: torch.Tensor) -> float:
+    """The sum of fl64(x_i)^2 over the 1-D tensor ``flat`` (each square is exact in fp64), in the one order the fused
+    engine uses: zero-padded to 4096 * 2^ceil(log2 ceil(n / 4096)) elements and added by adjacent pairs,
+    ``x = x[0::2] + x[1::2]``, until one value is left (per 4096-element tile, then over the tiles)."""
+    n = flat.numel()
+    tiles = max(1, -(-n // 4096))
+    x = torch.zeros(4096 << (tiles - 1).bit_length(), dtype=torch.float64, device=flat.device)
+    x[:n] = flat.detach().double()
+    x = x * x
+    while x.numel() > 1:
+        x = x[0::2] + x[1::2]
+    return float(x.item())
+
+
+def clip_factor(sumsq: float, thr: float):
+    """DGC's local gradient clipping of one tensor with squared norm ``sumsq`` (``pairwise_sumsq``) at ``thr`` =
+    c / sqrt(W): the fp32 factor fl32(thr / nrm) where nrm = sqrt(sumsq) is finite and > thr, else None (the gradient
+    stays as it is: NaN is never > thr, and an infinite element leaves it alone too)."""
+    nrm = math.sqrt(sumsq)
+    if math.isfinite(nrm) and nrm > thr:
+        return torch.tensor(thr / nrm, dtype=torch.float32)
+    return None
 
 
 class NoneMemory(Memory):
@@ -81,11 +107,19 @@ class DgcMemory(Memory):
 
     ``weight_decay = wd > 0``: g is first replaced by ``fl(g + fl(wd * w))``, w the parameter ``bind_parameters`` bound
     to the tensor's name, as torch's momentum SGD puts the decay through its momentum buffer; the optimizer then runs
-    without weight decay too.  With ``wd = 0`` nothing is read or added."""
+    without weight decay too.  With ``wd = 0`` nothing is read or added.
 
-    def __init__(self, momentum: float = 0.9, weight_decay: float = 0.0):
+    ``clip_norm = c``: DGC's local gradient clipping, ahead of the weight decay.  Each tensor's g is replaced by
+    ``fl32(g * fl32(thr / nrm))`` where its norm ``nrm`` (fp64, ``pairwise_sumsq`` over g in storage order, the order
+    it has in a flat gradient bucket) is finite and > ``thr = c / sqrt(world_size)``.  Per tensor: the chunks of a
+    split parameter are one tensor here anyway.  With no ``clip_norm`` nothing is computed."""
+
+    def __init__(self, momentum: float = 0.9, weight_decay: float = 0.0, clip_norm=None, world_size: int = 1):
         self.momentum = float(momentum)
         self.weight_decay = float(weight_decay)
+        self.clip_norm = None if clip_norm is None else float(clip_norm)
+        self.world_size = int(world_size)
+        self.clip_thr = None if clip_norm is None else self.clip_norm / math.sqrt(self.world_size)
         self.momenta: dict[str, torch.Tensor] = {}
         self.residuals: dict[str, torch.Tensor] = {}
         self.parameters: dict[str, torch.Tensor] = {}
@@ -120,7 +154,16 @@ class DgcMemory(Memory):
                 w = w.as_strided((w.numel(),), (1,))              # storage order
         return w.reshape(shape).to(dtype)
 
+    def _clip(self, tensor):
+        flat = tensor.as_strided((tensor.numel(),), (1,)) if _dense(tensor) else tensor.reshape(-1)
+        f = clip_factor(pairwise_sumsq(flat), self.clip_thr)
+        if f is None:
+            return tensor
+        return (tensor.float() * f.to(tensor.device)).to(tensor.dtype)
+
     def compensate(self, tensor, name):
+        if self.clip_thr is not None:
+            tensor = self._clip(tensor)
         if self.weight_decay != 0.0:
             tensor = tensor + (self.weight_decay * self._weights(name, tensor.shape, tensor.dtype))
         if name in self.momenta:

@@ -638,6 +638,16 @@ struct Engine {
     P.wparams = reinterpret_cast<const unsigned long long*>(table); P.weight_decay = (float)weight_decay;
   }
 
+  // 'dgc' local gradient clipping: the scratch of the per-tile sums (fp64, one per tile) and of the factors (fp32, one
+  // per plan tensor), the {first tile, tile count} table of every plan tensor's parameter, and c / sqrt(W); part = 0:
+  // off (the 'dgc' kernels without clipping)
+  void set_clip(int64_t part, int64_t factors, int64_t owner_table, double thr) {
+    TORCH_CHECK(part == 0 || (factors != 0 && owner_table != 0 && thr > 0.0), "set_clip: incomplete clipping setup");
+    TORCH_CHECK(part == 0 || P.mom != nullptr, "set_clip: clipping runs in the 'dgc' kernels: set_momentum first");
+    P.clip_part = reinterpret_cast<double*>(part); P.clip_f = reinterpret_cast<float*>(factors);
+    P.clip_owner = reinterpret_cast<const uint32_t*>(owner_table); P.clip_thr = thr;
+  }
+
   int get_grid() {
     if (grid == 0) grid = dr::engine_max_grid(blocks_per_sm, dyn_smem);
     return grid;
@@ -865,6 +875,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("set_buffers", &Engine::set_buffers)
       .def("set_momentum", &Engine::set_momentum)
       .def("set_weight_decay", &Engine::set_weight_decay)
+      .def("set_clip", &Engine::set_clip)
       .def("set_bf16", &Engine::set_bf16)
       .def("set_poly", &Engine::set_poly)
       .def("set_shard", &Engine::set_shard)

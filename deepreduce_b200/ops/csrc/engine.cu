@@ -409,6 +409,105 @@ DR_D uint2 load_weights_bf16(const EngineParams& P, uint32_t t, uint32_t e, uint
   return make_uint2(h[0] | (h[1] << 16), h[2] | (h[3] << 16));
 }
 
+// 'dgc' local gradient clipping.  A parameter's squared norm is the sum of fl64(g_i)^2 (each square exact) over its
+// elements zero-padded to 4096 * 2^ceil(log2(tiles)), added by adjacent pairs level after level: a perfect binary tree,
+// so a tile's pairwise sum is a subtree (clip_tile_sums) and the parameter's sum is the tree over its tiles' sums
+// (clip_factors).  The fixed order is what engine_oracle and DgcMemory reproduce in torch.
+constexpr uint32_t kClipLeaves = 2048;   // tile sums reduced per shared-memory tree (a larger tree runs in blocks)
+
+DR_D double sumsq4(float4 g) {
+  const double x = g.x, y = g.y, z = g.z, w = g.w;
+  return __dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dadd_rn(__dmul_rn(z, z), __dmul_rn(w, w)));
+}
+
+// pairwise sum of buf[0 .. L) (L a power of two), each level written behind the previous one (buf holds 2L - 1
+// doubles); every thread gets the result
+DR_D double smem_pairwise(double* buf, uint32_t L) {
+  uint32_t in = 0, out = L;
+  for (uint32_t w = L >> 1; w != 0u; w >>= 1) {
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < w; i += kThreads) buf[out + i] = __dadd_rn(buf[in + 2u * i], buf[in + 2u * i + 1u]);
+    in = out; out += w;
+  }
+  __syncthreads();
+  const double s = buf[in];
+  __syncthreads();
+  return s;
+}
+
+// step 1: the pairwise sum of the squares of every tile of my accumulate range into clip_part.  Thread tid holds the
+// aligned quads tid of both half-tiles; the shuffles add adjacent lanes, so every warp sum is a subtree of 128 elements,
+// and thread 0 adds the 32 warp sums by pairs.  One more read of the gradient.
+template <bool kB>
+DR_D void clip_tile_sums(const EngineParams& P) {
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  double* red = reinterpret_cast<double*>(g_filter_smem);
+  uint32_t t0, t_end;
+  tile_range(P, kPartAccum, t0, t_end);
+  for (uint32_t tile = t0; tile < t_end; ++tile) {
+    const Tile ti = load_tile(P.tiles, tile);
+#pragma unroll
+    for (uint32_t h = 0; h < 2u; ++h) {
+      const uint32_t e0 = h * kHalf + tid * 4u;
+      float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (e0 < ti.n) {
+        if constexpr (kB) g = widen_bf16x4(__ldcs(reinterpret_cast<const uint2*>(P.grad_bf16 + ti.base + e0)));
+        else g = __ldcs(reinterpret_cast<const float4*>(P.grad + ti.base + e0));
+        if (e0 + 1u >= ti.n) g.y = 0.f;                                    // the buffers' padding is not the tensor's
+        if (e0 + 2u >= ti.n) g.z = 0.f;
+        if (e0 + 3u >= ti.n) g.w = 0.f;
+      }
+      double v = sumsq4(g);
+#pragma unroll
+      for (uint32_t o = 1; o < 32u; o <<= 1) {
+        const double p = __shfl_down_sync(0xFFFFFFFFu, v, o);
+        if ((lane & (2u * o - 1u)) == 0u) v = __dadd_rn(v, p);
+      }
+      if (lane == 0) red[h * kWarps + warp] = v;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      for (uint32_t w = kWarps; w != 0u; w >>= 1)                          // in place: pair i reads 2i, 2i + 1 >= i
+        for (uint32_t i = 0; i < w; ++i) red[i] = __dadd_rn(red[2u * i], red[2u * i + 1u]);
+      __stcg(P.clip_part + tile, red[0]);
+    }
+    __syncthreads();
+  }
+}
+
+// step 2 (after a grid barrier): the factor of every plan tensor from the tree over its parameter's tile sums.  The
+// chunks of a split parameter each compute the same tree.  The factor is read by other CTAs after the next barrier.
+DR_D void clip_factors(const EngineParams& P) {
+  double* red = reinterpret_cast<double*>(g_filter_smem);                 // 2 * kClipLeaves - 1 doubles
+  double* outer = red + 2u * kClipLeaves;                                  // block sums: <= 2^20 tiles / kClipLeaves
+  for (uint32_t t = blockIdx.x; t < P.n_tensors; t += gridDim.x) {
+    const uint2 ow = __ldg(reinterpret_cast<const uint2*>(P.clip_owner) + t);
+    uint32_t L = 1;
+    while (L < ow.y) L <<= 1;
+    double s;
+    if (L <= kClipLeaves) {
+      for (uint32_t i = threadIdx.x; i < L; i += kThreads) red[i] = i < ow.y ? __ldcg(P.clip_part + ow.x + i) : 0.0;
+      s = smem_pairwise(red, L);
+    } else {
+      for (uint32_t b = 0; b < L / kClipLeaves; ++b) {
+        for (uint32_t i = threadIdx.x; i < kClipLeaves; i += kThreads) {
+          const uint32_t j = b * kClipLeaves + i;
+          red[i] = j < ow.y ? __ldcg(P.clip_part + ow.x + j) : 0.0;
+        }
+        const double sb = smem_pairwise(red, kClipLeaves);
+        if (threadIdx.x == 0) outer[b] = sb;
+      }
+      s = smem_pairwise(outer, L / kClipLeaves);
+    }
+    if (threadIdx.x == 0) {
+      // NaN is never > thr, and an infinite norm (an infinite element) leaves the gradient untouched too
+      const double nrm = __dsqrt_rn(s);
+      const float f = (nrm > P.clip_thr && isfinite(nrm)) ? __double2float_rn(__ddiv_rn(P.clip_thr, nrm)) : 1.0f;
+      __stcg(P.clip_f + t, f);
+    }
+  }
+}
+
 // kTma = true : g / r half-tiles arrive through a CTA-wide TMA ring (cp.async.bulk + full/empty mbarriers, one producer
 //               thread); kTma = false: every THREAD copies its own float4 of g and r with cp.async (LDGSTS) into a
 //               private slot of the ring and reads it back itself — no mbarriers, no producer, warps never wait for
@@ -424,7 +523,9 @@ DR_D uint2 load_weights_bf16(const EngineParams& P, uint32_t t, uint32_t e, uint
 //               element of u is read by exactly the thread that uses it.  With weight decay (P.weight_decay != 0,
 //               CTA-uniform) the thread reads its four elements of the parameter w the same way, next to u, and adds
 //               fl(weight_decay * w) to g before the momentum; with weight_decay == 0 nothing is read or added.
-template <bool kTma, bool kFull, bool kB, bool kDgc>
+// kClip = true : 'dgc' local gradient clipping.  clip_tile_sums and clip_factors have run (two grid barriers ago), and
+//               g = fl(g * f) with the tensor's factor f ahead of everything else, where f != 1.
+template <bool kTma, bool kFull, bool kB, bool kDgc, bool kClip = false>
 DR_D void phase_accum(const EngineParams& P, Smem& sm) {
   const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
   const uint32_t parity_slot = P.epoch & 1u;
@@ -536,6 +637,8 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
     // last step's threshold bin: the guess under which digit 2 is binned speculatively (one-tile tensors finish both
     // digits from registers below and need no guess)
     const uint32_t guess = (do_hist && !single) ? __ldcg(&P.sel[cur].bin1) : 0xFFFFFFFFu;
+    float clip_f = 1.0f;
+    if constexpr (kClip) clip_f = __ldcg(P.clip_f + cur);                 // written by another CTA in this launch
     uint32_t n_mine = 0;
     uint32_t keys[8];
     while (true) {                                                         // tiles of this tensor inside my range
@@ -588,6 +691,12 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
             float4 a;
             if constexpr (kDgc) {                                          // two roundings each: no contracted FMA
               const float mu = P.momentum, wd = P.weight_decay;
+              if constexpr (kClip) {
+                if (clip_f != 1.0f) {                                      // CTA-uniform
+                  g.x = __fmul_rn(g.x, clip_f); g.y = __fmul_rn(g.y, clip_f);
+                  g.z = __fmul_rn(g.z, clip_f); g.w = __fmul_rn(g.w, clip_f);
+                }
+              }
               if (wd != 0.0f) {                                            // d = fl(g + fl(wd * w)) replaces g
                 if constexpr (kB) w = widen_bf16x4(w_bf16);
                 g.x = __fadd_rn(g.x, __fmul_rn(wd, w.x)); g.y = __fadd_rn(g.y, __fmul_rn(wd, w.y));
@@ -2285,7 +2394,7 @@ DR_D bool phase_active(const EngineParams& P, int ph) {
   }
 }
 
-template <int kMinBlocks, bool kFull, bool kB, bool kDgc = false>
+template <int kMinBlocks, bool kFull, bool kB, bool kDgc = false, bool kClip = false>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const __grid_constant__ EngineParams P) {
   __shared__ Smem sm;
   if (threadIdx.x == 0) {
@@ -2316,7 +2425,15 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
       }
     }
     switch (ph) {
-      case kPhAccum: if (P.use_tma) phase_accum<true, kFull, kB, kDgc>(P, sm); else phase_accum<false, kFull, kB, kDgc>(P, sm); break;
+      case kPhAccum:
+        if constexpr (kClip) {                 // every CTA passes both barriers, also one without tiles or tensors
+          clip_tile_sums<kB>(P);
+          grid_barrier(P.barrier, bar_epoch, P.status, P.spin_limit);
+          clip_factors(P);
+          grid_barrier(P.barrier, bar_epoch, P.status, P.spin_limit);
+        }
+        if (P.use_tma) phase_accum<true, kFull, kB, kDgc, kClip>(P, sm); else phase_accum<false, kFull, kB, kDgc, kClip>(P, sm);
+        break;
       case kPhFallback: phase_fallback<kFull>(P, sm); break;
       case kPhHist2: phase_hist2(P, sm); break;
       case kPhInsert: phase_insert(P, sm); break;
@@ -2369,8 +2486,13 @@ static const void* kernel_for(int blocks_per_sm, bool full, bool bf16) {
 }
 
 // ... and the 'dgc' memory (momentum correction + factor masking): the full feature set only, fp32 or bf16 buckets, a
-// separate instantiation again, so that the eight kernels above are compiled from unchanged code
-static const void* dgc_kernel_for(int blocks_per_sm, bool bf16) {
+// separate instantiation again, so that the eight kernels above are compiled from unchanged code; with local gradient
+// clipping one more (<.., true, .., true, true>), so that the 'dgc' kernels without it are unchanged too
+static const void* dgc_kernel_for(int blocks_per_sm, bool bf16, bool clip) {
+  if (clip) {
+    if (blocks_per_sm >= 2) return bf16 ? (const void*)dr_engine_kernel<2, true, true, true, true> : (const void*)dr_engine_kernel<2, true, false, true, true>;
+    return bf16 ? (const void*)dr_engine_kernel<1, true, true, true, true> : (const void*)dr_engine_kernel<1, true, false, true, true>;
+  }
   if (blocks_per_sm >= 2) return bf16 ? (const void*)dr_engine_kernel<2, true, true, true> : (const void*)dr_engine_kernel<2, true, false, true>;
   return bf16 ? (const void*)dr_engine_kernel<1, true, true, true> : (const void*)dr_engine_kernel<1, true, false, true>;
 }
@@ -2382,8 +2504,10 @@ static void ensure_attr() {
         cudaFuncSetAttribute(kernel_for(1, full, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         cudaFuncSetAttribute(kernel_for(2, full, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
       }
-      cudaFuncSetAttribute(dgc_kernel_for(1, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      cudaFuncSetAttribute(dgc_kernel_for(2, bf16), cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
+      for (int clip = 0; clip < 2; ++clip) {
+        cudaFuncSetAttribute(dgc_kernel_for(1, bf16, clip), cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        cudaFuncSetAttribute(dgc_kernel_for(2, bf16, clip), cudaFuncAttributeMaxDynamicSharedMemorySize, 88 * 1024);
+      }
     }
     g_attr_set = true;
   }
@@ -2400,9 +2524,9 @@ int engine_max_grid(int blocks_per_sm, int dyn_smem_bytes) {
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kernel_for(blocks_per_sm, v & 1, v >> 1), kThreads, (size_t)dyn_smem_bytes);
     if (o < occ) occ = o;
   }
-  for (int bf16 = 0; bf16 < 2; ++bf16) {
+  for (int v = 0; v < 4; ++v) {
     int o = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, dgc_kernel_for(blocks_per_sm, bf16), kThreads, (size_t)dyn_smem_bytes);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, dgc_kernel_for(blocks_per_sm, v & 1, v >> 1), kThreads, (size_t)dyn_smem_bytes);
     if (o < occ) occ = o;
   }
   if (occ < 1) occ = 1;
@@ -2419,7 +2543,7 @@ cudaError_t engine_launch(const EngineParams& P, int grid, int blocks_per_sm, in
   void* args[] = {const_cast<EngineParams*>(&P)};
   count_launch(1);
   const bool full = P.n_poly != 0 || P.n_poly_tasks != 0 || P.has_rle != 0 || P.has_shared != 0 || P.has_bf16_values != 0;
-  const void* kernel = P.mom != nullptr ? dgc_kernel_for(blocks_per_sm, P.bf16 != 0)
+  const void* kernel = P.mom != nullptr ? dgc_kernel_for(blocks_per_sm, P.bf16 != 0, P.clip_part != nullptr)
                                         : kernel_for(blocks_per_sm, full, P.bf16 != 0);
   return cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kThreads), args, (size_t)dyn_smem_bytes, stream);
 }

@@ -129,7 +129,7 @@ constexpr uint32_t kArenaHdrWords = 128;
 // and the same 22-bit rule applies to it: a superset of the K smallest hashes, plus ~numel / 2^22 elements sharing the
 // threshold's prefix.  The set depends on (numel, K, epoch, salt) only, so every rank computes the same one.
 enum Phase : int {
-  kPhAccum = 0,      // r = beta*r + gamma*g (dgc: u = m*u + g [+ wd*w], r = r + u) ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
+  kPhAccum = 0,      // r = beta*r + gamma*g (dgc: [g = f*g,] u = m*u + g [+ wd*w], r = r + u) ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
   kPhFallback = 1,   // (only if some bound was unsafe) digit 1 redone without the bound, candidate lists rebuilt in full
   kPhHist2 = 2,      // digit 2 of the candidate keys in the threshold bin
   kPhInsert = 3,     // selected candidates -> bloom filter + occupancy hint (bloom) / positive masks (raw, rle)
@@ -248,6 +248,14 @@ struct EngineParams {
   // split parameter points at its offset).  Only the tensor's numel elements are read: the padding takes w = 0.
   const unsigned long long* wparams;  // [n_tensors]
   float weight_decay;
+  // 'dgc' local gradient clipping (clip_part != nullptr, the <.., true, .., true, true> kernels): the accumulate phase
+  // first sums the squares of every parameter's gradient in fp64 by adjacent pairs (per tile into clip_part, then over
+  // the parameter's tiles), and where nrm = sqrt(sum) is finite and > clip_thr it multiplies the gradient by
+  // f = fl32(clip_thr / nrm) ahead of the weight decay and the momentum.  A split parameter's chunks share one norm.
+  double* clip_part;             // [n_tiles] scratch: pairwise sum of the squares of each tile's gradient
+  float* clip_f;                 // [n_tensors] scratch: factor of each plan tensor (1: not clipped)
+  const uint32_t* clip_owner;    // [2 * n_tensors] {first tile, tile count} of the parameter the plan tensor belongs to
+  double clip_thr;               // c / sqrt(W)
 };
 
 // Slot and slice layout, shared by the kernel and the host that launches it (binding.cpp)

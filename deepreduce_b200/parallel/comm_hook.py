@@ -22,6 +22,8 @@ stepping the DDP model must run without one (e.g. ``torch.optim.SGD(..., momentu
 the dict the memory adds the decay ahead of its momentum, reading the parameters of each bucket, so that optimizer also
 runs with ``weight_decay=0``.  The parameters are read in the order of their gradients in the bucket, i.e. in their
 storage order, which DDP gives a dense parameter's gradient; their layouts must not change after DDP built its buckets.
+``'clip_norm'`` clips each parameter's gradient inside the memory, in both routes, because the hook runs inside backward
+and no user code can clip in between; the norm is per parameter, summed in the gradient's order in the bucket.
 """
 from typing import Dict, List, Optional, Sequence, Tuple
 

@@ -180,7 +180,7 @@ def engine_split_numel(params: dict, blocks_per_sm: int) -> int:
 
 
 def engine_kwargs(params: dict) -> dict:
-    """The ``BucketEngine`` memory arguments for ``params``: beta, gamma, momentum, weight decay and averaging.  They
+    """The ``BucketEngine`` memory arguments for ``params``: beta, gamma, momentum, weight decay, clipping and averaging.  They
     follow the per-tensor memory GRACE builds for the same dict: only ``ResidualMemory`` scales the gradient by gamma,
     so 'none' and 'dgc' memory run with gamma = 1 ('dgc' accepts no other), and without a residual beta is 0."""
     memory = params.get('memory', 'none')
@@ -188,16 +188,18 @@ def engine_kwargs(params: dict) -> dict:
                 gamma=float(params.get('gamma', 1.0)) if memory == 'residual' else 1.0,
                 average=params.get('average', True),
                 momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None,
-                weight_decay=float(params.get('weight_decay', 0.0)) if memory == 'dgc' else 0.0)
+                weight_decay=float(params.get('weight_decay', 0.0)) if memory == 'dgc' else 0.0,
+                clip_norm=float(params['clip_norm']) if memory == 'dgc' and 'clip_norm' in params else None)
 
 
 def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: bool, blocks_per_sm: int,
                 grad_dtype: torch.dtype, parameters=None, owner=None) -> BucketEngine:
     """The ``BucketEngine`` of one bucket for ``params`` (memory arguments from ``engine_kwargs``), with its tile
     partitions calibrated unless ``'calibrate_partition': False``.  ``parameters`` / ``owner``: the bucket's parameters
-    and the plan tensors' owners (``split_large``), bound when the engine applies weight decay.  Collective at W > 1."""
+    and the plan tensors' owners (``split_large``), bound when the engine applies weight decay; ``owner`` also makes
+    the chunks of a split parameter one tensor for ``'clip_norm'``.  Collective at W > 1."""
     eng = BucketEngine(plan, device=device, group=group, use_history=use_history, blocks_per_sm=blocks_per_sm,
-                       grad_dtype=grad_dtype, **engine_kwargs(params))
+                       grad_dtype=grad_dtype, owner=owner, **engine_kwargs(params))
     if eng.weight_decay != 0.0:
         if parameters is None:
             raise ValueError("'weight_decay' reads the parameters: make_engine needs the bucket's parameters")

@@ -36,6 +36,7 @@ from ..codecs.bf16 import bf16_bits_oracle, bf16_widen_oracle
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
 from ..codecs.polyfit import get_segments, polyfit_eval_oracle, polyfit_fit_oracle
 from ..codecs.qsgd import qsgd_decode_oracle, qsgd_encode_oracle
+from ..grace.memory import clip_factor, pairwise_sumsq
 from .plan import update_cta_speeds
 from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID, SLOT_HEADER_WORDS,
                    VMODE_BF16, VMODE_DEXP, VMODE_QSGD, BucketPlan, rle_stream_words)
@@ -313,9 +314,50 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
     return resid, sel, vals
 
 
+def owner_spans(plan: BucketPlan, owner: Optional[Sequence[int]] = None) -> list:
+    """Per plan tensor, (first tile, tile count) of the parameter it belongs to: ``owner[j]`` is the parameter of plan
+    tensor j (``split_large``; default: one each).  A parameter's chunks must be consecutive plan tensors."""
+    tensors = plan.tensors
+    owner = list(range(len(tensors))) if owner is None else [int(o) for o in owner]
+    if len(owner) != len(tensors):
+        raise ValueError(f"owner has {len(owner)} entries for the plan's {len(tensors)} tensors")
+    spans, j = [None] * len(tensors), 0
+    while j < len(tensors):
+        k = j
+        while k + 1 < len(tensors) and owner[k + 1] == owner[j]:
+            k += 1
+        if owner[j] in owner[:j]:
+            raise ValueError(f"owner {owner}: the chunks of parameter {owner[j]} are not consecutive")
+        span = (tensors[j].tile_begin, sum(tensors[i].n_tiles for i in range(j, k + 1)))
+        for i in range(j, k + 1):
+            spans[i] = span
+        j = k + 1
+    return spans
+
+
+def clip_oracle(plan: BucketPlan, g: torch.Tensor, thr: float, owner: Optional[Sequence[int]] = None) -> torch.Tensor:
+    """'dgc' local gradient clipping of the flat fp32 gradient ``g`` (plan layout) at ``thr`` = c / sqrt(W): per
+    parameter (the chunks of ``owner`` together), the squared norm by ``pairwise_sumsq`` over its elements in plan
+    order, and g = fl32(g * f) where ``clip_factor`` gives a factor."""
+    g = g.clone()
+    spans = owner_spans(plan, owner)
+    j = 0
+    while j < len(plan.tensors):
+        k = j
+        while k + 1 < len(plan.tensors) and spans[k + 1] == spans[j]:
+            k += 1
+        chunks = [slice(t.elem_off, t.elem_off + t.numel) for t in plan.tensors[j:k + 1]]
+        f = clip_factor(pairwise_sumsq(torch.cat([g[c] for c in chunks])), thr)
+        if f is not None:
+            for c in chunks:
+                g[c] = g[c] * f
+        j = k + 1
+    return g
+
+
 def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Sequence[torch.Tensor], *, beta=1.0,
                   gamma=1.0, average=True, seed=spec.DEFAULT_SEED, epoch=1, momentum=None, moms=None,
-                  weight_decay=0.0, weights=None):
+                  weight_decay=0.0, weights=None, clip_norm=None, owner=None):
     """One bucket step for W ranks on the CPU.  grads/resids: per-rank flat
     buffers (plan.total_elems).  Returns (dense_out, new_resids, slots).
 
@@ -324,18 +366,25 @@ def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Seque
     the rank's own decoded value is non-zero; returns (dense_out, new_resids, slots, new_moms).
 
     ``weight_decay`` wd != 0 (with ``momentum``): ``weights`` are the per-rank parameters, flat in plan layout (zeros in
-    the padding), and g is replaced by d = g + (wd * w), two roundings, before the momentum."""
+    the padding), and g is replaced by d = g + (wd * w), two roundings, before the momentum.
+
+    ``clip_norm`` c (with ``momentum``): ahead of that, each rank's gradient is clipped per parameter at c / sqrt(W)
+    (``clip_oracle``; ``owner`` maps the plan tensors to parameters as ``split_large`` returns it)."""
     W = len(grads)
     dgc = momentum is not None
     if dgc and (beta != 1.0 or gamma != 1.0 or moms is None or len(moms) != W):
         raise ValueError("engine_oracle: momentum needs beta = gamma = 1 and one momentum buffer per rank")
     if weight_decay != 0.0 and (not dgc or weights is None or len(weights) != W):
         raise ValueError("engine_oracle: weight_decay needs momentum and one parameter buffer per rank")
+    if clip_norm is not None and not dgc:
+        raise ValueError("engine_oracle: clip_norm needs momentum")
     out = torch.zeros(plan.total_elems, dtype=torch.float32)
     new_resids, slots, new_moms = [], [], []
     for r in range(W):
         g = grads[r].detach().cpu().float()
         res = resids[r].detach().cpu().float()
+        if clip_norm is not None:
+            g = clip_oracle(plan, g, float(clip_norm) / math.sqrt(W), owner)
         if weight_decay != 0.0:
             g = g + (float(weight_decay) * weights[r].detach().cpu().float())
         if dgc:
@@ -495,7 +544,8 @@ class BucketEngine:
                  rank: Optional[int] = None, filter_smem_bytes: Optional[int] = None, use_tma: bool = True,
                  hist_shift: int = 22, shard: Optional[bool] = None, transport: Optional[str] = None,
                  peer_timeout_ms: Optional[int] = None, fault: int = 0, grad_dtype: torch.dtype = torch.float32,
-                 momentum: Optional[float] = None, weight_decay: float = 0.0):
+                 momentum: Optional[float] = None, weight_decay: float = 0.0, clip_norm: Optional[float] = None,
+                 owner: Optional[Sequence[int]] = None):
         # grad_dtype=torch.bfloat16: the flat gradient (in: local, out: aggregate) is bf16.  The residual, the select,
         # the codecs and the wire stay fp32 (widening bf16 is exact), so the engine computes exactly what an fp32 engine
         # fed the widened gradient computes, and rounds the aggregate once (to nearest even) where it is final.  The
@@ -517,6 +567,16 @@ class BucketEngine:
             raise ValueError("weight_decay is added inside the 'dgc' memory: it needs momentum")
         self.weight_decay = float(wd)
         self._bound = None                       # (parameters, owner, data_ptrs, strides) of the last bind_parameters
+        # clip_norm=c ('dgc' only): DGC's local gradient clipping of every parameter at c / sqrt(W), ahead of the weight
+        # decay; ``owner`` (split_large) makes the chunks of a split parameter one norm (engine_oracle(clip_norm=...))
+        c = clip_norm
+        if c is not None:
+            if isinstance(c, bool) or not isinstance(c, (int, float)) or not math.isfinite(c) or c <= 0:
+                raise ValueError(f"clip_norm must be a finite number > 0 (got {c!r})")
+            if momentum is None:
+                raise ValueError("clip_norm clips inside the 'dgc' memory: it needs momentum")
+        self.clip_norm = None if c is None else float(c)
+        self.owner = None if owner is None else [int(o) for o in owner]
         from .. import ops
         self.mod = ops.cuda_module()
         self.plan = plan
@@ -584,6 +644,15 @@ class BucketEngine:
                 self.ctx.set_momentum(self.mom.data_ptr(), self.momentum)
             # one parameter address per plan tensor (bind_parameters); the kernel reads it only when weight_decay != 0
             self.wparams = torch.zeros(nT, dtype=torch.int64, device=dev)
+            self.clip_thr = None
+            if self.clip_norm is not None:
+                self.clip_thr = self.clip_norm / math.sqrt(self.world)
+                spans = owner_spans(plan, self.owner)
+                self.clip_owner = torch.tensor([v for sp in spans for v in sp], dtype=torch.int32, device=dev)
+                self.clip_part = torch.zeros(nt, dtype=torch.float64, device=dev)
+                self.clip_f = torch.ones(nT, dtype=torch.float32, device=dev)
+                self.ctx.set_clip(self.clip_part.data_ptr(), self.clip_f.data_ptr(), self.clip_owner.data_ptr(),
+                                  self.clip_thr)
             if grad_dtype == torch.bfloat16:
                 # fp32 sums of the bloom apply (every sender of a tile is added before the one rounding): one 4096-float
                 # row per tile this rank decodes; not needed when every bloom tensor is scattered by emit (W = 1, fp32

@@ -86,6 +86,7 @@ def _bits_equal_across_ranks(x: torch.Tensor, group=None) -> bool:
 def multi_gpu_check(engine, seed: int = 4242) -> dict:
     """Run one checked exchange step on ``engine`` (a live ``BucketEngine``; its residual / epoch advance by one
     step).  Returns ``{"status": "ok" | "FAILED: ...", ...details}``; collective — every rank must call it."""
+    from ..parallel.engine import clip_oracle
     W, rank, plan = engine.world, engine.rank, engine.plan
     dev = engine.device
     gen = torch.Generator(device=dev).manual_seed(seed + 1000 * rank)
@@ -94,7 +95,8 @@ def multi_gpu_check(engine, seed: int = 4242) -> dict:
         v.copy_(torch.randn(v.shape, device=dev, generator=gen) * 1e-2)
     g = g.to(engine.grad.dtype).float()         # bf16 engine: the widened bf16 gradient is what the engine accumulates
     if engine.mom is not None:                  # 'dgc': the momentum is compensated, then added to the residual
-        d = g + (engine.weight_decay * engine.parameter_buffer()) if engine.weight_decay != 0.0 else g
+        c = clip_oracle(plan, g, engine.clip_thr, engine.owner) if engine.clip_thr is not None else g
+        d = c + (engine.weight_decay * engine.parameter_buffer()) if engine.weight_decay != 0.0 else c
         acc = engine.resid + (engine.momentum * engine.mom + d)
     else:
         acc = engine.beta * engine.resid + engine.gamma * g if engine.beta != 0.0 else engine.gamma * g
