@@ -15,7 +15,9 @@ from __future__ import annotations
 import math
 import warnings
 from dataclasses import asdict, dataclass
-from typing import Optional
+from typing import Optional, Tuple
+
+from . import spec
 
 COMPRESSORS = ("none", "topk", "threshold", "randomk")
 OUT_OF_SCOPE_COMPRESSORS = ("SKCompressCPU", "SKCompressGPU", "sketch")        # comparison baselines of a GRACE fork
@@ -32,7 +34,7 @@ KNOWN_KEYS = frozenset({
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
     "p2_pick_mask", "fused_rle_values", "fused_dexp", "momentum", "gradient_clipping", "weight_decay",
-    "clip_norm",
+    "clip_norm", "warmup_ratios", "warmup_steps",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -66,6 +68,8 @@ class DeepReduceConfig:
     world_size: Optional[int] = None
     hint: bool = True
     min_numel: int = 1000
+    warmup_ratios: Optional[Tuple[float, ...]] = None
+    warmup_steps: Optional[int] = None
 
     # ------------------------------------------------------------------
     @classmethod
@@ -95,6 +99,10 @@ class DeepReduceConfig:
             world_size=None if g("world_size", None) is None else int(g("world_size")),
             hint=bool(g("hint", True)), min_numel=int(g("min_numel", 1000)))
         cfg.validate()
+        wu = warmup_from_params(params)
+        if wu is not None:
+            object.__setattr__(cfg, "warmup_ratios", wu.ratios)
+            object.__setattr__(cfg, "warmup_steps", wu.steps)
         # 'dgc' memory (momentum correction + momentum factor masking, Lin et al. 2018): the momentum factor rides in
         # 'momentum'; it replaces the optimizer's momentum, and the residual it keeps is the plain one (beta = gamma = 1)
         if "momentum" in params:
@@ -203,11 +211,40 @@ class DeepReduceConfig:
             need(self.communicator == "allgather",
                  f"compressor {self.compressor!r} produces per-rank index sets: use 'communicator': 'allgather'")
 
+    def ratio_at(self, exchange: int) -> float:
+        """Compress ratio of the 0-based ``exchange`` (``spec.Warmup``; ``compress_ratio`` without a warm-up)."""
+        if self.warmup_ratios is None:
+            return self.compress_ratio
+        return spec.Warmup(self.warmup_ratios, self.warmup_steps, self.compress_ratio).ratio_at(exchange)
+
     def to_params(self) -> dict:
         """Back to the dict form the codecs/wrappers take (a fresh dict; the 'micro-benchmark' key keeps its dash)."""
         d = asdict(self)
         d["micro-benchmark"] = d.pop("micro_benchmark")
         return {k: v for k, v in d.items() if v is not None}
+
+
+def warmup_from_params(params: dict) -> Optional[spec.Warmup]:
+    """The sparsity warm-up of ``params`` (``'warmup_ratios'``: a non-empty list of compress ratios in (0, 1],
+    ``'warmup_steps'``: exchanges per stage, an int >= 1), validated; None when neither key is given."""
+    has_r, has_s = "warmup_ratios" in params, "warmup_steps" in params
+    if not (has_r or has_s):
+        return None
+    if has_r != has_s:
+        raise ConfigError("'warmup_ratios' and 'warmup_steps' go together: give both or neither")
+    comp = params.get("compressor", "none") or "none"
+    if comp not in ("topk", "randomk"):
+        raise ConfigError(f"the sparsity warm-up schedules the compress ratio of 'topk' or 'randomk' (got "
+                          f"compressor={comp!r})")
+    rs, n = params["warmup_ratios"], params["warmup_steps"]
+    if not isinstance(rs, (list, tuple)) or not rs:
+        raise ConfigError(f"'warmup_ratios' must be a non-empty list of numbers in (0, 1] (got {rs!r})")
+    for r in rs:
+        if isinstance(r, bool) or not isinstance(r, (int, float)) or not 0.0 < float(r) <= 1.0:
+            raise ConfigError(f"'warmup_ratios' must be a non-empty list of numbers in (0, 1] (got {rs!r})")
+    if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+        raise ConfigError(f"'warmup_steps' must be an int >= 1 (got {n!r})")
+    return spec.Warmup(tuple(float(r) for r in rs), int(n), float(params.get("compress_ratio", 0.01)))
 
 
 def validate_params(params: dict, *, strict: bool = False) -> DeepReduceConfig:

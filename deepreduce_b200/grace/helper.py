@@ -27,6 +27,11 @@ def tensor_bits(tensors: Iterable) -> int:
     return total
 
 
+def sparsifier_of(grc):
+    """The sparsifier of a GRACE communicator, under the DeepReduce codec wrapper if there is one."""
+    return getattr(grc.compressor, "sparsifier", grc.compressor)
+
+
 def grace_from_params(params: dict):
     """Build ``Communicator(compressor, memory)`` from the GRACE params dict
     (reference README.md:36-38)."""
@@ -36,12 +41,14 @@ def grace_from_params(params: dict):
     world_size = params.get('world_size', None)
     average = params.get('average', True)
 
+    from ..config import warmup_from_params
+    warmup = warmup_from_params(params)
     if comp == 'topk':
-        compressor = TopKCompressor(params.get('compress_ratio', 0.01), average=average)
+        compressor = TopKCompressor(params.get('compress_ratio', 0.01), average=average, warmup=warmup)
     elif comp == 'threshold':
         compressor = ThresholdCompressor(params.get('threshold', 0.0), average=average)
     elif comp == 'randomk':
-        compressor = RandomKCompressor(params.get('compress_ratio', 0.01), average=average)
+        compressor = RandomKCompressor(params.get('compress_ratio', 0.01), average=average, warmup=warmup)
     elif comp in ('none', None):
         compressor = NoneCompressor(average=average)
     elif comp in ('SKCompressCPU', 'SKCompressGPU', 'sketch'):

@@ -33,14 +33,38 @@ class NoneCompressor(Compressor):
         return tensors[0]
 
 
-class TopKCompressor(Compressor):
-    def __init__(self, compress_ratio: float = 0.01, average: bool = True):
-        super().__init__(average=average, tensors_size_are_same=True)
+class _Scheduled:
+    """The sparsity warm-up of a ratio sparsifier (``spec.Warmup``, or None: ``compress_ratio`` throughout).  A bare
+    ``grc.step(grad, name)`` has no other step counter, so the exchanges are counted per tensor name: a tensor that
+    gets no gradient on some step falls behind in its count by that step."""
+
+    def _init_warmup(self, compress_ratio, warmup):
         self.compress_ratio = compress_ratio
+        self.warmup = warmup
+        self.exchanges: dict = {}
+
+    def _ratio(self, name) -> float:
+        if self.warmup is None:
+            return self.compress_ratio
+        e = self.exchanges.get(name, 0)
+        self.exchanges[name] = e + 1
+        return self.warmup.ratio_at(e)
+
+    def state_dict(self) -> dict:
+        return {"exchanges": dict(self.exchanges)}
+
+    def load_state_dict(self, state: dict) -> None:
+        self.exchanges = {k: int(v) for k, v in state.get("exchanges", {}).items()}
+
+
+class TopKCompressor(_Scheduled, Compressor):
+    def __init__(self, compress_ratio: float = 0.01, average: bool = True, warmup: spec.Warmup | None = None):
+        super().__init__(average=average, tensors_size_are_same=True)
+        self._init_warmup(compress_ratio, warmup)
 
     def compress(self, tensor, name):
         flat = tensor.flatten()
-        k = spec.topk_k(flat.numel(), self.compress_ratio)
+        k = spec.topk_k(flat.numel(), self._ratio(name))
         if flat.is_cuda:
             from .. import ops
             values, indices = ops.topk_select(flat, k)
@@ -71,20 +95,21 @@ class ThresholdCompressor(Compressor):
         return _desparsify(tensors, ctx)
 
 
-class RandomKCompressor(Compressor):
+class RandomKCompressor(_Scheduled, Compressor):
     """Uniform random K coordinates, the same on every rank for a given
     (step, name) — TF twin: tensorflow/deepreduce.py:290-298."""
 
-    def __init__(self, compress_ratio: float = 0.01, average: bool = True, seed: int = 1):
+    def __init__(self, compress_ratio: float = 0.01, average: bool = True, seed: int = 1,
+                 warmup: spec.Warmup | None = None):
         super().__init__(average=average, tensors_size_are_same=True)
-        self.compress_ratio = compress_ratio
+        self._init_warmup(compress_ratio, warmup)
         self.seed = seed
         self.global_step = 0
 
     def compress(self, tensor, name):
         flat = tensor.flatten()
         d = flat.numel()
-        k = spec.topk_k(d, self.compress_ratio)
+        k = spec.topk_k(d, self._ratio(name))
         tid = sum(name.encode()) if isinstance(name, str) else int(name)
         seed = spec.policy_seed(self.global_step + self.seed, tid)
         self.global_step += 1

@@ -31,7 +31,8 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
-from .ddp import BUCKET_DTYPES, engine_split_numel, fused_path, make_engine, plan_kwargs_from_params
+from ..grace.helper import sparsifier_of
+from .ddp import BUCKET_DTYPES, engine_split_numel, fused_path, make_engine, stage_plans
 from .engine import STATUS_NAMES, BucketEngine
 from .plan import BucketPlan, split_large
 
@@ -117,6 +118,8 @@ class DeepReduceHookState:
         self.average = bool(self.params.get('average', True))
         self.dense = self.params.get('compressor', 'none') in ('none', None)
         self.fused_params = not self.dense and fused_path(self.params)
+        from ..config import warmup_from_params
+        self.warmup = warmup_from_params(self.params)   # sparsity warm-up: stages counted in exchanges (hook calls)
         self._names: Dict[int, str] = {id(p): n for n, p in module.named_parameters()}
         self._layouts: List[_Layout] = []            # every engine not yet closed
         self._by_index: Dict[int, _Layout] = {}      # the layout a bucket index had last
@@ -125,6 +128,7 @@ class DeepReduceHookState:
         self._pending_mom: Dict[str, torch.Tensor] = {}  # ... and their loaded 'dgc' momenta
         self.dgc = self.params.get('memory') == 'dgc'
         self._pending_epoch = 0
+        self._plans: Dict[tuple, list] = {}          # warm-up: every stage's plan of a layout, built when first met
         self._stream: Optional[torch.cuda.Stream] = None
         self.grc = None
         self.step_count = 0
@@ -219,26 +223,36 @@ class DeepReduceHookState:
     def _layout_for(self, bucket, buf) -> _Layout:
         params = bucket.parameters()
         segments = bucket_segments(bucket)
-        key = (bucket.index(), tuple(id(p) for p in params), tuple(segments), buf.numel(), buf.dtype)
+        # the warm-up stage is part of the layout: a new stage builds the stage's engine and carries the state into it
+        stage = 0 if self.warmup is None else self.warmup.stage(self.step_count)
+        key = (bucket.index(), tuple(id(p) for p in params), tuple(segments), buf.numel(), buf.dtype, stage)
         lay = self._by_index.get(bucket.index())
         if lay is not None and lay.key == key:
             return lay
-        return self._new_layout(key, bucket.index(), params, segments, buf)
+        return self._new_layout(key, bucket.index(), params, segments, buf, stage)
 
-    def _new_layout(self, key, index, params, segments, buf) -> _Layout:
+    def _new_layout(self, key, index, params, segments, buf, stage=0) -> _Layout:
         """Plan, engine and segment table of a layout met for the first time, with the residuals carried over.
 
         Collective at W > 1 (IPC handle exchange and barriers in ``BucketEngine``, the partition calibration's exchange
         steps, and ``BucketEngine.close`` of a superseded engine), here inside a DDP hook.  That is safe only because
         every rank meets the same layouts in the same order: DDP calls the hook in bucket-index order, and its bucket
-        rebuild broadcasts rank 0's order, so every rank builds and closes the same engines at the same point."""
+        rebuild broadcasts rank 0's order, so every rank builds and closes the same engines at the same point.  A
+        sparsity warm-up stage switch meets every bucket again, on the same exchange on every rank (each counts the same
+        hook calls).  Every stage's plan of a layout is built when the layout is first met (and kept), so a stage a plan
+        refuses raises on the first exchange."""
         from .. import ops
         names = [self._name(p) for p in params]
         numels = [n for _, n in segments]
         shapes = [tuple(p.shape) for p in params]
         numels, pnames, shapes, owner = split_large(numels, names, shapes,
                                                      engine_split_numel(self.params, self.blocks_per_sm))
-        plan = BucketPlan(numels, pnames, shapes, **plan_kwargs_from_params(self.params))
+        plans = self._plans.get(key[:-1])
+        if plans is None:
+            plans = stage_plans(numels, pnames, shapes, self.params, self.warmup)
+            if self.warmup is not None:
+                self._plans[key[:-1]] = plans
+        plan = plans[stage]
         # 'weight_decay': the engine reads every parameter in storage order, where the bucket holds its gradient (DDP
         # lays a dense parameter's gradient out with the parameter's strides; bind_parameters refuses any other).  The
         # parameters' layouts are recorded here and must stay as DDP found them: a later change raises at the next step
@@ -257,6 +271,11 @@ class DeepReduceHookState:
                 dst.copy_(old.resid_of(p))
                 if self.dgc:
                     lay.mom_of(p).copy_(old.mom_of(p))
+                if self.warmup is not None:
+                    # a warm-up run's engines only move their epochs forward, across stage switches and DDP's rebuild
+                    # alike; without the keys a new layout keeps its own count, as it always has (its arena is new
+                    # and zeroed, so no stale flag can match)
+                    eng.epoch = max(eng.epoch, old.engine.epoch)
                 old.live -= 1
                 if old.live == 0:
                     self._close_layout(old)
@@ -357,6 +376,8 @@ class DeepReduceHookState:
             out["momentum"] = mom
         if self.grc is not None:
             out["memory"] = self.grc.memory.state_dict()
+            if self.warmup is not None:               # the per-name exchange counts of the warm-up
+                out["sparsifier"] = sparsifier_of(self.grc).state_dict()
         return out
 
     def load_state_dict(self, state: dict):
@@ -387,6 +408,8 @@ class DeepReduceHookState:
                 self._make_grc()
             dev = next(self.module.parameters()).device
             self.grc.memory.load_state_dict(state["memory"], device=dev)
+            if self.warmup is not None:               # a checkpoint from before the warm-up: every count at 0
+                sparsifier_of(self.grc).load_state_dict(state.get("sparsifier", {}))
 
     def close(self):
         """Release the engines and their arenas (collective at W > 1)."""

@@ -25,6 +25,7 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from .. import spec
+from ..grace.helper import sparsifier_of
 from ..wrappers import deepreduce_from_params
 from .engine import BucketEngine
 from .plan import BucketPlan
@@ -192,14 +193,46 @@ def engine_kwargs(params: dict) -> dict:
                 clip_norm=float(params['clip_norm']) if memory == 'dgc' and 'clip_norm' in params else None)
 
 
+def stage_plans(numels, names, shapes, params: dict, warmup) -> List[BucketPlan]:
+    """The ``BucketPlan`` of every sparsity warm-up stage (``spec.Warmup``) of one bucket, over the same list of plan
+    tensors, the last one at ``'compress_ratio'``; without a warm-up, the one plan of ``params``.  The chunking
+    (``engine_split_numel``) follows the final ratio, so the tile offsets and ``total_elems`` are those of the final
+    plan in every stage and only K, the filter sizes and the slot layout change.  Built up front: a stage a plan
+    refuses (e.g. P2's positive limit at a dense ratio) raises before the first exchange."""
+    kw = plan_kwargs_from_params(params)
+    if warmup is None:
+        return [BucketPlan(numels, names, shapes, **kw)]
+    return [BucketPlan(numels, names, shapes, **{**kw, 'compress_ratio': warmup.ratio(s)})
+            for s in range(warmup.n_stages)]
+
+
+def switch_engine(old: BucketEngine, build) -> BucketEngine:
+    """A sparsity warm-up stage switch of one bucket: ``build(grad)`` makes the new stage's engine adopting ``grad``, the
+    old engine's gradient buffer (``make_engine(..., grad=grad)``; collective at W > 1, like everything here), so
+    ``p.grad`` keeps viewing it.  The buffer's aggregate is saved across the build, whose partition calibration writes
+    it; the stages share one layout, so the residual and the 'dgc' momentum carry over as whole buffers, bit for bit;
+    the select history does not (the selection is exact without it); the epoch only moves forward; the old engine is
+    closed.  Returns the new engine."""
+    agg = old.grad.clone()
+    new = build(old.grad)
+    new.grad.copy_(agg)
+    new.resid.copy_(old.resid)
+    if new.mom is not None:
+        new.mom.copy_(old.mom)
+    new.epoch = max(new.epoch, old.epoch)
+    old.close()
+    return new
+
+
 def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: bool, blocks_per_sm: int,
-                grad_dtype: torch.dtype, parameters=None, owner=None) -> BucketEngine:
+                grad_dtype: torch.dtype, parameters=None, owner=None, grad=None) -> BucketEngine:
     """The ``BucketEngine`` of one bucket for ``params`` (memory arguments from ``engine_kwargs``), with its tile
     partitions calibrated unless ``'calibrate_partition': False``.  ``parameters`` / ``owner``: the bucket's parameters
     and the plan tensors' owners (``split_large``), bound when the engine applies weight decay; ``owner`` also makes
-    the chunks of a split parameter one tensor for ``'clip_norm'``.  Collective at W > 1."""
+    the chunks of a split parameter one tensor for ``'clip_norm'``.  ``grad``: the flat gradient buffer to adopt
+    (``BucketEngine``); the calibration overwrites it.  Collective at W > 1."""
     eng = BucketEngine(plan, device=device, group=group, use_history=use_history, blocks_per_sm=blocks_per_sm,
-                       grad_dtype=grad_dtype, owner=owner, **engine_kwargs(params))
+                       grad_dtype=grad_dtype, owner=owner, grad=grad, **engine_kwargs(params))
     if eng.weight_decay != 0.0:
         if parameters is None:
             raise ValueError("'weight_decay' reads the parameters: make_engine needs the bucket's parameters")
@@ -248,6 +281,9 @@ class DeepReduceDDP:
         self._status_host = None          # pinned copies of the engines' status words (async check)
         self._status_event = None
         self.overlap_grid_cap = int(overlap_grid if overlap_grid is not None else (self.params.get('overlap_grid', 0) or 0))
+        from ..config import warmup_from_params
+        self.warmup = warmup_from_params(self.params)        # sparsity warm-up: stages counted in exchanges (finish())
+        self.stage = 0
         if self.world > 1 and broadcast_parameters:
             # replicas must start from the same weights: rank 0's parameters and buffers win (torch DDP does the same)
             with torch.no_grad():
@@ -269,6 +305,8 @@ class DeepReduceDDP:
     # ---- bucket construction ------------------------------------------------
     def _build_buckets(self, cap_mb, blocks_per_sm, use_history):
         self.buckets: List[List] = group_buckets(self.named, cap_mb)
+        self._plans: List[List[BucketPlan]] = []           # fused: [bucket][warm-up stage]
+        self._engine_args: List[dict] = []
         for b, items in enumerate(self.buckets):
             dtype = items[0][1].dtype
             numels = [p.numel() for _, p in items]
@@ -281,10 +319,12 @@ class DeepReduceDDP:
                     from .plan import split_large
                     numels, names, shapes, owner = split_large(numels, names, shapes, int(sn))
             if self.fused:
-                plan = BucketPlan(numels, names, shapes, **plan_kwargs_from_params(self.params))
-                eng = make_engine(plan, self.params, device=self.device, group=self.group, use_history=use_history,
-                                  blocks_per_sm=blocks_per_sm, grad_dtype=dtype, parameters=[p for _, p in items],
-                                  owner=owner)
+                self._plans.append(stage_plans(numels, names, shapes, self.params, self.warmup))
+                self._engine_args.append(dict(device=self.device, group=self.group, use_history=use_history,
+                                              blocks_per_sm=blocks_per_sm, grad_dtype=dtype,
+                                              parameters=[p for _, p in items], owner=owner))
+                plan = self._plans[b][self.stage]
+                eng = make_engine(plan, self.params, **self._engine_args[b])
                 self.engines.append(eng)
                 flat, views = eng.grad, eng.grad_views
             else:
@@ -400,6 +440,17 @@ class DeepReduceDDP:
                 for f in self.flat:
                     f.div_(self.world)
         self.step_count += 1
+        if self.fused and self.warmup is not None and self.warmup.stage(self.step_count) != self.stage:
+            self._switch_stage(self.warmup.stage(self.step_count))
+
+    def _switch_stage(self, stage: int):
+        """Move every bucket to the engine of warm-up ``stage`` between two exchanges (``switch_engine``; collective at
+        W > 1: every rank counts the same exchanges, so all switch after the same ``finish()``).  ``p.grad`` still
+        holds this exchange's aggregate for the optimizer step."""
+        for b, old in enumerate(self.engines):
+            plan, args = self._plans[b][stage], self._engine_args[b]
+            self.engines[b] = switch_engine(old, lambda grad: make_engine(plan, self.params, grad=grad, **args))
+        self.stage = stage
 
     def _check_grad_views(self):
         """``p.grad`` must still be the view into the flat bucket: ``optimizer.zero_grad(set_to_none=True)`` (torch's
@@ -484,16 +535,24 @@ class DeepReduceDDP:
         if self.fused:
             return {"step": self.step_count, "engines": [e.state_dict() for e in self.engines]}
         if self.grc is not None:
-            return {"step": self.step_count, "memory": self.grc.memory.state_dict()}
+            out = {"step": self.step_count, "memory": self.grc.memory.state_dict()}
+            if self.warmup is not None:               # the per-name exchange counts of the warm-up
+                out["sparsifier"] = sparsifier_of(self.grc).state_dict()
+            return out
         return {"step": self.step_count}
 
     def load_state_dict(self, state):
         self.step_count = int(state.get("step", 0))
         if self.fused:
+            if self.warmup is not None and self.warmup.stage(self.step_count) != self.stage:
+                self._switch_stage(self.warmup.stage(self.step_count))
             for e, s in zip(self.engines, state["engines"]):
                 e.load_state_dict(s)
-        elif self.grc is not None and "memory" in state:
-            self.grc.memory.load_state_dict(state["memory"], device=self.device)
+        elif self.grc is not None:
+            if "memory" in state:
+                self.grc.memory.load_state_dict(state["memory"], device=self.device)
+            if self.warmup is not None:               # a checkpoint from before the warm-up: every count at 0
+                sparsifier_of(self.grc).load_state_dict(state.get("sparsifier", {}))
 
     def close(self):
         for h in self._handles:

@@ -545,7 +545,10 @@ class BucketEngine:
                  hist_shift: int = 22, shard: Optional[bool] = None, transport: Optional[str] = None,
                  peer_timeout_ms: Optional[int] = None, fault: int = 0, grad_dtype: torch.dtype = torch.float32,
                  momentum: Optional[float] = None, weight_decay: float = 0.0, clip_norm: Optional[float] = None,
-                 owner: Optional[Sequence[int]] = None):
+                 owner: Optional[Sequence[int]] = None, grad: Optional[torch.Tensor] = None):
+        # grad: adopt this flat gradient buffer (``plan.total_elems`` of ``grad_dtype`` on ``device``) instead of
+        # allocating one, so that views into it (``p.grad``) stay valid across engines of the same layout (the sparsity
+        # warm-up's stage switch); calibrate_partition scribbles on it like on an own buffer
         # grad_dtype=torch.bfloat16: the flat gradient (in: local, out: aggregate) is bf16.  The residual, the select,
         # the codecs and the wire stay fp32 (widening bf16 is exact), so the engine computes exactly what an fp32 engine
         # fed the widened gradient computes, and rounds the aggregate once (to nearest even) where it is final.  The
@@ -601,7 +604,14 @@ class BucketEngine:
         dev = self.device
         nT, nt = len(plan.tensors), plan.n_tiles
         with torch.cuda.device(dev):
-            self.grad = torch.zeros(plan.total_elems, dtype=grad_dtype, device=dev)
+            if grad is None:
+                self.grad = torch.zeros(plan.total_elems, dtype=grad_dtype, device=dev)
+            elif (grad.shape != (plan.total_elems,) or grad.dtype != grad_dtype or grad.device != dev
+                  or not grad.is_contiguous()):
+                raise ValueError(f"grad must be a flat {grad_dtype} buffer of {plan.total_elems} elements on {dev} (got "
+                                 f"{grad.dtype} {tuple(grad.shape)} on {grad.device})")
+            else:
+                self.grad = grad
             self.resid = torch.zeros(plan.total_elems, dtype=torch.float32, device=dev)
             self.mom = (torch.zeros(plan.total_elems, dtype=torch.float32, device=dev) if self.momentum is not None
                         else None)

@@ -22,6 +22,7 @@ bit and packs with cupy just before the collective, reference :446-455).
 from __future__ import annotations
 
 import math
+from dataclasses import dataclass
 from typing import Tuple
 
 import torch
@@ -159,6 +160,30 @@ def bloom_configuration(k: int, fpr: float) -> Tuple[int, int]:
 def topk_k(numel: int, ratio: float) -> int:
     """GRACE top-k K (SURVEY §2.5)."""
     return max(1, int(numel * ratio))
+
+
+@dataclass(frozen=True)
+class Warmup:
+    """DGC's sparsity warm-up (params keys ``'warmup_ratios'``, ``'warmup_steps'``): exchange ``e`` (0-based, counted
+    in exchanges, not micro-steps) is in stage ``min(e // steps, len(ratios))``; stage ``s < len(ratios)`` selects with
+    compress ratio ``ratios[s]``, the last stage with ``final`` (the dict's ``'compress_ratio'``).  Every route reads
+    the ratio of an exchange from here."""
+    ratios: Tuple[float, ...]
+    steps: int
+    final: float
+
+    @property
+    def n_stages(self) -> int:
+        return len(self.ratios) + 1
+
+    def stage(self, exchange: int) -> int:
+        return min(int(exchange) // self.steps, len(self.ratios))
+
+    def ratio(self, stage: int) -> float:
+        return self.ratios[stage] if stage < len(self.ratios) else self.final
+
+    def ratio_at(self, exchange: int) -> float:
+        return self.ratio(self.stage(exchange))
 
 
 def bits_for(n: int) -> int:
