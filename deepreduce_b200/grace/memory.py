@@ -19,7 +19,7 @@ import torch
 from .base import Memory
 
 
-def _dense(t: torch.Tensor) -> bool:
+def is_dense(t: torch.Tensor) -> bool:
     """True if t's strides describe a permutation of a contiguous layout (contiguous, channels_last, ...): the layouts
     in which DDP keeps a parameter's gradient with the parameter's strides."""
     expect = 1
@@ -150,12 +150,12 @@ class DgcMemory(Memory):
             if tuple(w.stride()) != layout:
                 raise ValueError(f"'dgc' weight decay: parameter {name!r} changed its layout from strides {layout} "
                                  f"to {tuple(w.stride())} after it was bound; its gradient keeps the old order")
-            if _dense(w):
+            if is_dense(w):
                 w = w.as_strided((w.numel(),), (1,))              # storage order
         return w.reshape(shape).to(dtype)
 
     def _clip(self, tensor):
-        flat = tensor.as_strided((tensor.numel(),), (1,)) if _dense(tensor) else tensor.reshape(-1)
+        flat = tensor.as_strided((tensor.numel(),), (1,)) if is_dense(tensor) else tensor.reshape(-1)
         f = clip_factor(pairwise_sumsq(flat), self.clip_thr)
         if f is None:
             return tensor

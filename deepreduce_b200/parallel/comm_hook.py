@@ -31,10 +31,13 @@ import torch
 import torch.distributed as dist
 import torch.nn as nn
 
-from ..grace.helper import sparsifier_of
-from .ddp import BUCKET_DTYPES, engine_split_numel, fused_path, make_engine, stage_plans
-from .engine import STATUS_NAMES, BucketEngine
+from .ddp import (BUCKET_DTYPES, engine_split_numel, fused_path, grace_state_dict, load_grace_state_dict, make_engine,
+                  make_grc, stage_plans)
+from .engine import BucketEngine, StatusPoller, total_stats
 from .plan import BucketPlan, split_large
+
+# the checkpoint key of each engine memory buffer (``BucketEngine.memory_buffers``), a map by parameter name
+MEMORY_KEYS = {"resid": "residuals", "mom": "momentum"}
 
 
 # ---------------------------------------------------------------------------
@@ -83,14 +86,17 @@ class _Layout:
         self.slot = {id(p): i for i, p in enumerate(params)}
         self.live = len(params)          # parameters whose residual still lives in this engine
 
-    def resid_of(self, p) -> torch.Tensor:
+    def memory_of(self, p) -> Dict[str, torch.Tensor]:
+        """The parameter's slice of each of the engine's memory buffers, by buffer name."""
         i = self.slot[id(p)]
-        return self.engine.resid[self.eng_off[i]:self.eng_off[i] + self.segments[i][1]]
+        lo, hi = self.eng_off[i], self.eng_off[i] + self.segments[i][1]
+        return {k: t[lo:hi] for k, t in self.engine.memory_buffers().items()}
+
+    def resid_of(self, p) -> torch.Tensor:
+        return self.memory_of(p)["resid"]
 
     def mom_of(self, p) -> torch.Tensor:
-        """The parameter's 'dgc' momentum in this engine (same place as its residual)."""
-        i = self.slot[id(p)]
-        return self.engine.mom[self.eng_off[i]:self.eng_off[i] + self.segments[i][1]]
+        return self.memory_of(p)["mom"]
 
 
 # ---------------------------------------------------------------------------
@@ -124,16 +130,15 @@ class DeepReduceHookState:
         self._layouts: List[_Layout] = []            # every engine not yet closed
         self._by_index: Dict[int, _Layout] = {}      # the layout a bucket index had last
         self._owner: Dict[int, _Layout] = {}         # id(parameter) -> the layout holding its residual
-        self._pending: Dict[str, torch.Tensor] = {}  # loaded residuals of parameters no engine holds yet
-        self._pending_mom: Dict[str, torch.Tensor] = {}  # ... and their loaded 'dgc' momenta
-        self.dgc = self.params.get('memory') == 'dgc'
+        # the loaded memory of parameters no engine holds yet, by buffer name ('dgc' engines add the momentum)
+        buffers = ("resid", "mom") if self.params.get('memory') == 'dgc' else ("resid",)
+        self._pending: Dict[str, Dict[str, torch.Tensor]] = {k: {} for k in buffers}
         self._pending_epoch = 0
         self._plans: Dict[tuple, list] = {}          # warm-up: every stage's plan of a layout, built when first met
         self._stream: Optional[torch.cuda.Stream] = None
         self.grc = None
         self.step_count = 0
-        self._status_host = None
-        self._status_event = None
+        self._status = StatusPoller()
 
     # ---- routing ------------------------------------------------------------------
     def path(self, buffer: torch.Tensor) -> str:
@@ -173,12 +178,9 @@ class DeepReduceHookState:
         return work.get_future().then(lambda f: f.value()[0])
 
     def _make_grc(self):
-        from ..wrappers import deepreduce_from_params
-        self.grc = deepreduce_from_params(self.params)
-        if hasattr(self.grc.memory, "bind_parameters"):           # 'dgc' weight decay reads the parameters
-            # bucket.gradients() are plain reshapes of the flat bucket, which holds every gradient in its
-            # parameter's storage order: the memory reads the parameters in that order too
-            self.grc.memory.bind_parameters(self.module.named_parameters(), storage_order=True)
+        # bucket.gradients() are plain reshapes of the flat bucket, which holds every gradient in its parameter's
+        # storage order: a memory that reads the parameters reads them in that order too
+        self.grc = make_grc(self.params, self.module.named_parameters(), storage_order=True)
 
     def _grace(self, bucket, buf):
         if self.grc is None:
@@ -262,15 +264,14 @@ class DeepReduceHookState:
         table = segment_table(segments, plan, owner)
         repack = ops.cuda_module().Repack(table, buf.numel(), plan.total_elems, eng.grad)
         lay = _Layout(key, index, list(params), names, list(segments), plan, eng, table, repack)
-        # carry every parameter's residual, by parameter identity and in storage order, from the engine that held it;
+        # carry every parameter's memory, by parameter identity and in storage order, from the engine that held it;
         # an engine closes once none of its parameters is left in it
         for p, n in zip(params, names):
-            dst = lay.resid_of(p)
+            dst = lay.memory_of(p)
             old = self._owner.get(id(p))
             if old is not None:
-                dst.copy_(old.resid_of(p))
-                if self.dgc:
-                    lay.mom_of(p).copy_(old.mom_of(p))
+                for k, t in old.memory_of(p).items():
+                    dst[k].copy_(t)
                 if self.warmup is not None:
                     # a warm-up run's engines only move their epochs forward, across stage switches and DDP's rebuild
                     # alike; without the keys a new layout keeps its own count, as it always has (its arena is new
@@ -280,10 +281,9 @@ class DeepReduceHookState:
                 if old.live == 0:
                     self._close_layout(old)
             else:
-                if n in self._pending:
-                    dst.copy_(self._pending.pop(n).to(dst.device, torch.float32).reshape(-1))
-                if self.dgc and n in self._pending_mom:
-                    lay.mom_of(p).copy_(self._pending_mom.pop(n).to(dst.device, torch.float32).reshape(-1))
+                for k, pending in self._pending.items():
+                    if n in pending:
+                        dst[k].copy_(pending.pop(n).to(eng.device, torch.float32).reshape(-1))
             self._owner[id(p)] = lay
         eng.epoch = max(eng.epoch, self._pending_epoch)
         self._by_index[index] = lay
@@ -314,21 +314,9 @@ class DeepReduceHookState:
     def check_async(self):
         """Per-step failure detection without a host sync (as ``DeepReduceDDP.check_async``): copy the status words to
         pinned memory on the current stream, and inspect the copy the previous call enqueued once it has landed."""
-        if self._status_host is not None and self._status_event.query():
-            st, idx = self._status_host
-            for b in range(len(idx)):
-                if int(st[b, 0]) != 0:
-                    raise RuntimeError(f"[rank {self.rank}/{self.world}] DDP bucket {idx[b]} (step {self.step_count}): "
-                                       f"deepreduce engine error: {STATUS_NAMES.get(int(st[b, 0]), int(st[b, 0]))} "
-                                       f"(aux={int(st[b, 1])})")
-        if not self._layouts:
-            return
-        st = torch.zeros(len(self._layouts), 8, dtype=torch.int32).pin_memory()
-        for b, lay in enumerate(self._layouts):
-            st[b].copy_(lay.engine.status, non_blocking=True)
-        self._status_host = (st, [lay.index for lay in self._layouts])
-        self._status_event = torch.cuda.Event()
-        self._status_event.record()
+        bad = self._status.poll([(lay.index, lay.engine) for lay in self._layouts])
+        if bad is not None:
+            raise RuntimeError(f"[rank {self.rank}/{self.world}] DDP bucket {bad[0]} (step {self.step_count}): {bad[1]}")
 
     # ---- accounting ---------------------------------------------------------------
     def dense_bytes(self) -> int:
@@ -347,37 +335,28 @@ class DeepReduceHookState:
         """Device-side counters of the last exchanged step, summed over the live engines (fused path); synchronises."""
         if not self._layouts:
             return {"wire_bytes": self.wire_bytes_per_step(), "dense_bytes": self.dense_bytes()}
-        torch.cuda.synchronize(self._layouts[0].engine.device)
-        tot: dict = {}
-        for e in self.engines:
-            for k, v in e.stats()["total"].items():
-                tot[k] = tot.get(k, 0) + v
-        tot["relative_volume"] = tot["wire_bytes"] / max(1, tot["dense_bytes"])
-        return tot
+        return total_stats(self.engines)
 
     # ---- checkpoint / resume ----------------------------------------------------------
+    def _held_memory(self) -> Dict[str, Dict[str, torch.Tensor]]:
+        """By parameter name, ``_Layout.memory_of`` of every parameter in the engine that holds it."""
+        return {n: lay.memory_of(p) for lay in self._layouts for p, n in zip(lay.params, lay.names)
+                if self._owner.get(id(p)) is lay}
+
     def state_dict(self) -> dict:
         """Keyed by parameter name, so that a checkpoint loads into a run with other buckets: the residual of every
         parameter (fused path, flat in storage order; with 'dgc' its momentum too, under ``"momentum"``) or the GRACE
         memory (per-tensor path)."""
         if self._layouts:
             torch.cuda.synchronize(self._layouts[0].engine.device)
-        resid = {n: t.clone() for n, t in self._pending.items()}
-        mom = {n: t.clone() for n, t in self._pending_mom.items()}
-        for lay in self._layouts:
-            for p, n in zip(lay.params, lay.names):
-                if self._owner.get(id(p)) is lay:
-                    resid[n] = lay.resid_of(p).detach().cpu().clone()
-                    if self.dgc:
-                        mom[n] = lay.mom_of(p).detach().cpu().clone()
-        out = {"step": self.step_count, "residuals": resid,
-               "epoch": max([self._pending_epoch] + [e.epoch for e in self.engines])}
-        if self.dgc:
-            out["momentum"] = mom
+        memory = {k: {n: t.clone() for n, t in pending.items()} for k, pending in self._pending.items()}
+        for n, held in self._held_memory().items():
+            for k, t in held.items():
+                memory[k][n] = t.detach().cpu().clone()
+        out = {"step": self.step_count, "epoch": max([self._pending_epoch] + [e.epoch for e in self.engines])}
+        out.update((MEMORY_KEYS[k], m) for k, m in memory.items())
         if self.grc is not None:
-            out["memory"] = self.grc.memory.state_dict()
-            if self.warmup is not None:               # the per-name exchange counts of the warm-up
-                out["sparsifier"] = sparsifier_of(self.grc).state_dict()
+            out.update(grace_state_dict(self.grc, self.warmup))
         return out
 
     def load_state_dict(self, state: dict):
@@ -386,30 +365,20 @@ class DeepReduceHookState:
         self._pending_epoch = max(self._pending_epoch, int(state.get("epoch", 0)))
         for e in self.engines:
             e.epoch = max(e.epoch, self._pending_epoch)
-        by_name = {}
-        for lay in self._layouts:
-            for p, n in zip(lay.params, lay.names):
-                if self._owner.get(id(p)) is lay:
-                    by_name[n] = lay
-        if self.dgc != ("momentum" in state) and state.get("residuals"):
+        held = self._held_memory()
+        if ("mom" in self._pending) != ("momentum" in state) and state.get("residuals"):
             raise ValueError("hook state of another memory: 'dgc' states carry a 'momentum' map, other states do not")
-        self._pending, self._pending_mom = {}, {}
-        for key, pending, view in (("residuals", self._pending, _Layout.resid_of),
-                                   ("momentum", self._pending_mom, _Layout.mom_of)):
-            for n, t in state.get(key, {}).items():
-                lay = by_name.get(n)
-                if lay is None:
-                    pending[n] = t.detach().cpu().clone()
+        self._pending = {k: {} for k in self._pending}
+        for k, pending in self._pending.items():
+            for n, t in state.get(MEMORY_KEYS[k], {}).items():
+                if n in held:
+                    held[n][k].copy_(t.to(held[n][k].device, torch.float32).reshape(-1))
                 else:
-                    p = next(q for q, m in zip(lay.params, lay.names) if m == n)
-                    view(lay, p).copy_(t.to(lay.engine.device, torch.float32).reshape(-1))
+                    pending[n] = t.detach().cpu().clone()
         if "memory" in state:
             if self.grc is None:
                 self._make_grc()
-            dev = next(self.module.parameters()).device
-            self.grc.memory.load_state_dict(state["memory"], device=dev)
-            if self.warmup is not None:               # a checkpoint from before the warm-up: every count at 0
-                sparsifier_of(self.grc).load_state_dict(state.get("sparsifier", {}))
+            load_grace_state_dict(self.grc, state, self.warmup, next(self.module.parameters()).device)
 
     def close(self):
         """Release the engines and their arenas (collective at W > 1)."""

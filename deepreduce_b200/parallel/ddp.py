@@ -26,22 +26,10 @@ import torch.nn as nn
 
 from .. import spec
 from ..grace.helper import sparsifier_of
+from ..grace.memory import is_dense
 from ..wrappers import deepreduce_from_params
-from .engine import BucketEngine
+from .engine import BucketEngine, StatusPoller, total_stats
 from .plan import BucketPlan
-
-
-def _is_dense(p: torch.Tensor) -> bool:
-    """True if p's strides describe a permutation-dense layout (contiguous / channels_last / ...)."""
-    sizes, strides = list(p.size()), list(p.stride())
-    expect = 1
-    for st, sz in sorted(zip(strides, sizes)):
-        if sz == 1:
-            continue
-        if st != expect:
-            return False
-        expect *= sz
-    return True
 
 
 def _fused_supported(params: dict) -> bool:
@@ -216,9 +204,9 @@ def switch_engine(old: BucketEngine, build) -> BucketEngine:
     agg = old.grad.clone()
     new = build(old.grad)
     new.grad.copy_(agg)
-    new.resid.copy_(old.resid)
-    if new.mom is not None:
-        new.mom.copy_(old.mom)
+    buffers = new.memory_buffers()
+    for k, t in old.memory_buffers().items():
+        buffers[k].copy_(t)
     new.epoch = max(new.epoch, old.epoch)
     old.close()
     return new
@@ -247,10 +235,33 @@ def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: b
             warnings.warn(f"deepreduce_b200: partition calibration skipped ({e!r}); using the static cut")
             eng.cta_speeds = None
             eng._set_cuts()
-            eng.resid.zero_(); eng.sel.zero_(); eng.grad.zero_()
-            if eng.mom is not None:
-                eng.mom.zero_()
+            eng.reset_state()
     return eng
+
+
+def make_grc(params: dict, named_parameters, storage_order: bool = False):
+    """The GRACE communicator of the per-tensor path for ``params``; a memory that reads the parameters ('dgc' weight
+    decay) is bound to the ``(name, parameter)`` pairs (``storage_order``: see ``DgcMemory.bind_parameters``)."""
+    grc = deepreduce_from_params(params)
+    if hasattr(grc.memory, "bind_parameters"):
+        grc.memory.bind_parameters(named_parameters, storage_order=storage_order)
+    return grc
+
+
+def grace_state_dict(grc, warmup) -> dict:
+    """The per-tensor path's checkpoint: the GRACE ``memory``, plus the warm-up's per-name ``sparsifier`` counts."""
+    out = {"memory": grc.memory.state_dict()}
+    if warmup is not None:
+        out["sparsifier"] = sparsifier_of(grc).state_dict()
+    return out
+
+
+def load_grace_state_dict(grc, state: dict, warmup, device):
+    """Restore what ``grace_state_dict`` saved.  A checkpoint from before the warm-up restores every count to 0."""
+    if "memory" in state:
+        grc.memory.load_state_dict(state["memory"], device=device)
+    if warmup is not None:
+        sparsifier_of(grc).load_state_dict(state.get("sparsifier", {}))
 
 
 class DeepReduceDDP:
@@ -278,8 +289,7 @@ class DeepReduceDDP:
         self._handles = []
         self._exchange = True
         self._grad_views: Dict[int, torch.Tensor] = {}
-        self._status_host = None          # pinned copies of the engines' status words (async check)
-        self._status_event = None
+        self._status = StatusPoller()
         self.overlap_grid_cap = int(overlap_grid if overlap_grid is not None else (self.params.get('overlap_grid', 0) or 0))
         from ..config import warmup_from_params
         self.warmup = warmup_from_params(self.params)        # sparsity warm-up: stages counted in exchanges (finish())
@@ -298,9 +308,7 @@ class DeepReduceDDP:
             if self.overlap:
                 self._install_hooks()
         else:
-            self.grc = deepreduce_from_params(self.params)
-            if hasattr(self.grc.memory, "bind_parameters"):       # 'dgc' weight decay reads the parameters
-                self.grc.memory.bind_parameters(self.named)
+            self.grc = make_grc(self.params, self.named)
 
     # ---- bucket construction ------------------------------------------------
     def _build_buckets(self, cap_mb, blocks_per_sm, use_history):
@@ -340,7 +348,7 @@ class DeepReduceDDP:
                 seg = flat[t.elem_off:t.elem_off + p.numel()]        # chunks are tile multiples: contiguous
                 # the gradient view mirrors the parameter's own (dense) layout — e.g. channels_last conv
                 # weights — so fused optimizers see identical strides; the bucket is in storage order
-                p.grad = seg.as_strided(p.size(), p.stride()) if _is_dense(p) else seg.view(p.shape)
+                p.grad = seg.as_strided(p.size(), p.stride()) if is_dense(p) else seg.view(p.shape)
                 self._grad_views[id(p)] = p.grad
                 self.bucket_of[id(p)] = b
         self._in_backward = False
@@ -468,24 +476,11 @@ class DeepReduceDDP:
             p.grad = v
 
     def check_async(self):
-        """Per-step failure detection without a host sync: enqueue a copy of every engine's status word to pinned host
-        memory, and inspect the copy enqueued by the PREVIOUS call once its event has completed (it has, a step
-        later).  Raises like :meth:`check` one step after a watchdog fired."""
-        if not self.engines:
-            return
-        if self._status_host is not None and self._status_event.query():
-            st = self._status_host
-            for b in range(len(self.engines)):
-                if int(st[b, 0]) != 0:
-                    from .engine import STATUS_NAMES
-                    raise RuntimeError(f"[rank {self.rank}/{self.world}] bucket {b} (step {self.step_count}): deepreduce "
-                                       f"engine error: {STATUS_NAMES.get(int(st[b, 0]), int(st[b, 0]))} (aux={int(st[b, 1])})")
-        if self._status_host is None:
-            self._status_host = torch.zeros(len(self.engines), 8, dtype=torch.int32).pin_memory()
-            self._status_event = torch.cuda.Event()
-        for b, e in enumerate(self.engines):
-            self._status_host[b].copy_(e.status, non_blocking=True)
-        self._status_event.record()
+        """Per-step failure detection without a host sync (``StatusPoller``): raises like :meth:`check` one step after
+        a watchdog fired."""
+        bad = self._status.poll(list(enumerate(self.engines)))
+        if bad is not None:
+            raise RuntimeError(f"[rank {self.rank}/{self.world}] bucket {bad[0]} (step {self.step_count}): {bad[1]}")
 
     def check(self):
         """Read the engines' device status words (one small D2H each); raises with rank and bucket on a watchdog."""
@@ -522,23 +517,14 @@ class DeepReduceDDP:
         Call it after ``finish()`` (i.e. after a training step); it synchronises the device, so every N steps."""
         if not self.fused:
             return {"wire_bytes": self.wire_bytes_per_step(), "dense_bytes": self.dense_bytes()}
-        torch.cuda.synchronize(self.device)
-        tot: dict = {}
-        for e in self.engines:
-            for k, v in e.stats()["total"].items():
-                tot[k] = tot.get(k, 0) + v
-        tot["relative_volume"] = tot["wire_bytes"] / max(1, tot["dense_bytes"])
-        return tot
+        return total_stats(self.engines)
 
     # ---- checkpoint / resume (SURVEY §5) -------------------------------------------
     def state_dict(self):
         if self.fused:
             return {"step": self.step_count, "engines": [e.state_dict() for e in self.engines]}
         if self.grc is not None:
-            out = {"step": self.step_count, "memory": self.grc.memory.state_dict()}
-            if self.warmup is not None:               # the per-name exchange counts of the warm-up
-                out["sparsifier"] = sparsifier_of(self.grc).state_dict()
-            return out
+            return {"step": self.step_count, **grace_state_dict(self.grc, self.warmup)}
         return {"step": self.step_count}
 
     def load_state_dict(self, state):
@@ -549,10 +535,7 @@ class DeepReduceDDP:
             for e, s in zip(self.engines, state["engines"]):
                 e.load_state_dict(s)
         elif self.grc is not None:
-            if "memory" in state:
-                self.grc.memory.load_state_dict(state["memory"], device=self.device)
-            if self.warmup is not None:               # a checkpoint from before the warm-up: every count at 0
-                sparsifier_of(self.grc).load_state_dict(state.get("sparsifier", {}))
+            load_grace_state_dict(self.grc, state, self.warmup, self.device)
 
     def close(self):
         for h in self._handles:

@@ -36,7 +36,7 @@ from ..codecs.bf16 import bf16_bits_oracle, bf16_widen_oracle
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
 from ..codecs.polyfit import get_segments, polyfit_eval_oracle, polyfit_fit_oracle
 from ..codecs.qsgd import qsgd_decode_oracle, qsgd_encode_oracle
-from ..grace.memory import clip_factor, pairwise_sumsq
+from ..grace.memory import clip_factor, is_dense, pairwise_sumsq
 from .plan import update_cta_speeds
 from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID, SLOT_HEADER_WORDS,
                    VMODE_BF16, VMODE_DEXP, VMODE_QSGD, BucketPlan, rle_stream_words)
@@ -48,6 +48,37 @@ MAGIC = 0xD33B2000
 STATUS_NAMES = {0: "ok", 1: "(unused)", 2: "peer flag watchdog", 3: "select resolve failed", 4: "grid barrier watchdog", 5: "TMA mbarrier watchdog",
                 6: "stage-2 slot overflow (sharded decode)",
                 7: "ranks disagree on the 'randomk' draw (a sender's header differs from the receiver's)"}
+
+
+def status_error(row) -> str:
+    """The error text of an engine status word ``[code, aux, ...]`` with a non-zero code."""
+    return f"deepreduce engine error: {STATUS_NAMES.get(int(row[0]), int(row[0]))} (aux={int(row[1])})"
+
+
+class StatusPoller:
+    """Failure detection without a host sync: each ``poll`` copies the engines' status words to pinned host memory on
+    the current stream, and reads the copy the previous call enqueued once its event has completed (a step later)."""
+
+    def __init__(self):
+        self._host, self._event, self._labels = None, None, []
+
+    def poll(self, engines) -> Optional[tuple]:
+        """``engines``: ``(label, BucketEngine)`` pairs.  Returns ``(label, status_error text)`` of the first failed
+        engine in the previous call's copy, and then enqueues nothing; else enqueues the copy and returns None."""
+        if self._event is not None and self._event.query():
+            for label, row in zip(self._labels, self._host.tolist()):
+                if row[0] != 0:
+                    return label, status_error(row)
+        if not engines:
+            return None
+        if self._host is None or len(self._host) != len(engines):
+            self._host = torch.zeros(len(engines), 8, dtype=torch.int32).pin_memory()
+            self._event = torch.cuda.Event()
+        for b, (_, e) in enumerate(engines):
+            self._host[b].copy_(e.status, non_blocking=True)
+        self._labels = [label for label, _ in engines]
+        self._event.record()
+        return None
 
 
 # ---------------------------------------------------------------------------
@@ -535,6 +566,17 @@ def stats_from_slot(plan: BucketPlan, slot) -> dict:
     return {"tensors": per, "total": tot}
 
 
+def total_stats(engines) -> dict:
+    """``stats()["total"]`` of the last exchanged step summed over ``engines``, with its relative volume; synchronises."""
+    torch.cuda.synchronize(engines[0].device)
+    tot: dict = {}
+    for e in engines:
+        for k, v in e.stats()["total"].items():
+            tot[k] = tot.get(k, 0) + v
+    tot["relative_volume"] = tot["wire_bytes"] / max(1, tot["dense_bytes"])
+    return tot
+
+
 class BucketEngine:
     """One flat bucket + its fused exchange kernel."""
 
@@ -767,10 +809,17 @@ class BucketEngine:
                 self._set_cuts()
         finally:
             self.ctx.set_debug_times(0)
-        self.resid.zero_(); self.sel.zero_(); self.grad.zero_()
-        if self.mom is not None:
-            self.mom.zero_()
+        self.reset_state()
         return log
+
+    def memory_buffers(self) -> dict:
+        """The engine's per-element memory by name: the residual ``resid``, and with a momentum ('dgc') ``mom``."""
+        return {"resid": self.resid} if self.mom is None else {"resid": self.resid, "mom": self.mom}
+
+    def reset_state(self):
+        """Zero the memory buffers, the select history and the gradient buffer."""
+        for t in (*self.memory_buffers().values(), self.sel, self.grad):
+            t.zero_()
 
     # ---- arena -------------------------------------------------------------
     def _setup_arena(self):
@@ -875,7 +924,6 @@ class BucketEngine:
         engine's device, of the bucket's dtype, and dense, so that its storage order is the order of its gradient in
         the bucket.  The table is uploaded on the current stream; call it again (or ``refresh_parameters``) when a
         parameter's storage moves."""
-        from .ddp import _is_dense
         params = list(parameters)
         owner = list(range(len(params))) if owner is None else [int(o) for o in owner]
         tensors = self.plan.tensors
@@ -890,7 +938,7 @@ class BucketEngine:
             if p.device != self.device or p.dtype != self.grad_dtype:
                 raise ValueError(f"bind_parameters: parameter {i} ({t.name}) is {p.dtype} on {p.device}; the engine's "
                                  f"bucket is {self.grad_dtype} on {self.device}")
-            if not _is_dense(p):
+            if not is_dense(p):
                 raise ValueError(f"bind_parameters: parameter {i} ({t.name}) is not dense in memory: its storage order "
                                  f"is not the order of its gradient in the bucket")
             ptrs.append(p.data_ptr() + done[i] * p.element_size())
@@ -992,26 +1040,24 @@ class BucketEngine:
     def check_status(self):
         st = self.status.cpu().tolist()
         if st[0] != 0:
-            raise RuntimeError(f"deepreduce engine error: {STATUS_NAMES.get(st[0], st[0])} (aux={st[1]})")
+            raise RuntimeError(status_error(st))
 
     def grid(self) -> int:
         return int(self.ctx.grid())
 
     # ---- state (checkpoint / resume; SURVEY §5) ----------------------------
     def state_dict(self):
-        out = {"resid": self.resid.detach().cpu().clone(), "epoch": self.epoch,
-               "sel": self.sel.detach().cpu().clone()}
-        if self.mom is not None:
-            out["mom"] = self.mom.detach().cpu().clone()
+        out = {k: t.detach().cpu().clone() for k, t in self.memory_buffers().items()}
+        out.update(epoch=self.epoch, sel=self.sel.detach().cpu().clone())
         return out
 
     def load_state_dict(self, state):
-        if ("mom" in state) != (self.mom is not None):
+        buffers = self.memory_buffers()
+        if ("mom" in state) != ("mom" in buffers):
             raise ValueError("engine state of another memory: a 'dgc' engine loads only 'dgc' states (with 'mom'), "
                              "any other engine only states without it")
-        self.resid.copy_(state["resid"].to(self.device))
-        if self.mom is not None:
-            self.mom.copy_(state["mom"].to(self.device))
+        for k, t in buffers.items():
+            t.copy_(state[k].to(self.device))
         self.sel.copy_(state["sel"].to(self.device))
         # never move the step counter backwards inside a live process group: the peers' flags in the arena carry
         # epochs this engine has already used (e.g. during calibrate_partition)

@@ -7,6 +7,7 @@ hook's own plan for that layout and the residual the test carries itself: ``ref_
 configuration compares within the fp32-vs-fp64 tolerances of ``test_gpu_engine``.  When DDP rebuilds its buckets,
 the residual each parameter finds in its new engine must be the one it left in the old."""
 import os
+import re
 import subprocess
 import sys
 import tempfile
@@ -345,6 +346,47 @@ def test_ddp_hook_state_dict_into_other_bucket_cap(nccl_world1):
     finally:
         sa.close()
         sb.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.timeout(600)
+def test_status_checks_name_front_end_and_status(nccl_world1):
+    """``check()`` and ``check_async()`` of ``DeepReduceDDP`` and of the hook turn a non-zero engine status word into
+    an error with the front end's rank / bucket label and the status name: ``check()`` at once, ``check_async()`` on
+    the call after the one that enqueued the copy.  The word is written from the host between steps."""
+    from deepreduce_b200.parallel import DeepReduceDDP, register_deepreduce_hook
+    cfg = dict(CONFIGS["topk"], calibrate_partition=False)
+
+    def linear():
+        torch.manual_seed(0)
+        return nn.Linear(64, 64).cuda()
+
+    ours = DeepReduceDDP(linear(), cfg)
+    model = linear()
+    ddp = DDP(model, device_ids=[0])
+    hook = register_deepreduce_hook(ddp, cfg)
+    ddp(torch.randn(8, 64, device="cuda")).pow(2).mean().backward()
+    torch.cuda.synchronize()
+    fronts = ((ours, "[rank 0/1] bucket 0"), (hook, "[rank 0/1] DDP bucket 0"))
+    try:
+        for st, label in fronts:
+            assert len(st.engines) == 1
+            st.check()
+            st.check_async()
+            torch.cuda.synchronize()
+            st.engines[0].status.copy_(torch.tensor([2, 7, 0, 0, 0, 0, 0, 0], dtype=torch.int32))
+            err = "deepreduce engine error: peer flag watchdog (aux=7)"
+            with pytest.raises(RuntimeError, match=re.escape(f"{label} (2 tensors, step {st.step_count}): {err}")):
+                st.check()
+            st.check_async()                 # reads the clean copy, enqueues the failed word
+            torch.cuda.synchronize()
+            with pytest.raises(RuntimeError, match=re.escape(f"{label} (step {st.step_count}): {err}")):
+                st.check_async()
+    finally:
+        for e in ours.engines + hook.engines:
+            e.status.copy_(torch.zeros(8, dtype=torch.int32))
+        hook.close()
+        ours.close()
 
 
 @pytest.mark.gpu
