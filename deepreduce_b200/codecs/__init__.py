@@ -5,6 +5,7 @@ from .bf16 import BF16
 from .bloom import Bloom, Bloomfilter, get_BFconfig
 from .bloom_cpu import BloomCPU, bloom_compress_blob, bloom_decompress_blob
 from .dexp import DoubleExp
+from .elias_fano import EliasFano
 from .integer import IntegerIndex
 from .lossless import Gzip, Huffman
 from .polyfit import PolyFit, PolyFitCPU, get_segments
@@ -12,5 +13,5 @@ from .qsgd import QSGD
 from .rle import RunLength
 
 __all__ = ["SparseCompressor", "compressor", "register", "bitpack", "BF16", "Bloom", "Bloomfilter", "get_BFconfig",
-           "BloomCPU", "bloom_compress_blob", "bloom_decompress_blob", "DoubleExp", "IntegerIndex", "Gzip",
+           "BloomCPU", "bloom_compress_blob", "bloom_decompress_blob", "DoubleExp", "EliasFano", "IntegerIndex", "Gzip",
            "Huffman", "PolyFit", "PolyFitCPU", "get_segments", "QSGD", "RunLength"]

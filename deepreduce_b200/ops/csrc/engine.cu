@@ -870,6 +870,30 @@ DR_D uint32_t rle_get(const uint32_t* stream, uint32_t j) {
 }
 
 // ===========================================================================
+// kModeEf helpers (spec.py ef_layout): entry p with in-tile offset e in tile-local tile t puts e & (2^L - 1) at bit p*L
+// of the low stream (off_idx) and sets bit p + t * (kTile >> L) + (e >> L) of the high stream (off_hi), LSB-first
+// ===========================================================================
+DR_D void ef_put(uint32_t* slot, const TensorDesc* td, uint32_t p, uint32_t t, uint32_t e) {
+  const uint32_t L = __ldg(&td->ef_low_bits);
+  if (L) {
+    uint32_t* lo = slot + __ldg(&td->off_idx);
+    const uint32_t f = e & ((1u << L) - 1u), bit = p * L, w = bit >> 5, sh = bit & 31u;
+    atomicOr(lo + w, f << sh);
+    if (sh + L > 32u) atomicOr(lo + w + 1, f >> (32u - sh));
+  }
+  const uint32_t hb = p + t * (kTile >> L) + (e >> L);
+  atomicOr(slot + __ldg(&td->off_hi) + (hb >> 5), 1u << (hb & 31u));
+}
+
+DR_D uint32_t ef_low(const uint32_t* lo, uint32_t p, uint32_t L) {
+  if (!L) return 0u;
+  const uint32_t bit = p * L, w = bit >> 5, sh = bit & 31u;
+  uint32_t v = __ldcg(lo + w) >> sh;
+  if (sh + L > 32u) v |= __ldcg(lo + w + 1) << (32u - sh);
+  return v & ((1u << L) - 1u);
+}
+
+// ===========================================================================
 // Walk of a warp's candidate chunks (one per tile) with the heads of the next kPF chunks in flight: cp.async copies
 // the first 32 entries (256 B) and the count of chunk tile+kPF into a warp-private SMEM ring while chunk `tile` is
 // processed.  The lists were written a phase ago and sit in DRAM; every chunk head is a separate 256-byte request,
@@ -1405,6 +1429,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
                 if (P.world == 1) put_out<kB>(P, gi, dec * P.scale);
                 if (mode == (uint32_t)kModeRaw) idxs[rp] = ti.local0 + e;
                 else if (mode == (uint32_t)kModeRle) rle_put(idxs, rp, e);
+                else if (mode == (uint32_t)kModeEf) ef_put(my_slot, P.tensors + cur, rp, tile_local, e);
                 if (rp == limit - 1u) dyn->cutoff = ti.local0 + e;
                 return;
               }
@@ -1416,6 +1441,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
             if (scatter) put_out<kB>(P, gi, v * P.scale);
             if (mode == (uint32_t)kModeRaw) idxs[rp] = ti.local0 + e;
             else if (kFull && mode == (uint32_t)kModeRle) rle_put(idxs, rp, e);
+            else if (kFull && mode == (uint32_t)kModeEf) ef_put(my_slot, P.tensors + cur, rp, tile_local, e);
             if (kFull && vmode != kVmodeFp32) my_slot[off_selidx + rp] = (uint32_t)gi;
             if (rp == limit - 1u) dyn->cutoff = ti.local0 + e;
           };
@@ -1427,7 +1453,7 @@ DR_D void phase_emit(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
       if (lane == 0) {
         // bloom: shipped prefix table; shared: sender-local scratch that the decode reads back from the own slot
         if (mode == (uint32_t)kModeBloom || (kFull && mode == (uint32_t)kModeShared)) my_slot[off_prefix + tile_local] = min(excl, limit);
-        else if (kFull && mode == (uint32_t)kModeRle)
+        else if (kFull && (mode == (uint32_t)kModeRle || mode == (uint32_t)kModeEf))
           reinterpret_cast<uint16_t*>(my_slot + off_prefix)[tile_local] =
               (uint16_t)(excl >= limit ? 0u : min(total, limit - excl));
         if (tile_local + 1u == n_tiles) {
@@ -2112,7 +2138,7 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
         }
         for (uint32_t e = tid; e < ti.n; e += kThreads) put_out<kB>(P, ti.base + e, sm.u.acc[e]);
       }
-    } else if (kFull && sm.td.mode == (uint32_t)kModeRle) {
+    } else if (kFull && (sm.td.mode == (uint32_t)kModeRle || sm.td.mode == (uint32_t)kModeEf)) {
       // running entry prefix of every sender at my first tile of this tensor = sum of the earlier tiles' counts
       __syncthreads();
       if (tid < 16) sm.s.rle_pre[tid] = 0u;
@@ -2137,10 +2163,44 @@ DR_D void phase_compact(const EngineParams& P, Smem& sm, uint32_t& bar_epoch) {
           const uint32_t pre = sm.s.rle_pre[r];
           const float* vals = reinterpret_cast<const float*>(slot + sm.td.off_vals);
           const float* fitted = P.expand_buf + (size_t)r * P.poly_total + sm.td.poly_off;   // 'both': rank r's curve
-          for (uint32_t j = tid; j < c; j += kThreads) {
-            const uint32_t rp = pre + j;
-            if (rp < sm.td.val_cap)                         // distinct positions per sender
-              sm.u.acc[rle_get(slot + sm.td.off_idx, rp)] += coded_value<kFull>(slot, sm.td, vals, fitted, rp) * P.scale;
+          if (sm.td.mode == (uint32_t)kModeRle) {
+            for (uint32_t j = tid; j < c; j += kThreads) {
+              const uint32_t rp = pre + j;
+              if (rp < sm.td.val_cap)                       // distinct positions per sender
+                sm.u.acc[rle_get(slot + sm.td.off_idx, rp)] += coded_value<kFull>(slot, sm.td, vals, fitted, rp) * P.scale;
+            }
+          } else if (c) {
+            // Elias-Fano: the tile's high-stream range [pre + t*B, pre + t*B + c + B) (at most 256 words), funnel-shifted
+            // to its start, one word per thread; the popcount scan gives every set bit its rank j and the thread lists
+            // its high part q - j at j (SMEM), then every thread takes one entry, as the run-length loop does: offset
+            // (q - j) << L | its low field.  Bits past the range (the next tile's) are masked off.
+            const uint32_t L = sm.td.ef_low_bits, B = kTile >> L;
+            const uint32_t s = pre + (tile - sm.td.tile_begin) * B, len = c + B, nw = (len + 31u) >> 5;
+            const uint32_t* hi = slot + sm.td.off_hi;
+            const uint32_t hi_words = (sm.td.val_cap + sm.td.n_tiles * B + 31u) >> 5;
+            uint32_t x = 0u;
+            if (tid < nw) {
+              const uint32_t w = (s >> 5) + tid;
+              const uint32_t a = w < hi_words ? __ldcg(hi + w) : 0u, b = w + 1u < hi_words ? __ldcg(hi + w + 1u) : 0u;
+              x = __funnelshift_r(a, b, s & 31u);
+              if (len - 32u * tid < 32u) x &= (1u << (len - 32u * tid)) - 1u;
+            }
+            const uint32_t n = (uint32_t)__popc(x), incl = warp_incl_scan(n, lane);
+            if (lane == 31u) sm.s.warp_tot[warp] = incl;
+            __syncthreads();
+            uint16_t* list = reinterpret_cast<uint16_t*>(g_filter_smem);   // high part of the j-th entry
+            uint32_t j = incl - n;
+            for (uint32_t w = 0; w < warp; ++w) j += sm.s.warp_tot[w];
+            for (; x; x &= x - 1u, ++j) {
+              const uint32_t h = 32u * tid + (uint32_t)(__ffs((int)x) - 1) - j;
+              if (j < c) list[j] = (uint16_t)min(h, B);     // B: not in this tile's range (a malformed stream)
+            }
+            __syncthreads();
+            for (uint32_t q = tid; q < c; q += kThreads) {
+              const uint32_t h = list[q], rp = pre + q;
+              if (h < B && rp < sm.td.val_cap)              // distinct positions per sender
+                sm.u.acc[(h << L) | ef_low(slot + sm.td.off_idx, rp, L)] += coded_value<kFull>(slot, sm.td, vals, fitted, rp) * P.scale;
+            }
           }
           __syncthreads();                                  // senders are added in rank order: deterministic sums
           if (tid == 0) sm.s.rle_pre[r] = pre + c;
@@ -2473,7 +2533,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) dr_engine_kernel(const _
 static bool g_attr_set = false;
 
 // ... x two feature sets: <.., false, ..> index-only (plain pairs / bloom), <.., true, ..> + value codecs (bf16 values
-// included), run-length index and the shared 'randomk' index; ... x the gradient type: <.., .., false> fp32 buckets,
+// included), run-length and Elias-Fano indices (has_rle) and the shared 'randomk' index; ... x the gradient type: <.., .., false> fp32 buckets,
 // <.., .., true> bf16 buckets (a separate instantiation, so the fp32 kernels are compiled from exactly the code they had
 // before bf16 existed)
 static const void* kernel_for(int blocks_per_sm, bool full, bool bf16) {

@@ -27,6 +27,8 @@ enum TensorMode : uint32_t {
                     // zero-run offset of every selected element inside its tile, 12 bits each, LSB-first (off_idx)
   kModeShared = 3,  // 'randomk': the index set is a seeded draw every rank computes itself (selection rule below), so
                     // only the values travel; off_prefix is sender-local scratch (per-tile exclusive prefix)
+  kModeEf = 4,      // lossless tile-local Elias-Fano (spec.py ef_layout): kModeRle's u16 count per tile (off_prefix), the
+                    // L low bits of every entry's in-tile offset (off_idx) and its unary high part (off_hi), L = ef_low_bits
 };
 
 enum ValueMode : uint32_t {  // TensorDesc::vmode: how a tensor's values travel in the slot (parallel/plan.py VMODE_*)
@@ -76,7 +78,9 @@ struct TensorDesc {
   uint32_t pos_cap;        // the pick runs over the first min(n_pos, pos_cap) positives
   uint32_t off_pos_prefix; // [n_tiles] positives before each tile, capped at pos_cap
   uint32_t off_pick;       // [ceil(pos_cap / 32)] pick bitmask: bit q <=> the q-th positive carries a value
-  uint32_t reserved[2];
+  // ---- kModeEf tensors; 0 otherwise ----
+  uint32_t ef_low_bits;    // L: low bits per entry (0..12); the high stream gives each tile kTile >> L bits + its count
+  uint32_t off_hi;         // [ceil((val_cap + n_tiles * (kTile >> L)) / 32)] high stream
 };
 static_assert(sizeof(TensorDesc) == 128, "TensorDesc must be 32 words");
 constexpr int kDescWords = 32;
@@ -222,7 +226,8 @@ struct EngineParams {
   uint32_t peer_timeout_ms;      // peer-flag waits give up after this long (status 2, output poisoned with NaN, CTA exits)
   int fault;                     // fault injection (tests): 1 = this rank never releases its stage-1 flags
   uint32_t* mc_arena;            // NVLS multicast mapping of the symmetric arena (nullptr: per-peer P2P stores)
-  int has_rle;                   // some tensor uses kModeRle (its bit stream is OR-ed, so it is zeroed every step)
+  int has_rle;                   // some tensor uses kModeRle or kModeEf (their bit streams are OR-ed into the slot, which is
+                                 // zeroed every step; only the <.., true> kernels carry those paths)
   int has_shared;                // some tensor uses kModeShared ('randomk': only the <.., true> kernel carries that path)
   int shard;                     // 1: sharded decode + stage-2 exchange (when world > 1)
   uint32_t s2_words;             // words per stage-2 slot: [count, epoch, 0, 0][idx x cap][val x cap]

@@ -10,6 +10,7 @@ side stream; ``finish()`` makes the optimizer's stream wait on the done events.
 
 CUDA + ('topk' [+ 'index': 'bloom' | plain])  -> fused engine (one kernel/bucket)
 CUDA + 'both' + 'rle' + 'fused_rle_values'    -> fused engine, value codec over the run-length index
+CUDA + 'index'/'both' + 'elias_fano'          -> fused engine, Elias-Fano index (fp32 or any fused value codec)
 CUDA + 'dexp' values + 'fused_dexp'           -> fused engine, double-exponential values (plain, bloom or rle index)
 CUDA + 'bf16' values                          -> fused engine, 16-bit values (plain, bloom or rle index, or 'randomk')
 CUDA + 'randomk' [+ QSGD or bf16 values]      -> fused engine, values only on the wire (shared-seed index)
@@ -44,6 +45,8 @@ def _fused_supported(params: dict) -> bool:
     the per-tensor route it always had (and its checkpoint format).
     Double-exponential values ('dexp') are fused only with ``'fused_dexp': True``, for the same reason: 'value', or
     'both' over the bloom or run-length index.
+    The Elias-Fano index ('elias_fano') is fused wherever the run-length index is, with every value codec and no
+    opt-in key: no earlier dict names it.
     Not fused: 'conflict_sets' without that key (per-tensor GPU kernel), host codecs (Huffman, Deflate, the integer
     family), dexp without 'fused_dexp', non-512 QSGD buckets."""
     if params.get('compressor') not in ('topk', 'threshold') or params.get('communicator', 'allgather') != 'allgather':
@@ -67,6 +70,8 @@ def _fused_supported(params: dict) -> bool:
         return pol_ok
     if dr == 'index' and params.get('index') == 'rle':
         return True                      # lossless tile-local run coding inside the fused kernel
+    if dr == 'index' and params.get('index') == 'elias_fano':
+        return policy != 'conflict_sets'  # lossless tile-local Elias-Fano; the fused plan refuses P2 outside bloom
     if dr == 'value':
         return value_ok or dexp_ok       # coded values + plain indices
     if dr == 'both' and params.get('index', 'bloom') == 'bloom':
@@ -76,6 +81,9 @@ def _fused_supported(params: dict) -> bool:
         # bf16 values need no key, and 'fused_rle_values' keeps its meaning: it refuses them
         rv, bf16 = params.get('fused_rle_values') is True, params.get('value') == 'bf16'
         return ((rv and value_ok and not bf16) or dexp_ok or (bf16 and not rv)) and policy != 'conflict_sets'
+    if dr == 'both' and params.get('index') == 'elias_fano':
+        # every value codec the run-length index fuses, with no opt-in key: no earlier dict names this index
+        return (value_ok or params.get('value') in ('dexp', 'double_exp')) and policy != 'conflict_sets'
     return False
 
 

@@ -17,7 +17,8 @@ Parity with the reference (hangxu0304/DeepReduce), per tensor of the bucket:
   * 'both' (index first, value codec on the re-gathered values, mapping back) — :250-302;
     polyfit segments / fit / restore — :341-425; QSGD — :861-907;
   * per-rank decode + aggregate (+ average) — GRACE Allgather communicator, reference README.md:37;
-  * lossless run-length index (``'index': 'rle'``) — :805-846, here tile-local (see ``ops/csrc/plan.h``).
+  * lossless run-length index (``'index': 'rle'``) — :805-846, here tile-local (see ``ops/csrc/plan.h``);
+  * lossless tile-local Elias-Fano index (``'index': 'elias_fano'``, ``spec.ef_layout``) — no reference counterpart.
 """
 from __future__ import annotations
 
@@ -38,7 +39,7 @@ from ..codecs.polyfit import get_segments, polyfit_eval_oracle, polyfit_fit_orac
 from ..codecs.qsgd import qsgd_decode_oracle, qsgd_encode_oracle
 from ..grace.memory import clip_factor, is_dense, pairwise_sumsq
 from .plan import update_cta_speeds
-from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID, SLOT_HEADER_WORDS,
+from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_EF, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID, SLOT_HEADER_WORDS,
                    VMODE_BF16, VMODE_DEXP, VMODE_QSGD, BucketPlan, rle_stream_words)
 
 (PH_ACCUM, PH_FALLBACK, PH_HIST2, PH_INSERT, PH_QUERY, PH_EMIT, PH_RANK_HIST, PH_RANK_SCAN, PH_RANK_SCATTER,
@@ -103,6 +104,62 @@ def rle_unpack12(stream: np.ndarray, n: int) -> np.ndarray:
     s64 = stream.astype(np.uint64)
     both = s64[w] | (s64[np.minimum(w + 1, s64.size - 1)] << np.uint64(32))
     return ((both >> sh) & np.uint64(0xFFF)).astype(np.int64)
+
+
+def ef_pack(idx: np.ndarray, numel: int, cap: int):
+    """The tile-local Elias-Fano index (``spec.ef_layout``) of the ascending in-tensor indices ``idx`` (at most ``cap``
+    of them) of a ``numel``-element tensor: uint32 words (u16 count per tile, low stream, high stream)."""
+    n_tiles = (int(numel) + spec.TILE - 1) // spec.TILE
+    L, lo_words, hi_words = spec.ef_layout(int(cap), n_tiles)
+    idx = np.asarray(idx, dtype=np.int64)
+    assert idx.size <= cap and np.all(np.diff(idx) > 0) and (idx.size == 0 or (idx[0] >= 0 and idx[-1] < numel))
+    tile, e = idx // spec.TILE, idx % spec.TILE
+    p = np.arange(idx.size, dtype=np.int64)
+    cnt = np.zeros(((n_tiles + 1) // 2) * 2, dtype=np.uint16)
+    cnt[:n_tiles] = np.bincount(tile, minlength=n_tiles)
+    lo = np.zeros(lo_words + 1, dtype=np.uint64)
+    if L:
+        bit = p * L
+        v = (e & ((1 << L) - 1)).astype(np.uint64) << (bit & 31).astype(np.uint64)     # up to 43 bits
+        np.bitwise_or.at(lo, bit >> 5, v & np.uint64(0xFFFFFFFF))
+        np.bitwise_or.at(lo, (bit >> 5) + 1, v >> np.uint64(32))
+    hb = p + tile * (spec.TILE >> L) + (e >> L)
+    hi = np.zeros(hi_words, dtype=np.uint32)
+    np.bitwise_or.at(hi, hb >> 5, np.left_shift(np.uint32(1), (hb & 31).astype(np.uint32)))
+    return cnt.view(np.uint32), lo[:lo_words].astype(np.uint32), hi
+
+
+def ef_unpack(cnt_words: np.ndarray, lo: np.ndarray, hi: np.ndarray, numel: int, cap: int, n: int) -> np.ndarray:
+    """The receiver side of ``ef_pack``: the ``n`` ascending in-tensor indices, read tile by tile as the kernel does
+    (the j-th set bit q of tile t's range gives e = ((q - pre_t - t * B - j) << L) | low(pre_t + j))."""
+    n_tiles = (int(numel) + spec.TILE - 1) // spec.TILE
+    L, lo_words, hi_words = spec.ef_layout(int(cap), n_tiles)
+    B = spec.TILE >> L
+    cnt = np.asarray(cnt_words, dtype=np.uint32).view(np.uint16)[:n_tiles].astype(np.int64)
+    assert int(cnt.sum()) == n <= cap, (int(cnt.sum()), n, cap)
+    bits = np.unpackbits(np.asarray(hi, dtype=np.uint32)[:hi_words].view(np.uint8), bitorder="little")
+    lo64 = np.concatenate([np.asarray(lo, dtype=np.uint32)[:lo_words], [0]]).astype(np.uint64)
+    out, pre = [], 0
+    for t in range(n_tiles):
+        c = int(cnt[t])
+        rng = bits[pre + t * B:pre + c + (t + 1) * B]
+        q = np.flatnonzero(rng)
+        assert q.size == c, (t, q.size, c)           # the range holds exactly the tile's entries
+        j = np.arange(c, dtype=np.int64)
+        h = q - j
+        assert np.all(h < B)
+        p = pre + j
+        if L:
+            bit = p * L
+            w, sh = bit >> 5, (bit & 31).astype(np.uint64)
+            low = (((lo64[w] | (lo64[w + 1] << np.uint64(32))) >> sh) & np.uint64((1 << L) - 1)).astype(np.int64)
+        else:
+            low = np.zeros(c, dtype=np.int64)
+        out.append(t * spec.TILE + ((h << L) | low))
+        pre += c
+    idx = np.concatenate(out) if out else np.zeros(0, dtype=np.int64)
+    assert idx.size == 0 or idx[-1] < numel
+    return idx
 
 
 def _abs_keys(x: torch.Tensor) -> torch.Tensor:
@@ -276,6 +333,16 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
         cnt[:tp.n_tiles] = np.bincount(s_np // spec.TILE, minlength=tp.n_tiles).astype(np.uint16)
         slot[tp.off_prefix:tp.off_prefix + (tp.n_tiles + 1) // 2] = cnt.view(np.uint32)
         slot[tp.off_idx:tp.off_idx + rle_stream_words(tp.val_cap)] = rle_pack12(s_np % spec.TILE, tp.val_cap)
+        cutoff = int(sel[-1].item()) if n_pos >= limit else 0xFFFFFFFF
+    elif tp.mode == MODE_EF:
+        # the run-length index's shipped set, counts and cutoff; the in-tile offsets as the two Elias-Fano streams
+        n_pos = int(sel_topk.numel())
+        limit = tp.val_cap
+        sel = sel_topk[:limit]
+        cnt, lo, hi = ef_pack(sel.cpu().numpy(), tp.numel, tp.val_cap)
+        slot[tp.off_prefix:tp.off_prefix + cnt.size] = cnt
+        slot[tp.off_idx:tp.off_idx + lo.size] = lo
+        slot[tp.off_hi:tp.off_hi + hi.size] = hi
         cutoff = int(sel[-1].item()) if n_pos >= limit else 0xFFFFFFFF
     elif tp.mode == MODE_SHARED:
         # no index on the wire: every receiver draws the same set (the per-tile prefix is sender-local scratch)
@@ -512,6 +579,11 @@ def shipped_index_oracle(plan: BucketPlan, slot, ti: int, *, seed=spec.DEFAULT_S
         assert int(cnt.sum()) == n_sel, t.name
         local = rle_unpack12(a[t.off_idx:t.off_idx + rle_stream_words(t.val_cap)], n_sel)
         idx = torch.from_numpy(np.repeat(np.arange(t.n_tiles, dtype=np.int64), cnt) * spec.TILE + local)
+    elif t.mode == MODE_EF:
+        _, lo_words, hi_words = spec.ef_layout(t.val_cap, t.n_tiles)
+        idx = torch.from_numpy(ef_unpack(a[t.off_prefix:t.off_prefix + (t.n_tiles + 1) // 2],
+                                         a[t.off_idx:t.off_idx + lo_words], a[t.off_hi:t.off_hi + hi_words],
+                                         t.numel, t.val_cap, n_sel))
     elif t.mode == MODE_SHARED:
         # the index set is drawn again from the plan and the epoch in slot word 1; the sender's threshold must match
         pos, thr = select_randomk_oracle(t.numel, t.k, int(a[1]), t.salt)
@@ -734,7 +806,7 @@ class BucketEngine:
                 self.ctx.set_shard(1, s2w, cap)
             if getattr(self, "multicast_ptr", 0):
                 self.ctx.set_multicast(self.multicast_ptr)
-            self.ctx.set_has_rle(int(any(t.mode == MODE_RLE for t in plan.tensors)))
+            self.ctx.set_has_rle(int(any(t.mode in (MODE_RLE, MODE_EF) for t in plan.tensors)))
             # P2 ('conflict_sets'): scratch of the sender stage the C++ engine launches before emit (ops/csrc/p2.cu)
             p2_table, n_p2, p2_words, p2_cap = plan.p2_tables()
             self.p2_table = p2_table.to(dev)

@@ -19,7 +19,7 @@ import torch
 from .. import spec
 from ..codecs.dexp import MIN_NUMEL as DEXP_MIN_NUMEL
 
-MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED = 0, 1, 2, 3
+MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED, MODE_EF = 0, 1, 2, 3, 4
 VMODE_FP32, VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_BF16 = 0, 1, 2, 3, 4   # TensorDesc.vmode (plan.h ValueMode)
 KEY_SPAN = 1 << 31                    # select keys are 31-bit
 POLICY_ID = {"leftmost": 0, "random": 1, "p0": 2, "conflict_sets": 3}
@@ -159,13 +159,16 @@ class TensorPlan:
     pos_cap: int = 0          # P2: the pick runs over the first min(n_pos, pos_cap) positives
     off_pos_prefix: int = 0   # P2: [n_tiles] positives before each tile, capped at pos_cap
     off_pick: int = 0         # P2: [ceil(pos_cap / 32)] pick bitmask over the positives
+    ef_low_bits: int = 0      # MODE_EF: L of spec.ef_layout (the low stream is at off_idx)
+    off_hi: int = 0           # MODE_EF: the high stream
 
     def words(self) -> List[int]:
         return [self.elem_off, self.numel, self.k, self.tile_begin, self.n_tiles, self.mode, self.m_bits,
                 self.n_hash, self.off_vals, self.off_filter, self.off_prefix, self.off_idx, self.val_cap,
                 self.salt, self.n_filter_words, self.off_hint, self.vmode, self.off_coef, self.off_rankmap,
                 self.off_selidx, self.off_sorted, self.poly_degree, self.rank_u32, self.poly_off, self.poly_ord,
-                self.fixed_thr, self.shared_lb, self.pos_cap, self.off_pos_prefix, self.off_pick, 0, 0]
+                self.fixed_thr, self.shared_lb, self.pos_cap, self.off_pos_prefix, self.off_pick, self.ef_low_bits,
+                self.off_hi]
 
     @property
     def ranked(self) -> bool:
@@ -199,6 +202,9 @@ class TensorPlan:
                         (self.n_tiles + (self.pos_cap + 31) // 32 if self.pos_cap else 0))
         if self.mode == MODE_RLE:
             return 4 * ((self.n_tiles + 1) // 2 + rle_stream_words(self.val_cap))
+        if self.mode == MODE_EF:
+            _, lo, hi = spec.ef_layout(self.val_cap, self.n_tiles)
+            return 4 * ((self.n_tiles + 1) // 2 + lo + hi)
         return 0 if self.mode == MODE_SHARED else 4 * self.val_cap
 
 
@@ -208,7 +214,8 @@ class BucketPlan:
     names: Optional[Sequence[str]] = None
     shapes: Optional[Sequence[tuple]] = None
     compress_ratio: float = 0.01
-    index: Optional[str] = "bloom"        # 'bloom', 'rle' (lossless tile-local run coding) or None (plain top-k pairs)
+    index: Optional[str] = "bloom"        # 'bloom', 'rle' (lossless tile-local run coding), 'elias_fano' (lossless
+                                          # tile-local Elias-Fano, spec.ef_layout) or None (plain top-k pairs)
     fpr: Optional[float] = None
     policy: str = "leftmost"
     min_numel: int = spec.SMALL_TENSOR_NUMEL
@@ -230,8 +237,8 @@ class BucketPlan:
     tensors: List[TensorPlan] = field(default_factory=list, init=False)
 
     def __post_init__(self):
-        if self.index not in (None, "bloom", "rle"):
-            raise ValueError(f"fused engine index codecs: None, 'bloom', 'rle'; got {self.index!r}")
+        if self.index not in (None, "bloom", "rle", "elias_fano"):
+            raise ValueError(f"fused engine index codecs: None, 'bloom', 'rle', 'elias_fano'; got {self.index!r}")
         if self.value not in (None, "polyfit", "qsgd", "dexp", "bf16"):
             raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp', 'bf16'; got {self.value!r}")
         if self.sparsifier not in ("topk", "threshold", "randomk"):
@@ -327,6 +334,18 @@ class BucketPlan:
                 word = _align(word + (n_tiles + 1) // 2, 4)
                 tp.off_idx = word
                 word = _align(word + rle_stream_words(k), 4)
+            elif self.index == "elias_fano" and d > self.min_numel:
+                # lossless tile-local Elias-Fano (spec.ef_layout): the values, rle's u16 count per tile, then the low
+                # and the high stream; a static size for the capacity k, whatever is selected
+                tp.mode = MODE_EF
+                tp.val_cap = k
+                word = self._value_region(tp, word, scratch)
+                tp.off_prefix = word
+                word = _align(word + (n_tiles + 1) // 2, 4)
+                tp.ef_low_bits, lo_words, hi_words = spec.ef_layout(k, n_tiles)
+                tp.off_idx = word
+                tp.off_hi = word + lo_words                  # the two streams back to back
+                word = _align(tp.off_hi + hi_words, 4)
             else:
                 tp.val_cap = min(d, k + int(self.raw_slack))
                 if d > self.min_numel:           # value-only mode ('deepreduce': 'value'): coded values + plain indices

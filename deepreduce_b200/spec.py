@@ -157,6 +157,18 @@ def bloom_configuration(k: int, fpr: float) -> Tuple[int, int]:
     return m, int(math.ceil(h))
 
 
+def ef_layout(cap: int, n_tiles: int) -> Tuple[int, int, int]:
+    """Tile-local Elias-Fano index (``'index': 'elias_fano'``) of a tensor of ``n_tiles`` tiles holding up to ``cap``
+    entries: (L, low-stream words, high-stream words).  L = argmin over 0..12 of cap * L + n_tiles * (TILE >> L), the
+    smallest on ties.  Entry p (its rank in ascending index order), with in-tile offset e in tile-local tile t, puts
+    e & (2^L - 1) at bit p * L of the low stream (cap * L bits) and sets bit p + t * (TILE >> L) + (e >> L) of the high
+    stream (cap + n_tiles * (TILE >> L) bits), both LSB-first; a u16 entry count per tile (the run-length index's table)
+    goes with them.  Tile t owns the high bits [pre_t + t * B, pre_t + c_t + (t + 1) * B), B = TILE >> L, where pre_t
+    entries lie in the earlier tiles and c_t in t: its j-th set bit q gives e = ((q - pre_t - t * B - j) << L) | low."""
+    L = min(range(13), key=lambda l: cap * l + n_tiles * (TILE >> l))
+    return L, (cap * L + 31) // 32, (cap + n_tiles * (TILE >> L) + 31) // 32
+
+
 def topk_k(numel: int, ratio: float) -> int:
     """GRACE top-k K (SURVEY §2.5)."""
     return max(1, int(numel * ratio))

@@ -66,6 +66,8 @@ def main():
                            ("BF (leftmost) + Fit-Poly ('both')", {**base, 'compress_ratio': 0.01, 'deepreduce': 'both',
                                                                   'index': 'bloom', 'value': 'polyfit'}, None),
                            ("RLE index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'rle'}, None),
+                           ("Elias-Fano index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index',
+                                                 'index': 'elias_fano'}, None),
                            ("delta + bp128 index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'integer'}, None),
                            ("Huffman index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'huffman'}, None)):
         ours = top if cfg is None else model_volume(m, cfg)
