@@ -11,7 +11,8 @@ from .lossless import Gzip, Huffman
 from .polyfit import PolyFit, PolyFitCPU, get_segments
 from .qsgd import QSGD
 from .rle import RunLength
+from .sign import Sign
 
 __all__ = ["SparseCompressor", "compressor", "register", "bitpack", "BF16", "Bloom", "Bloomfilter", "get_BFconfig",
            "BloomCPU", "bloom_compress_blob", "bloom_decompress_blob", "DoubleExp", "EliasFano", "IntegerIndex", "Gzip",
-           "Huffman", "PolyFit", "PolyFitCPU", "get_segments", "QSGD", "RunLength"]
+           "Huffman", "PolyFit", "PolyFitCPU", "get_segments", "QSGD", "RunLength", "Sign"]

@@ -148,6 +148,10 @@ class DeepReduceConfig:
             raise ConfigError("'p2_pick_mask' applies to the top-k sparsifier with the bloom index and policy "
                               f"'conflict_sets' (got compressor={cfg.compressor!r}, deepreduce={cfg.deepreduce!r}, "
                               f"index={cfg.index!r}, policy={cfg.policy!r})")
+        # scaled-sign values code fixed 512-value buckets, in the fused engine and per tensor alike
+        if cfg.deepreduce in ("value", "both") and cfg.value == "sign" and cfg.bucket_size != 512:
+            raise ConfigError(f"'value': 'sign' codes buckets of 512 values; 'bucket_size' must be 512 or left out "
+                              f"(got {cfg.bucket_size})")
         # opt-in route of 'both' + run-length index through the fused engine (the value codec rides behind the index);
         # without it that combination keeps the per-tensor path and its checkpoints
         rv = g("fused_rle_values", False)

@@ -145,6 +145,17 @@ def qsgd_decode(lvl, norms, q, bucket):
     return cuda_module().qsgd_decode(lvl.contiguous(), norms.contiguous(), int(q), int(bucket))
 
 
+def sign_encode(vals):
+    """Scaled-sign code of fp32 ``vals`` in 512-value buckets: (bits int32[ceil(K/32)], scales fp32[ceil(K/512)]);
+    torch oracle: codecs.sign.sign_encode_oracle."""
+    bits, scales = cuda_module().sign_encode(vals.float().contiguous())
+    return bits, scales
+
+
+def sign_decode(bits, scales, K):
+    return cuda_module().sign_decode(bits.contiguous(), scales.contiguous(), int(K))
+
+
 def pack_bits(vals, bits):
     return cuda_module().pack_bits(vals.contiguous(), int(bits))
 

@@ -91,6 +91,34 @@ static torch::Tensor qsgd_decode(torch::Tensor lvl, torch::Tensor norms, int64_t
   return out;
 }
 
+// scaled sign, 512-value buckets: {bits int32[ceil(K/32)], scales fp32[ceil(K/512)]}
+static std::vector<torch::Tensor> sign_encode(torch::Tensor vals) {
+  CHECK_CUDA_T(vals);
+  TORCH_CHECK(vals.scalar_type() == torch::kFloat32, "sign_encode: vals must be float32");
+  c10::cuda::CUDAGuard g(vals.device());
+  const int64_t K = vals.numel();
+  auto bits = torch::empty({(K + 31) / 32}, vals.options().dtype(torch::kInt32));
+  auto scales = torch::empty({(K + 511) / 512}, vals.options());
+  dr::launch_sign_encode(vals.data_ptr<float>(), K, (uint32_t*)bits.data_ptr<int32_t>(), scales.data_ptr<float>(),
+                         cur_stream());
+  check_last("sign_encode");
+  return {bits, scales};
+}
+
+static torch::Tensor sign_decode(torch::Tensor bits, torch::Tensor scales, int64_t K) {
+  CHECK_CUDA_T(bits); CHECK_CUDA_T(scales);
+  TORCH_CHECK(bits.scalar_type() == torch::kInt32 && scales.scalar_type() == torch::kFloat32,
+              "sign_decode: bits must be int32 and scales float32");
+  TORCH_CHECK(K >= 0 && bits.numel() == (K + 31) / 32 && scales.numel() == (K + 511) / 512,
+              "sign_decode: ", K, " values need ", (K + 31) / 32, " bit words and ", (K + 511) / 512, " scales");
+  c10::cuda::CUDAGuard g(bits.device());
+  auto out = torch::empty({K}, scales.options());
+  dr::launch_sign_decode((const uint32_t*)bits.data_ptr<int32_t>(), scales.data_ptr<float>(), K, out.data_ptr<float>(),
+                         cur_stream());
+  check_last("sign_decode");
+  return out;
+}
+
 static torch::Tensor pack_bits(torch::Tensor vals, int64_t bits) {
   CHECK_CUDA_T(vals);
   TORCH_CHECK(1 <= bits && bits <= 63, "pack_bits: bits must be in [1, 63], got ", bits);
@@ -827,6 +855,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bloom_select", &bloom_select);
   m.def("qsgd_encode", &qsgd_encode);
   m.def("qsgd_decode", &qsgd_decode);
+  m.def("sign_encode", &sign_encode);
+  m.def("sign_decode", &sign_decode);
   m.def("pack_bits", &pack_bits);
   m.def("unpack_bits", &unpack_bits);
   m.def("polyfit_fit", &polyfit_fit);

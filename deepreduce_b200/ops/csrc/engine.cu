@@ -32,6 +32,7 @@
 #include "common.cuh"
 #include "dexp_fit.cuh"
 #include "plan.h"
+#include "sign_values.cuh"
 #include "tiles.cuh"
 
 #include <cuda_bf16.h>
@@ -88,6 +89,7 @@ struct Smem {
     uint32_t excl[kTile];                     // emit: exclusive prefixes of a chunk of tiles
     uint32_t sel[kWarps][32];                 // insert: selected elements of one warp iteration
     DexpScratch dexp;                         // fit phase: one double-exponential fit
+    double sign_ws[kWarps];                   // fix phase, kVmodeSign: the warp sums of one bucket's |v|
   } u;
   ScanSmem s;
   TensorDesc td;                              // current tensor
@@ -1749,6 +1751,29 @@ DR_D void phase_fit(const EngineParams& P, Smem& sm) {
   }
 }
 
+// kVmodeSign fix task: this CTA owns one 512-value bucket and its 16 bit words (lane 0 of each warp writes its ballot).
+// Not inlined, so that its fp64 sums do not take registers from the rest of the kernel.
+template <bool kDgc>
+__device__ __noinline__ void fix_sign(const EngineParams& P, Smem& sm, uint32_t* my_slot, uint32_t t, uint32_t p0) {
+  const DynHeader* dyn = reinterpret_cast<const DynHeader*>(my_slot + kSlotHeaderWords) + t;
+  const uint32_t nq = __ldcg(&dyn->n_sel);
+  if (p0 >= nq) return;
+  const uint32_t p = p0 + threadIdx.x;
+  const float v = p < nq ? __ldcg(reinterpret_cast<const float*>(my_slot + sm.td.off_vals) + p) : 0.f;
+  const float mu = sign_scale(v, min(nq - p0, kSignBucket), sm.u.sign_ws);
+  const uint32_t word = sign_word(v);
+  if (threadIdx.x == 0) reinterpret_cast<float*>(my_slot + sm.td.off_coef)[p0 >> 9] = mu;
+  if (p < nq) {
+    if ((threadIdx.x & 31u) == 0) my_slot[sm.td.off_rankmap + (p >> 5)] = word;
+    // the residual keeps v - d, 0 where d is not finite (a NaN or inf in the bucket); the sign bit follows v, so
+    // v - d cannot overflow
+    const float d = sign_decoded(v < 0.f, mu);
+    const uint32_t gi = __ldcg(my_slot + sm.td.off_selidx + p);
+    P.resid[gi] = isfinite(d) ? __fsub_rn(v, d) : 0.0f;
+    if constexpr (kDgc) { if (d != 0.0f) P.mom[gi] = 0.0f; }
+  }
+}
+
 // phase 11: error feedback sees the fit error: resid[idx_p] = value_p - fitted_p
 // (kDgc: and the momentum of idx_p is cleared when the decoded value, the one every receiver rebuilds, is non-zero)
 template <bool kDgc>
@@ -1790,6 +1815,7 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
       }
       continue;
     }
+    if (sm.td.vmode == kVmodeSign) { fix_sign<kDgc>(P, sm, my_slot, t, p0); continue; }
     const int deg = (int)sm.td.poly_degree;
     const uint32_t* tail = my_slot + sm.td.off_coef + coef_words(sm.td.vmode, deg);
     const int num_pos = (int)__ldcg(tail), n = (int)__ldcg(tail + 1);
@@ -1914,6 +1940,9 @@ DR_D float coded_value(const uint32_t* slot, const TensorDesc& td, const float* 
   if (kFull && ranked(td.vmode)) return __ldcg(fitted + load_rank(slot, td, rp));
   if constexpr (kFull) {
     if (td.vmode == kVmodeBf16) return __uint_as_float((uint32_t)__ldcg(reinterpret_cast<const uint16_t*>(vals) + rp) << 16);
+    if (td.vmode == kVmodeSign)
+      return sign_decoded((__ldcg(slot + td.off_rankmap + (rp >> 5)) >> (rp & 31u)) & 1u,
+                          __ldcg(reinterpret_cast<const float*>(slot + td.off_coef) + (rp >> 9)));
   }
   if (kFull && td.vmode == kVmodeQsgd) {
     const float norm = __ldcg(reinterpret_cast<const float*>(slot + td.off_coef) + (rp >> 9));

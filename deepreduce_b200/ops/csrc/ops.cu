@@ -1,11 +1,12 @@
 // Stand-alone sm_90a kernels behind the GRACE-compatible per-tensor codec API
-// (deepreduce_b200/codecs/*): bloom insert / universe query+select, QSGD,
+// (deepreduce_b200/codecs/*): bloom insert / universe query+select, QSGD, scaled sign,
 // bit packing, Gram-polynomial fit/eval, delta+bp128 integer coding.
 // Each has a plain-torch oracle in the codec module; tests compare them.
 #include "common.cuh"
 #include "conflict_sets.cuh"
 #include "dexp_fit.cuh"
 #include "ops.h"
+#include "sign_values.cuh"
 
 namespace dr {
 namespace {
@@ -142,6 +143,26 @@ __global__ void qsgd_decode_kernel(const InT* __restrict__ lvl, const float* __r
                                    int q, float* __restrict__ out) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < K; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = norms[i / bucket] / (float)q * (float)lvl[i];
+}
+
+// ---------------------------------------------------------------------------
+// scaled sign: one 512-thread CTA per 512-value bucket (the fused engine's fix phase runs the same rule per task)
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads) sign_encode_kernel(const float* __restrict__ v, int64_t K,
+                                                               uint32_t* __restrict__ bits, float* __restrict__ scales) {
+  __shared__ double ws[kWarps];
+  const int64_t p = (int64_t)blockIdx.x * kSignBucket + threadIdx.x;
+  const float x = p < K ? v[p] : 0.f;
+  const float mu = sign_scale(x, (uint32_t)min((int64_t)kSignBucket, K - (int64_t)blockIdx.x * kSignBucket), ws);
+  const uint32_t word = sign_word(x);
+  if (threadIdx.x == 0) scales[blockIdx.x] = mu;
+  if ((threadIdx.x & 31u) == 0 && p < K) bits[p >> 5] = word;
+}
+
+__global__ void sign_decode_kernel(const uint32_t* __restrict__ bits, const float* __restrict__ scales, int64_t K,
+                                   float* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < K; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = sign_decoded((bits[i >> 5] >> (i & 31)) & 1u, scales[i / kSignBucket]);
 }
 
 // ---------------------------------------------------------------------------
@@ -432,6 +453,18 @@ void launch_qsgd_decode(const void* lvl, bool i16, const float* norms, int64_t K
   count_launch();
   if (i16) qsgd_decode_kernel<int16_t><<<grid_for(K, 256), 256, 0, st>>>((const int16_t*)lvl, norms, K, bucket, q, out);
   else qsgd_decode_kernel<int8_t><<<grid_for(K, 256), 256, 0, st>>>((const int8_t*)lvl, norms, K, bucket, q, out);
+}
+
+void launch_sign_encode(const float* v, int64_t K, uint32_t* bits, float* scales, cudaStream_t st) {
+  if (K == 0) return;
+  count_launch();
+  sign_encode_kernel<<<(unsigned)((K + kSignBucket - 1) / kSignBucket), kThreads, 0, st>>>(v, K, bits, scales);
+}
+
+void launch_sign_decode(const uint32_t* bits, const float* scales, int64_t K, float* out, cudaStream_t st) {
+  if (K == 0) return;
+  count_launch();
+  sign_decode_kernel<<<grid_for(K, 256), 256, 0, st>>>(bits, scales, K, out);
 }
 
 void launch_pack_bits(const int64_t* vals, int64_t n, int bits, uint32_t* out, int64_t n_words, cudaStream_t st) {

@@ -38,6 +38,9 @@ enum ValueMode : uint32_t {  // TensorDesc::vmode: how a tensor's values travel 
   kVmodeDexp = 3,     // double-exponential fit of each sign run + rank map
   kVmodeBf16 = 4,     // bf16 values: the p-th value's bits in half p % 2 (low half first) of word off_vals + p / 2,
                       // rounded by emit, which also writes the residual (no scratch, no rank / fit / fix phase)
+  kVmodeSign = 5,     // scaled sign (sign_values.cuh): per 512-value bucket b one fp32 scale mu_b at off_coef + b, then
+                      // one bit per value at off_rankmap, LSB first (value p is bit p % 32 of word p / 32, 1 <=> v < 0);
+                      // decodes to bit ? -mu_b : +mu_b.  off_vals / off_selidx are sender-local scratch (fix phase)
 };
 
 // kPolicyP2 ('conflict_sets', opt-in): the sender draws the pick over its positives and ships it as a bitmask (p2.cu);

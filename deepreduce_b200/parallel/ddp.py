@@ -13,7 +13,8 @@ CUDA + 'both' + 'rle' + 'fused_rle_values'    -> fused engine, value codec over 
 CUDA + 'index'/'both' + 'elias_fano'          -> fused engine, Elias-Fano index (fp32 or any fused value codec)
 CUDA + 'dexp' values + 'fused_dexp'           -> fused engine, double-exponential values (plain, bloom or rle index)
 CUDA + 'bf16' values                          -> fused engine, 16-bit values (plain, bloom or rle index, or 'randomk')
-CUDA + 'randomk' [+ QSGD or bf16 values]      -> fused engine, values only on the wire (shared-seed index)
+CUDA + 'sign' values                          -> fused engine, 1-bit scaled-sign values (wherever bf16 values are)
+CUDA + 'randomk' [+ QSGD, bf16 or sign values] -> fused engine, values only on the wire (shared-seed index)
 CUDA + 'none'/'allreduce'                     -> dense NCCL all-reduce of the flat bucket
 anything else (CPU/gloo, other codecs)        -> GRACE-compatible per-tensor path
 """
@@ -38,7 +39,8 @@ def _fused_supported(params: dict) -> bool:
     takes the GRACE-compatible per-tensor path, unless ``_fused_randomk_supported`` takes it).  Covers every recipe of
     the reference's launch script (run_deepreduce.sh:35-107): top-k or threshold sparsifier x {no codec, index (bloom
     leftmost / random / p0, run-length), value (polyfit, QSGD int8/int16), both}, and bf16 values (``'value': 'bf16'``)
-    over the plain, bloom or run-length index, with no opt-in key: no earlier dict names 'bf16'.
+    over the plain, bloom or run-length index, with no opt-in key: no earlier dict names 'bf16'.  Scaled-sign values
+    (``'value': 'sign'``, 512-value buckets) take every route bf16 values take, with no opt-in key either.
     Bloom policy 'conflict_sets' (P2) is fused only with top-k and ``'p2_pick_mask': True``: the sender then ships its pick as a
     bitmask over the positives, a different wire from the reference's, where every receiver redraws the pick.
     'both' with the run-length index is fused only with ``'fused_rle_values': True``: without the key that dict keeps
@@ -59,7 +61,7 @@ def _fused_supported(params: dict) -> bool:
     # P2 needs top-k: under 'threshold' K is the slot capacity, so the draw would keep every positive
     p2_ok = policy == 'conflict_sets' and params.get('p2_pick_mask') is True and params.get('compressor') == 'topk'
     pol_ok = policy in ('leftmost', 'random', 'p0') or p2_ok
-    value_ok = (params.get('value', 'polyfit') in ('polyfit', 'bf16')
+    value_ok = (params.get('value', 'polyfit') in ('polyfit', 'bf16', 'sign')
                 or (params.get('value') == 'qsgd' and 1 <= int(params.get('quantum_num', 127)) <= 32767
                     and int(params.get('bucket_size', 512)) == 512))
     # the same index rule whether the index is shipped ('both') or not ('value'), as the config check has it
@@ -78,9 +80,9 @@ def _fused_supported(params: dict) -> bool:
         return pol_ok and (value_ok or dexp_ok)
     if dr == 'both' and params.get('index') == 'rle':
         # the bloom policies do not apply to a lossless index; the fused plan refuses 'conflict_sets' outside bloom
-        # bf16 values need no key, and 'fused_rle_values' keeps its meaning: it refuses them
-        rv, bf16 = params.get('fused_rle_values') is True, params.get('value') == 'bf16'
-        return ((rv and value_ok and not bf16) or dexp_ok or (bf16 and not rv)) and policy != 'conflict_sets'
+        # bf16 and sign values need no key, and 'fused_rle_values' keeps its meaning: it refuses them
+        rv, keyless = params.get('fused_rle_values') is True, params.get('value') in ('bf16', 'sign')
+        return ((rv and value_ok and not keyless) or dexp_ok or (keyless and not rv)) and policy != 'conflict_sets'
     if dr == 'both' and params.get('index') == 'elias_fano':
         # every value codec the run-length index fuses, with no opt-in key: no earlier dict names this index
         return (value_ok or params.get('value') in ('dexp', 'double_exp')) and policy != 'conflict_sets'
@@ -91,14 +93,15 @@ def _fused_randomk_supported(params: dict) -> bool:
     """Which 'randomk' ``params`` dicts the fused engine serves in its shared-index mode (``kModeShared``): every rank
     draws the same index set from (step, tensor), so only values travel and the allgather and allreduce communicators
     give the same aggregate.  With no codec, with QSGD values (``'deepreduce': 'value', 'value': 'qsgd'``, bucket
-    512) or with bf16 values (``'value': 'bf16'``).  Not fused: 'randomk' with an index codec, 'both', or polyfit
-    values."""
+    512), with bf16 values (``'value': 'bf16'``) or with scaled-sign values (``'value': 'sign'``).  Not fused:
+    'randomk' with an index codec, 'both', or polyfit values."""
     if params.get('compressor') != 'randomk' or params.get('communicator', 'allgather') not in ('allgather', 'allreduce'):
         return False
     dr = params.get('deepreduce', None)
     v = params.get('value', 'polyfit')
-    return dr is None or (dr == 'value' and (v == 'bf16' or (v == 'qsgd' and 1 <= int(params.get('quantum_num', 127)) <= 32767
-                                                              and int(params.get('bucket_size', 512)) == 512)))
+    return dr is None or (dr == 'value' and (v in ('bf16', 'sign')
+                                             or (v == 'qsgd' and 1 <= int(params.get('quantum_num', 127)) <= 32767
+                                                 and int(params.get('bucket_size', 512)) == 512)))
 
 
 BUCKET_DTYPES = (torch.float32, torch.bfloat16)

@@ -20,7 +20,7 @@ from .. import spec
 from ..codecs.dexp import MIN_NUMEL as DEXP_MIN_NUMEL
 
 MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED, MODE_EF = 0, 1, 2, 3, 4
-VMODE_FP32, VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_BF16 = 0, 1, 2, 3, 4   # TensorDesc.vmode (plan.h ValueMode)
+VMODE_FP32, VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_BF16, VMODE_SIGN = 0, 1, 2, 3, 4, 5   # TensorDesc.vmode (plan.h ValueMode)
 KEY_SPAN = 1 << 31                    # select keys are 31-bit
 POLICY_ID = {"leftmost": 0, "random": 1, "p0": 2, "conflict_sets": 3}
 P2_MAX_POS_CAP = 1 << 20              # P2: the draw keeps one chosen bit per positive in shared memory (128 KB)
@@ -177,8 +177,8 @@ class TensorPlan:
 
     @property
     def coded(self) -> bool:
-        """A fix phase writes the residual (polyfit, QSGD, dexp); emit knows the other modes' decoded values."""
-        return self.vmode in (VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP)
+        """A fix phase writes the residual (polyfit, QSGD, dexp, sign); emit knows the other modes' decoded values."""
+        return self.vmode in (VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_SIGN)
 
     @property
     def coef_words(self) -> int:
@@ -192,6 +192,8 @@ class TensorPlan:
             return 4 * (self.coef_words + 2) + (4 if self.rank_u32 else 2) * self.val_cap
         if self.vmode == VMODE_QSGD:
             return 4 * ((self.val_cap + 511) // 512) + self.val_cap * (2 if self.rank_u32 else 1)
+        if self.vmode == VMODE_SIGN:
+            return 4 * ((self.val_cap + 511) // 512) + 4 * ((self.val_cap + 31) // 32)
         return (2 if self.vmode == VMODE_BF16 else 4) * self.val_cap
 
     @property
@@ -222,8 +224,8 @@ class BucketPlan:
     max_hash: int = 16
     ks: Optional[Sequence[int]] = None    # explicit per-tensor K (overrides compress_ratio)
     hint: bool = True                     # ship the 1-bit-per-32-elements occupancy hint next to each bloom filter
-    value: Optional[str] = None           # None (fp32 values), 'polyfit', 'qsgd', 'dexp' or 'bf16' ('both': bloom or rle
-                                          # index + value codec)
+    value: Optional[str] = None           # None (fp32 values), 'polyfit', 'qsgd', 'dexp', 'bf16' or 'sign' ('both': an
+                                          # index codec + value codec)
     quantum_num: int = 127                # QSGD levels (int8 on the wire)
     poly_degree: int = 5
     poly_min_k: int = 512                 # tensors shipping fewer values keep them as fp32 (the fit header would be larger)
@@ -239,8 +241,9 @@ class BucketPlan:
     def __post_init__(self):
         if self.index not in (None, "bloom", "rle", "elias_fano"):
             raise ValueError(f"fused engine index codecs: None, 'bloom', 'rle', 'elias_fano'; got {self.index!r}")
-        if self.value not in (None, "polyfit", "qsgd", "dexp", "bf16"):
-            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp', 'bf16'; got {self.value!r}")
+        if self.value not in (None, "polyfit", "qsgd", "dexp", "bf16", "sign"):
+            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp', 'bf16', 'sign'; "
+                             f"got {self.value!r}")
         if self.sparsifier not in ("topk", "threshold", "randomk"):
             raise ValueError(f"fused engine sparsifiers: 'topk', 'threshold', 'randomk'; got {self.sparsifier!r}")
         shared = self.sparsifier == "randomk"
@@ -248,7 +251,7 @@ class BucketPlan:
             raise ValueError("'randomk' ships no index (every rank draws the same set): pass index=None")
         if shared and self.value in ("polyfit", "dexp"):
             # rank_bin centres the value bins on the selection threshold, which here is a hash, not a magnitude
-            raise NotImplementedError(f"'randomk' is fused with fp32, QSGD or bf16 values, not with {self.value!r}")
+            raise NotImplementedError(f"'randomk' is fused with fp32, QSGD, bf16 or sign values, not with {self.value!r}")
         if self.value == "qsgd" and not (1 <= int(self.quantum_num) <= 32767):
             raise ValueError("quantum_num must be in [1, 32767]")
         fixed_thr = 0
@@ -390,6 +393,15 @@ class BucketPlan:
             word = _align(word + (tp.val_cap + 511) // 512, 4)
             tp.off_rankmap = word                        # levels
             word = _align(word + ((tp.val_cap + 1) // 2 if tp.rank_u32 else (tp.val_cap + 3) // 4), 4)
+            scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap)]
+        elif self.value == "sign":
+            # scaled sign (codecs/sign.py), 512-value buckets: one fp32 scale per bucket + one sign bit per value; the
+            # fix phase codes them from the fp32 values in sender-local scratch, as QSGD's does
+            tp.vmode = VMODE_SIGN
+            tp.off_coef = word                           # scales
+            word = _align(word + (tp.val_cap + 511) // 512, 4)
+            tp.off_rankmap = word                        # sign bits, LSB first
+            word = _align(word + (tp.val_cap + 31) // 32, 4)
             scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap)]
         else:
             # fp32 values, or bf16 values two per word (the p-th value in the low half of word p // 2): emit rounds them

@@ -68,6 +68,8 @@ def main():
                            ("RLE index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'rle'}, None),
                            ("Elias-Fano index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index',
                                                  'index': 'elias_fano'}, None),
+                           ("Elias-Fano index + sign values", {**base, 'compress_ratio': 0.01, 'deepreduce': 'both',
+                                                               'index': 'elias_fano', 'value': 'sign'}, None),
                            ("delta + bp128 index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'integer'}, None),
                            ("Huffman index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'huffman'}, None)):
         ours = top if cfg is None else model_volume(m, cfg)
