@@ -152,6 +152,11 @@ class DeepReduceConfig:
         if cfg.deepreduce in ("value", "both") and cfg.value == "sign" and cfg.bucket_size != 512:
             raise ConfigError(f"'value': 'sign' codes buckets of 512 values; 'bucket_size' must be 512 or left out "
                               f"(got {cfg.bucket_size})")
+        # fp8 values code fixed 32-value blocks (one warp each); 'bucket_size' may name that size or be left out
+        if (cfg.deepreduce in ("value", "both") and cfg.value == "fp8" and "bucket_size" in params
+                and params["bucket_size"] != 32):
+            raise ConfigError(f"'value': 'fp8' codes blocks of 32 values; 'bucket_size' must be 32 or left out "
+                              f"(got {params['bucket_size']!r})")
         # opt-in route of 'both' + run-length index through the fused engine (the value codec rides behind the index);
         # without it that combination keeps the per-tensor path and its checkpoints
         rv = g("fused_rle_values", False)

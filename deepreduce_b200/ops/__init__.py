@@ -156,6 +156,17 @@ def sign_decode(bits, scales, K):
     return cuda_module().sign_decode(bits.contiguous(), scales.contiguous(), int(K))
 
 
+def fp8_encode(vals):
+    """E4M3 code of fp32 ``vals`` with a scale byte per 32-value block: (scale words int32[ceil(ceil(K/32)/4)], element
+    words int32[ceil(K/4)]), four bytes per word; torch oracle: codecs.fp8.fp8_encode_oracle."""
+    scales, elems = cuda_module().fp8_encode(vals.float().contiguous())
+    return scales, elems
+
+
+def fp8_decode(scales, elems, K):
+    return cuda_module().fp8_decode(scales.contiguous(), elems.contiguous(), int(K))
+
+
 def pack_bits(vals, bits):
     return cuda_module().pack_bits(vals.contiguous(), int(bits))
 

@@ -119,6 +119,35 @@ static torch::Tensor sign_decode(torch::Tensor bits, torch::Tensor scales, int64
   return out;
 }
 
+// fp8 values, 32-value blocks: {scale bytes int32[ceil(ceil(K/32)/4)], element bytes int32[ceil(K/4)]}, four bytes per
+// word, byte p in bits 8 (p % 4) of word p / 4
+static std::vector<torch::Tensor> fp8_encode(torch::Tensor vals) {
+  CHECK_CUDA_T(vals);
+  TORCH_CHECK(vals.scalar_type() == torch::kFloat32, "fp8_encode: vals must be float32");
+  c10::cuda::CUDAGuard g(vals.device());
+  const int64_t K = vals.numel();
+  auto scales = torch::empty({(K + 127) / 128}, vals.options().dtype(torch::kInt32));
+  auto elems = torch::empty({(K + 3) / 4}, vals.options().dtype(torch::kInt32));
+  dr::launch_fp8_encode(vals.data_ptr<float>(), K, (uint32_t*)scales.data_ptr<int32_t>(),
+                        (uint32_t*)elems.data_ptr<int32_t>(), cur_stream());
+  check_last("fp8_encode");
+  return {scales, elems};
+}
+
+static torch::Tensor fp8_decode(torch::Tensor scales, torch::Tensor elems, int64_t K) {
+  CHECK_CUDA_T(scales); CHECK_CUDA_T(elems);
+  TORCH_CHECK(scales.scalar_type() == torch::kInt32 && elems.scalar_type() == torch::kInt32,
+              "fp8_decode: scales and elems must be int32 words");
+  TORCH_CHECK(K >= 0 && scales.numel() == (K + 127) / 128 && elems.numel() == (K + 3) / 4,
+              "fp8_decode: ", K, " values need ", (K + 127) / 128, " scale words and ", (K + 3) / 4, " element words");
+  c10::cuda::CUDAGuard g(scales.device());
+  auto out = torch::empty({K}, scales.options().dtype(torch::kFloat32));
+  dr::launch_fp8_decode((const uint32_t*)scales.data_ptr<int32_t>(), (const uint32_t*)elems.data_ptr<int32_t>(), K,
+                        out.data_ptr<float>(), cur_stream());
+  check_last("fp8_decode");
+  return out;
+}
+
 static torch::Tensor pack_bits(torch::Tensor vals, int64_t bits) {
   CHECK_CUDA_T(vals);
   TORCH_CHECK(1 <= bits && bits <= 63, "pack_bits: bits must be in [1, 63], got ", bits);
@@ -857,6 +886,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("qsgd_decode", &qsgd_decode);
   m.def("sign_encode", &sign_encode);
   m.def("sign_decode", &sign_decode);
+  m.def("fp8_encode", &fp8_encode);
+  m.def("fp8_decode", &fp8_decode);
   m.def("pack_bits", &pack_bits);
   m.def("unpack_bits", &unpack_bits);
   m.def("polyfit_fit", &polyfit_fit);

@@ -31,6 +31,7 @@
 // full/empty ring + warp-private work, probe chains run on dense survivor batches.
 #include "common.cuh"
 #include "dexp_fit.cuh"
+#include "fp8_values.cuh"
 #include "plan.h"
 #include "sign_values.cuh"
 #include "tiles.cuh"
@@ -90,6 +91,7 @@ struct Smem {
     uint32_t sel[kWarps][32];                 // insert: selected elements of one warp iteration
     DexpScratch dexp;                         // fit phase: one double-exponential fit
     double sign_ws[kWarps];                   // fix phase, kVmodeSign: the warp sums of one bucket's |v|
+    uint32_t fp8_scales[kWarps / 4];          // fix phase, kVmodeFp8: the scale bytes of one task's 16 blocks
   } u;
   ScanSmem s;
   TensorDesc td;                              // current tensor
@@ -1774,6 +1776,32 @@ __device__ __noinline__ void fix_sign(const EngineParams& P, Smem& sm, uint32_t*
   }
 }
 
+// kVmodeFp8 fix task: this CTA owns 512 values, 16 blocks of 32 (one per warp).  The 16 scale bytes are collected in
+// shared memory and written as 4 whole words; lanes 0, 4, .., 28 of each warp write the element words.  A task starts
+// at a multiple of 512 values, so no word is shared between tasks.  Not inlined, as fix_sign.
+template <bool kDgc>
+__device__ __noinline__ void fix_fp8(const EngineParams& P, Smem& sm, uint32_t* my_slot, uint32_t t, uint32_t p0) {
+  const DynHeader* dyn = reinterpret_cast<const DynHeader*>(my_slot + kSlotHeaderWords) + t;
+  const uint32_t nq = __ldcg(&dyn->n_sel);
+  if (p0 >= nq) return;
+  const uint32_t p = p0 + threadIdx.x, lane = threadIdx.x & 31u;
+  const float v = p < nq ? __ldcg(reinterpret_cast<const float*>(my_slot + sm.td.off_vals) + p) : 0.f;
+  const uint32_t s = fp8_block_scale(v);              // blocks past the end: A = 0, scale byte 0
+  const uint32_t word = fp8_elem_word(v, s);
+  if (lane == 0) reinterpret_cast<uint8_t*>(sm.u.fp8_scales)[threadIdx.x >> 5] = (uint8_t)s;
+  __syncthreads();
+  if (threadIdx.x < kWarps / 4 && p0 + 128u * threadIdx.x < nq)
+    my_slot[sm.td.off_coef + (p0 >> 7) + threadIdx.x] = sm.u.fp8_scales[threadIdx.x];
+  if (p < nq) {
+    if ((lane & 3u) == 0) my_slot[sm.td.off_rankmap + (p >> 2)] = word;
+    // the residual keeps v - d, 0 where d is not finite (an inf or a NaN in the block)
+    const float d = fp8_decoded(s, word & 0xFFu);     // every lane's own byte is the low byte of its word
+    const uint32_t gi = __ldcg(my_slot + sm.td.off_selidx + p);
+    P.resid[gi] = isfinite(d) ? __fsub_rn(v, d) : 0.0f;
+    if constexpr (kDgc) { if (d != 0.0f) P.mom[gi] = 0.0f; }
+  }
+}
+
 // phase 11: error feedback sees the fit error: resid[idx_p] = value_p - fitted_p
 // (kDgc: and the momentum of idx_p is cleared when the decoded value, the one every receiver rebuilds, is non-zero)
 template <bool kDgc>
@@ -1816,6 +1844,7 @@ DR_D void phase_fix(const EngineParams& P, Smem& sm) {
       continue;
     }
     if (sm.td.vmode == kVmodeSign) { fix_sign<kDgc>(P, sm, my_slot, t, p0); continue; }
+    if (sm.td.vmode == kVmodeFp8) { fix_fp8<kDgc>(P, sm, my_slot, t, p0); continue; }
     const int deg = (int)sm.td.poly_degree;
     const uint32_t* tail = my_slot + sm.td.off_coef + coef_words(sm.td.vmode, deg);
     const int num_pos = (int)__ldcg(tail), n = (int)__ldcg(tail + 1);
@@ -1943,6 +1972,9 @@ DR_D float coded_value(const uint32_t* slot, const TensorDesc& td, const float* 
     if (td.vmode == kVmodeSign)
       return sign_decoded((__ldcg(slot + td.off_rankmap + (rp >> 5)) >> (rp & 31u)) & 1u,
                           __ldcg(reinterpret_cast<const float*>(slot + td.off_coef) + (rp >> 9)));
+    if (td.vmode == kVmodeFp8)        // block rp / 32's scale byte, then the element byte; byte j in bits 8j
+      return fp8_decoded((__ldcg(slot + td.off_coef + (rp >> 7)) >> ((rp >> 2) & 24u)) & 0xFFu,
+                         (__ldcg(slot + td.off_rankmap + (rp >> 2)) >> ((rp & 3u) << 3)) & 0xFFu);
   }
   if (kFull && td.vmode == kVmodeQsgd) {
     const float norm = __ldcg(reinterpret_cast<const float*>(slot + td.off_coef) + (rp >> 9));

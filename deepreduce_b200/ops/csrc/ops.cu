@@ -1,10 +1,11 @@
 // Stand-alone sm_90a kernels behind the GRACE-compatible per-tensor codec API
 // (deepreduce_b200/codecs/*): bloom insert / universe query+select, QSGD, scaled sign,
-// bit packing, Gram-polynomial fit/eval, delta+bp128 integer coding.
+// fp8 values, bit packing, Gram-polynomial fit/eval, delta+bp128 integer coding.
 // Each has a plain-torch oracle in the codec module; tests compare them.
 #include "common.cuh"
 #include "conflict_sets.cuh"
 #include "dexp_fit.cuh"
+#include "fp8_values.cuh"
 #include "ops.h"
 #include "sign_values.cuh"
 
@@ -163,6 +164,32 @@ __global__ void sign_decode_kernel(const uint32_t* __restrict__ bits, const floa
                                    float* __restrict__ out) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < K; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = sign_decoded((bits[i >> 5] >> (i & 31)) & 1u, scales[i / kSignBucket]);
+}
+
+// ---------------------------------------------------------------------------
+// fp8 values: one warp per 32-value block, four blocks (one scale word) per 128-thread CTA (the fused engine's fix
+// phase runs the same rule per task)
+// ---------------------------------------------------------------------------
+constexpr int kFp8Threads = 4 * kFp8Block;
+
+__global__ void __launch_bounds__(kFp8Threads) fp8_encode_kernel(const float* __restrict__ v, int64_t K,
+                                                                 uint32_t* __restrict__ scales,
+                                                                 uint32_t* __restrict__ elems) {
+  __shared__ uint32_t sw;
+  const int64_t p = (int64_t)blockIdx.x * kFp8Threads + threadIdx.x;
+  const float x = p < K ? v[p] : 0.f;
+  const uint32_t s = fp8_block_scale(x);                // blocks past the end: scale byte 0
+  const uint32_t word = fp8_elem_word(x, s);
+  if ((threadIdx.x & 31u) == 0) reinterpret_cast<uint8_t*>(&sw)[threadIdx.x >> 5] = (uint8_t)s;
+  __syncthreads();
+  if (threadIdx.x == 0) scales[blockIdx.x] = sw;
+  if ((threadIdx.x & 3u) == 0 && p < K) elems[p >> 2] = word;
+}
+
+__global__ void fp8_decode_kernel(const uint32_t* __restrict__ scales, const uint32_t* __restrict__ elems, int64_t K,
+                                  float* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < K; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = fp8_decoded((scales[i >> 7] >> ((i >> 2) & 24)) & 0xFFu, (elems[i >> 2] >> ((i & 3) << 3)) & 0xFFu);
 }
 
 // ---------------------------------------------------------------------------
@@ -465,6 +492,18 @@ void launch_sign_decode(const uint32_t* bits, const float* scales, int64_t K, fl
   if (K == 0) return;
   count_launch();
   sign_decode_kernel<<<grid_for(K, 256), 256, 0, st>>>(bits, scales, K, out);
+}
+
+void launch_fp8_encode(const float* v, int64_t K, uint32_t* scales, uint32_t* elems, cudaStream_t st) {
+  if (K == 0) return;
+  count_launch();
+  fp8_encode_kernel<<<(unsigned)((K + kFp8Threads - 1) / kFp8Threads), kFp8Threads, 0, st>>>(v, K, scales, elems);
+}
+
+void launch_fp8_decode(const uint32_t* scales, const uint32_t* elems, int64_t K, float* out, cudaStream_t st) {
+  if (K == 0) return;
+  count_launch();
+  fp8_decode_kernel<<<grid_for(K, 256), 256, 0, st>>>(scales, elems, K, out);
 }
 
 void launch_pack_bits(const int64_t* vals, int64_t n, int bits, uint32_t* out, int64_t n_words, cudaStream_t st) {

@@ -58,6 +58,8 @@ void launch_qsgd_decode(const void* lvl, bool i16, const float* norms, int64_t K
                         cudaStream_t st);
 void launch_sign_encode(const float* v, int64_t K, uint32_t* bits, float* scales, cudaStream_t st);
 void launch_sign_decode(const uint32_t* bits, const float* scales, int64_t K, float* out, cudaStream_t st);
+void launch_fp8_encode(const float* v, int64_t K, uint32_t* scales, uint32_t* elems, cudaStream_t st);
+void launch_fp8_decode(const uint32_t* scales, const uint32_t* elems, int64_t K, float* out, cudaStream_t st);
 void launch_pack_bits(const int64_t* vals, int64_t n, int bits, uint32_t* out, int64_t n_words, cudaStream_t st);
 void launch_unpack_bits(const uint32_t* in, int64_t n_words, int64_t n, int bits, int64_t* out, cudaStream_t st);
 void launch_polyfit_fit(const float* y, const int* seg_off, const int* seg_len, int n_seg, int degree, float* coeffs,

@@ -41,6 +41,9 @@ enum ValueMode : uint32_t {  // TensorDesc::vmode: how a tensor's values travel 
   kVmodeSign = 5,     // scaled sign (sign_values.cuh): per 512-value bucket b one fp32 scale mu_b at off_coef + b, then
                       // one bit per value at off_rankmap, LSB first (value p is bit p % 32 of word p / 32, 1 <=> v < 0);
                       // decodes to bit ? -mu_b : +mu_b.  off_vals / off_selidx are sender-local scratch (fix phase)
+  kVmodeFp8 = 6,      // E4M3 values (fp8_values.cuh), a scale byte per 32-value block: the scale bytes at off_coef, then
+                      // the element bytes at off_rankmap, each packed four per word (byte p in bits 8 (p % 4) of word
+                      // p / 4).  off_vals / off_selidx are sender-local scratch (fix phase)
 };
 
 // kPolicyP2 ('conflict_sets', opt-in): the sender draws the pick over its positives and ships it as a bitmask (p2.cu);

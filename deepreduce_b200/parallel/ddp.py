@@ -14,7 +14,8 @@ CUDA + 'index'/'both' + 'elias_fano'          -> fused engine, Elias-Fano index 
 CUDA + 'dexp' values + 'fused_dexp'           -> fused engine, double-exponential values (plain, bloom or rle index)
 CUDA + 'bf16' values                          -> fused engine, 16-bit values (plain, bloom or rle index, or 'randomk')
 CUDA + 'sign' values                          -> fused engine, 1-bit scaled-sign values (wherever bf16 values are)
-CUDA + 'randomk' [+ QSGD, bf16 or sign values] -> fused engine, values only on the wire (shared-seed index)
+CUDA + 'fp8' values                           -> fused engine, E4M3 values with a scale per 32 (wherever sign values are)
+CUDA + 'randomk' [+ QSGD, bf16, sign or fp8 values] -> fused engine, values only on the wire (shared-seed index)
 CUDA + 'none'/'allreduce'                     -> dense NCCL all-reduce of the flat bucket
 anything else (CPU/gloo, other codecs)        -> GRACE-compatible per-tensor path
 """
@@ -40,7 +41,8 @@ def _fused_supported(params: dict) -> bool:
     the reference's launch script (run_deepreduce.sh:35-107): top-k or threshold sparsifier x {no codec, index (bloom
     leftmost / random / p0, run-length), value (polyfit, QSGD int8/int16), both}, and bf16 values (``'value': 'bf16'``)
     over the plain, bloom or run-length index, with no opt-in key: no earlier dict names 'bf16'.  Scaled-sign values
-    (``'value': 'sign'``, 512-value buckets) take every route bf16 values take, with no opt-in key either.
+    (``'value': 'sign'``, 512-value buckets) and fp8 values (``'value': 'fp8'``, 32-value blocks) take every route bf16
+    values take, with no opt-in key either.
     Bloom policy 'conflict_sets' (P2) is fused only with top-k and ``'p2_pick_mask': True``: the sender then ships its pick as a
     bitmask over the positives, a different wire from the reference's, where every receiver redraws the pick.
     'both' with the run-length index is fused only with ``'fused_rle_values': True``: without the key that dict keeps
@@ -61,7 +63,7 @@ def _fused_supported(params: dict) -> bool:
     # P2 needs top-k: under 'threshold' K is the slot capacity, so the draw would keep every positive
     p2_ok = policy == 'conflict_sets' and params.get('p2_pick_mask') is True and params.get('compressor') == 'topk'
     pol_ok = policy in ('leftmost', 'random', 'p0') or p2_ok
-    value_ok = (params.get('value', 'polyfit') in ('polyfit', 'bf16', 'sign')
+    value_ok = (params.get('value', 'polyfit') in ('polyfit', 'bf16', 'sign', 'fp8')
                 or (params.get('value') == 'qsgd' and 1 <= int(params.get('quantum_num', 127)) <= 32767
                     and int(params.get('bucket_size', 512)) == 512))
     # the same index rule whether the index is shipped ('both') or not ('value'), as the config check has it
@@ -80,8 +82,8 @@ def _fused_supported(params: dict) -> bool:
         return pol_ok and (value_ok or dexp_ok)
     if dr == 'both' and params.get('index') == 'rle':
         # the bloom policies do not apply to a lossless index; the fused plan refuses 'conflict_sets' outside bloom
-        # bf16 and sign values need no key, and 'fused_rle_values' keeps its meaning: it refuses them
-        rv, keyless = params.get('fused_rle_values') is True, params.get('value') in ('bf16', 'sign')
+        # bf16, sign and fp8 values need no key, and 'fused_rle_values' keeps its meaning: it refuses them
+        rv, keyless = params.get('fused_rle_values') is True, params.get('value') in ('bf16', 'sign', 'fp8')
         return ((rv and value_ok and not keyless) or dexp_ok or (keyless and not rv)) and policy != 'conflict_sets'
     if dr == 'both' and params.get('index') == 'elias_fano':
         # every value codec the run-length index fuses, with no opt-in key: no earlier dict names this index
@@ -93,13 +95,14 @@ def _fused_randomk_supported(params: dict) -> bool:
     """Which 'randomk' ``params`` dicts the fused engine serves in its shared-index mode (``kModeShared``): every rank
     draws the same index set from (step, tensor), so only values travel and the allgather and allreduce communicators
     give the same aggregate.  With no codec, with QSGD values (``'deepreduce': 'value', 'value': 'qsgd'``, bucket
-    512), with bf16 values (``'value': 'bf16'``) or with scaled-sign values (``'value': 'sign'``).  Not fused:
+    512), with bf16 values (``'value': 'bf16'``), with scaled-sign values (``'value': 'sign'``) or with fp8 values
+    (``'value': 'fp8'``).  Not fused:
     'randomk' with an index codec, 'both', or polyfit values."""
     if params.get('compressor') != 'randomk' or params.get('communicator', 'allgather') not in ('allgather', 'allreduce'):
         return False
     dr = params.get('deepreduce', None)
     v = params.get('value', 'polyfit')
-    return dr is None or (dr == 'value' and (v in ('bf16', 'sign')
+    return dr is None or (dr == 'value' and (v in ('bf16', 'sign', 'fp8')
                                              or (v == 'qsgd' and 1 <= int(params.get('quantum_num', 127)) <= 32767
                                                  and int(params.get('bucket_size', 512)) == 512)))
 

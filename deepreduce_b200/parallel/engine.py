@@ -35,13 +35,14 @@ import torch.distributed as dist
 from .. import spec
 from ..codecs.bf16 import bf16_bits_oracle, bf16_widen_oracle
 from ..codecs.bloom import bloom_insert_oracle, bloom_query_oracle, conflict_sets_oracle
+from ..codecs.fp8 import fp8_decode_oracle, fp8_encode_oracle
 from ..codecs.polyfit import get_segments, polyfit_eval_oracle, polyfit_fit_oracle
 from ..codecs.qsgd import qsgd_decode_oracle, qsgd_encode_oracle
 from ..codecs.sign import sign_decode_oracle, sign_encode_oracle
 from ..grace.memory import clip_factor, is_dense, pairwise_sumsq
 from .plan import update_cta_speeds
 from .plan import (DYN_WORDS, HIST_BINS, MODE_BLOOM, MODE_EF, MODE_RLE, MODE_SHARED, NUM_HIST, POLICY_ID, SLOT_HEADER_WORDS,
-                   VMODE_BF16, VMODE_DEXP, VMODE_QSGD, VMODE_SIGN, BucketPlan, rle_stream_words)
+                   VMODE_BF16, VMODE_DEXP, VMODE_FP8, VMODE_QSGD, VMODE_SIGN, BucketPlan, rle_stream_words)
 
 (PH_ACCUM, PH_FALLBACK, PH_HIST2, PH_INSERT, PH_QUERY, PH_EMIT, PH_RANK_HIST, PH_RANK_SCAN, PH_RANK_SCATTER,
  PH_RANK_EXACT, PH_FIT, PH_FIX, PH_PUSH, PH_SIGNAL, PH_EXPAND, PH_DECODE, PH_COMPACT, PH_PUSH2, PH_SIGNAL2,
@@ -402,6 +403,15 @@ def encode_tensor_oracle(tp, acc: torch.Tensor, slot: np.ndarray, t_index: int, 
         dec = sign_decode_oracle(bits, scales, n)
         resid[sel] = torch.where(torch.isfinite(dec), vals - dec, torch.zeros_like(dec))
         vals = dec
+    elif tp.vmode == VMODE_FP8:
+        # E4M3 values with a scale byte per 32-value block; the residual keeps v - d where d is finite, and is 0 where
+        # it is not (an inf or a NaN in the block)
+        scales, elems = fp8_encode_oracle(vals)
+        slot[tp.off_coef:tp.off_coef + scales.numel()] = scales.numpy().view(np.uint32)
+        slot[tp.off_rankmap:tp.off_rankmap + elems.numel()] = elems.numpy().view(np.uint32)
+        dec = fp8_decode_oracle(scales, elems, n)
+        resid[sel] = torch.where(torch.isfinite(dec), vals - dec, torch.zeros_like(dec))
+        vals = dec
     elif tp.vmode == VMODE_BF16:
         # bf16 values (round to nearest even, NaN -> 0x7FC0), two per word; the residual keeps the exact rounding error
         # where the widened value is finite, and is 0 (as for fp32 values) where it is not
@@ -547,6 +557,10 @@ def decode_slot_oracle(plan: BucketPlan, slot, *, seed=spec.DEFAULT_SEED) -> tor
             scales = torch.from_numpy(a[t.off_coef:t.off_coef + (n + 511) // 512].view(np.float32).copy())
             bits = torch.from_numpy(a[t.off_rankmap:t.off_rankmap + (n + 31) // 32].view(np.int32).copy())
             vals = sign_decode_oracle(bits, scales, n)
+        elif t.vmode == VMODE_FP8:
+            scales = torch.from_numpy(a[t.off_coef:t.off_coef + (n + 127) // 128].view(np.int32).copy())
+            elems = torch.from_numpy(a[t.off_rankmap:t.off_rankmap + (n + 3) // 4].view(np.int32).copy())
+            vals = fp8_decode_oracle(scales, elems, n)
         elif t.vmode == VMODE_BF16:
             bits = a[t.off_vals:t.off_vals + (n + 1) // 2].view(np.uint16)[:n].astype(np.int64)
             vals = bf16_widen_oracle(torch.from_numpy(bits))

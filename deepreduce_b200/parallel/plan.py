@@ -20,7 +20,8 @@ from .. import spec
 from ..codecs.dexp import MIN_NUMEL as DEXP_MIN_NUMEL
 
 MODE_RAW, MODE_BLOOM, MODE_RLE, MODE_SHARED, MODE_EF = 0, 1, 2, 3, 4
-VMODE_FP32, VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_BF16, VMODE_SIGN = 0, 1, 2, 3, 4, 5   # TensorDesc.vmode (plan.h ValueMode)
+# TensorDesc.vmode (plan.h ValueMode)
+VMODE_FP32, VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_BF16, VMODE_SIGN, VMODE_FP8 = 0, 1, 2, 3, 4, 5, 6
 KEY_SPAN = 1 << 31                    # select keys are 31-bit
 POLICY_ID = {"leftmost": 0, "random": 1, "p0": 2, "conflict_sets": 3}
 P2_MAX_POS_CAP = 1 << 20              # P2: the draw keeps one chosen bit per positive in shared memory (128 KB)
@@ -177,8 +178,9 @@ class TensorPlan:
 
     @property
     def coded(self) -> bool:
-        """A fix phase writes the residual (polyfit, QSGD, dexp, sign); emit knows the other modes' decoded values."""
-        return self.vmode in (VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_SIGN)
+        """A fix phase writes the residual (polyfit, QSGD, dexp, sign, fp8); emit knows the other modes' decoded
+        values."""
+        return self.vmode in (VMODE_POLYFIT, VMODE_QSGD, VMODE_DEXP, VMODE_SIGN, VMODE_FP8)
 
     @property
     def coef_words(self) -> int:
@@ -194,6 +196,8 @@ class TensorPlan:
             return 4 * ((self.val_cap + 511) // 512) + self.val_cap * (2 if self.rank_u32 else 1)
         if self.vmode == VMODE_SIGN:
             return 4 * ((self.val_cap + 511) // 512) + 4 * ((self.val_cap + 31) // 32)
+        if self.vmode == VMODE_FP8:
+            return (self.val_cap + 31) // 32 + self.val_cap
         return (2 if self.vmode == VMODE_BF16 else 4) * self.val_cap
 
     @property
@@ -224,8 +228,8 @@ class BucketPlan:
     max_hash: int = 16
     ks: Optional[Sequence[int]] = None    # explicit per-tensor K (overrides compress_ratio)
     hint: bool = True                     # ship the 1-bit-per-32-elements occupancy hint next to each bloom filter
-    value: Optional[str] = None           # None (fp32 values), 'polyfit', 'qsgd', 'dexp', 'bf16' or 'sign' ('both': an
-                                          # index codec + value codec)
+    value: Optional[str] = None           # None (fp32 values), 'polyfit', 'qsgd', 'dexp', 'bf16', 'sign' or 'fp8'
+                                          # ('both': an index codec + value codec)
     quantum_num: int = 127                # QSGD levels (int8 on the wire)
     poly_degree: int = 5
     poly_min_k: int = 512                 # tensors shipping fewer values keep them as fp32 (the fit header would be larger)
@@ -241,8 +245,8 @@ class BucketPlan:
     def __post_init__(self):
         if self.index not in (None, "bloom", "rle", "elias_fano"):
             raise ValueError(f"fused engine index codecs: None, 'bloom', 'rle', 'elias_fano'; got {self.index!r}")
-        if self.value not in (None, "polyfit", "qsgd", "dexp", "bf16", "sign"):
-            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp', 'bf16', 'sign'; "
+        if self.value not in (None, "polyfit", "qsgd", "dexp", "bf16", "sign", "fp8"):
+            raise ValueError(f"fused engine value codecs: None, 'polyfit', 'qsgd', 'dexp', 'bf16', 'sign', 'fp8'; "
                              f"got {self.value!r}")
         if self.sparsifier not in ("topk", "threshold", "randomk"):
             raise ValueError(f"fused engine sparsifiers: 'topk', 'threshold', 'randomk'; got {self.sparsifier!r}")
@@ -251,7 +255,8 @@ class BucketPlan:
             raise ValueError("'randomk' ships no index (every rank draws the same set): pass index=None")
         if shared and self.value in ("polyfit", "dexp"):
             # rank_bin centres the value bins on the selection threshold, which here is a hash, not a magnitude
-            raise NotImplementedError(f"'randomk' is fused with fp32, QSGD, bf16 or sign values, not with {self.value!r}")
+            raise NotImplementedError(f"'randomk' is fused with fp32, QSGD, bf16, sign or fp8 values, not with "
+                                      f"{self.value!r}")
         if self.value == "qsgd" and not (1 <= int(self.quantum_num) <= 32767):
             raise ValueError("quantum_num must be in [1, 32767]")
         fixed_thr = 0
@@ -402,6 +407,15 @@ class BucketPlan:
             word = _align(word + (tp.val_cap + 511) // 512, 4)
             tp.off_rankmap = word                        # sign bits, LSB first
             word = _align(word + (tp.val_cap + 31) // 32, 4)
+            scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap)]
+        elif self.value == "fp8":
+            # E4M3 values (codecs/fp8.py), a scale byte per 32-value block: the scale bytes, then the element bytes,
+            # each four per word; the fix phase codes them from the fp32 values in sender-local scratch, as sign's does
+            tp.vmode = VMODE_FP8
+            tp.off_coef = word                           # scale bytes
+            word = _align(word + (tp.val_cap + 127) // 128, 4)
+            tp.off_rankmap = word                        # element bytes
+            word = _align(word + (tp.val_cap + 3) // 4, 4)
             scratch += [(tp, "off_vals", tp.val_cap), (tp, "off_selidx", tp.val_cap)]
         else:
             # fp32 values, or bf16 values two per word (the p-th value in the low half of word p // 2): emit rounds them

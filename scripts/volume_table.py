@@ -70,6 +70,8 @@ def main():
                                                  'index': 'elias_fano'}, None),
                            ("Elias-Fano index + sign values", {**base, 'compress_ratio': 0.01, 'deepreduce': 'both',
                                                                'index': 'elias_fano', 'value': 'sign'}, None),
+                           ("Elias-Fano index + fp8 values", {**base, 'compress_ratio': 0.01, 'deepreduce': 'both',
+                                                              'index': 'elias_fano', 'value': 'fp8'}, None),
                            ("delta + bp128 index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'integer'}, None),
                            ("Huffman index", {**base, 'compress_ratio': 0.01, 'deepreduce': 'index', 'index': 'huffman'}, None)):
         ours = top if cfg is None else model_volume(m, cfg)
