@@ -16,8 +16,13 @@ the two gradients separately and the kernels add them as they load them, instead
 elementwise add that the backward passes then read again.
 
 Every fused result is bitwise that of the unfused graph: same reductions, same fp32 expressions, same bf16 rounding
-points.  ``eligible()`` decides per call; anything it rejects (CPU, eval mode, fp32, another memory layout) runs the
-unfused modules unchanged.  ``DR_FUSED_BN=0`` selects the unfused graph everywhere, for A/B comparisons.
+points.  ``eligible()`` decides per call.  It accepts a channels_last bf16 CUDA input with C % 8 == 0, C <= 2048
+(``kBnMaxChannels`` of ``ops/csrc/ops.h``: the row-walking kernels hold one row's C / 8 threads in a 256-thread CTA),
+fewer than 2^31 - 1 elements and more than one row, paired with a training, affine BatchNorm with eps > 0 that tracks
+running stats, and whose weight, bias, running_mean and running_var are fp32 on the input's device.  Anything it
+rejects (CPU, eval mode, fp32 or NCHW input, more channels, a bf16 BatchNorm, eps <= 0) runs the unfused modules
+unchanged.  ``DR_FUSED_BN=0`` selects the
+unfused graph everywhere, for A/B comparisons.
 """
 from __future__ import annotations
 
@@ -35,17 +40,20 @@ def enabled() -> bool:
 def _eligible_x(x: torch.Tensor) -> bool:
     # the layout the native training path runs its channels-last kernels on (and that the fused kernels assume)
     return (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.stride(1) == 1
-            and x.is_contiguous(memory_format=torch.channels_last) and x.size(1) % 8 == 0 and x.size(1) <= 8192
+            and x.is_contiguous(memory_format=torch.channels_last) and x.size(1) % 8 == 0 and x.size(1) <= 2048
             and x.numel() < 2 ** 31 - 1 and x.numel() // x.size(1) > 1)
 
 
-def _eligible_bn(bn: nn.BatchNorm2d) -> bool:
+def _eligible_bn(bn: nn.BatchNorm2d, device: torch.device) -> bool:
+    # the kernels read fp32 per-channel parameters and statistics (binding.cpp: check_chan); F.batch_norm refuses
+    # eps <= 0, so such a module runs unfused and raises there
     return (bn.training and bn.track_running_stats and bn.running_mean is not None and bn.momentum is not None
-            and bn.affine)
+            and bn.affine and bn.eps > 0 and all(t.dtype == torch.float32 and t.device == device
+                                  for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var)))
 
 
 def eligible(x: torch.Tensor, bn: nn.BatchNorm2d) -> bool:
-    return enabled() and _eligible_x(x) and _eligible_bn(bn)
+    return enabled() and _eligible_x(x) and _eligible_bn(bn, x.device)
 
 
 def _stats(x, bn):

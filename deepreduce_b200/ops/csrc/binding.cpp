@@ -404,7 +404,8 @@ static void check_bn_input(const torch::Tensor& x) {
   TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kBFloat16 && x.dim() == 4 && x.stride(1) == 1 &&
                   x.is_contiguous(at::MemoryFormat::ChannelsLast),
               "bn: x must be a channels_last bf16 CUDA tensor");
-  TORCH_CHECK(x.size(1) % 8 == 0 && x.size(1) <= 8192, "bn: channels must be a multiple of 8, at most 8192");
+  TORCH_CHECK(x.size(1) % 8 == 0 && x.size(1) <= dr::kBnMaxChannels, "bn: channels must be a multiple of 8, at most ",
+              dr::kBnMaxChannels);
   TORCH_CHECK(x.numel() < std::numeric_limits<int32_t>::max(), "bn: tensor too large for 32-bit indexing");
 }
 
@@ -905,6 +906,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("padding") = 1, py::arg("dilation") = 1, py::arg("ceil_mode") = false);
   m.def("bn_backward", &bn_backward, py::arg("mode"), py::arg("go"), py::arg("mask"), py::arg("x"), py::arg("p"),
         py::arg("z") = py::none(), py::arg("pz") = std::vector<torch::Tensor>{}, py::arg("go2") = py::none());
+  m.def("bn_row_tree", [](int64_t rows, int64_t C) { int by = 0, gy = 0; dr::bn_row_tree(rows, (int)C, &by, &gy);
+                                                     return std::make_pair(by, gy); });
   m.def("rle_runs", &rle_runs);
   m.def("rle_indices", &rle_indices);
   m.def("arena_alloc", &arena_alloc);

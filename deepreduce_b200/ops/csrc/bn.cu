@@ -772,6 +772,9 @@ __global__ void bn_update_stats_kernel(const float* __restrict__ mean, float* __
 }
 
 // Grid of a row-walking pass (apply, backward elementwise): every row once, at most as many CTAs as fit on the device.
+// A CTA holds one row's C / 8 threads at least, and the four row-walking kernels are __launch_bounds__(kApplyThreads),
+// so C is capped at kBnMaxChannels (binding.cpp's check_bn_input, fused_bn._eligible_x).
+static_assert(kBnMaxChannels / kVec <= kApplyThreads, "a row of kBnMaxChannels channels exceeds one apply CTA");
 template <typename K>
 cudaError_t rows_grid(K kernel, int64_t rows, int C, int& grid, int& threads) {
   const int groups = C / kVec;

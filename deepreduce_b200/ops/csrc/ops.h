@@ -96,7 +96,10 @@ int arena_enable_peer_access(const int* devices, int n);   // peers = the listed
 void launch_u8_to_nhwc_norm(const uint8_t* in, void* out_bf16, int64_t n_pix, const float* mean, const float* inv_std,
                             cudaStream_t st);
 
-// bn.cu — training BatchNorm (+ ReLU, + residual add) on NHWC bf16, C % 8 == 0; per-channel fp32 parameters
+// bn.cu — training BatchNorm (+ ReLU, + residual add) on NHWC bf16, C % 8 == 0, C <= kBnMaxChannels; per-channel fp32
+// parameters.  The row-walking passes (apply, pool, pool gradient, backward elementwise) run one thread per 8 channels
+// of a row in a CTA of at most 256 threads, so 2048 channels is the most they cover.
+constexpr int kBnMaxChannels = 2048;
 struct BnParams { const float* mean; const float* invstd; const float* weight; const float* bias; };
 // The (block_y, grid_y) of torch's channels-last reduction tree for rows x C (flexible_launch_configs, coop = true);
 // bn_stats and bn_backward reproduce it, and need block_y * grid_y <= rows.
