@@ -34,7 +34,7 @@ KNOWN_KEYS = frozenset({
     "beta", "gamma", "seed", "code", "hint", "min_numel", "dense_tensor", "hash_table", "split_numel", "pack_mapping",
     "qsgd_seed", "gzip_level", "dexp_min_numel", "overlap_grid", "capacity_ratio", "calibrate_partition",
     "p2_pick_mask", "fused_rle_values", "fused_dexp", "momentum", "gradient_clipping", "weight_decay",
-    "clip_norm", "warmup_ratios", "warmup_steps",
+    "clip_norm", "warmup_ratios", "warmup_steps", "nesterov", "weight_decay_exclude",
     # TF-side (tensorflow/deepreduce.py:34-36,57-59,282,307-343,361-369,458-490)
     "use_memory", "horovod_size", "bloom_fpr", "bloom_on", "threshold_val", "bloom_false_positives_aware",
     "bloom_policy", "bloom_logs_path", "gradient_id", "bloom_verbosity_frequency", "bloom_verbosity", "mem_mode",
@@ -120,6 +120,27 @@ class DeepReduceConfig:
             if (isinstance(wd, bool) or not isinstance(wd, (int, float)) or not math.isfinite(float(wd))
                     or float(wd) < 0.0):
                 raise ConfigError(f"'weight_decay' must be a finite number >= 0 (got {wd!r})")
+        # ... except on the parameters whose names match a pattern: the param group with weight_decay=0 that recipes
+        # give BatchNorm weights and biases
+        if "weight_decay_exclude" in params:
+            pats = params["weight_decay_exclude"]
+            if cfg.memory != "dgc":
+                raise ConfigError(f"'weight_decay_exclude' applies to 'memory': 'dgc' (got memory={cfg.memory!r})")
+            if not isinstance(pats, (list, tuple)) or not all(isinstance(p, str) for p in pats):
+                raise ConfigError(f"'weight_decay_exclude' must be a list of fnmatch patterns (strings) over parameter "
+                                  f"names (got {pats!r})")
+            if not float(params.get("weight_decay", 0.0)) > 0.0:
+                raise ConfigError("'weight_decay_exclude' excludes parameters from 'weight_decay': it needs "
+                                  "'weight_decay' > 0")
+        # ... and Nesterov momentum, as torch's SGD(nesterov=True) takes it
+        if "nesterov" in params:
+            nv = params["nesterov"]
+            if cfg.memory != "dgc":
+                raise ConfigError(f"'nesterov' applies to 'memory': 'dgc' (got memory={cfg.memory!r})")
+            if not isinstance(nv, bool):
+                raise ConfigError(f"'nesterov' must be True or False (got {nv!r})")
+            if nv and float(params.get("momentum", 0.9)) == 0.0:
+                raise ConfigError("'nesterov': True needs a momentum > 0 (got 'momentum': 0)")
         # ... and DGC's local gradient clipping: each tensor's gradient is scaled down to norm c / sqrt(W) before it
         # enters the momentum, inside the memory, because no user code runs between backward and the exchange
         if "clip_norm" in params:

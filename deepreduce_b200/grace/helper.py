@@ -62,7 +62,9 @@ def grace_from_params(params: dict):
     elif mem == 'dgc':
         import torch.distributed as dist
         memory = DgcMemory(params.get('momentum', 0.9), params.get('weight_decay', 0.0), params.get('clip_norm'),
-                           dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1)
+                           dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1,
+                           nesterov=params.get('nesterov', False),
+                           weight_decay_exclude=params.get('weight_decay_exclude', ()))
     elif mem in ('none', None):
         memory = NoneMemory()
     else:

@@ -12,6 +12,7 @@ decoded contribution is non-zero.
 """
 from __future__ import annotations
 
+import fnmatch
 import math
 
 import torch
@@ -44,6 +45,21 @@ def pairwise_sumsq(flat: torch.Tensor) -> float:
     while x.numel() > 1:
         x = x[0::2] + x[1::2]
     return float(x.item())
+
+
+def decay_excluded(name: str, patterns) -> bool:
+    """True if the parameter name matches one of the ``fnmatch`` patterns of ``'weight_decay_exclude'`` (matched case
+    sensitively on every platform)."""
+    return any(fnmatch.fnmatchcase(name, p) for p in patterns or ())
+
+
+def check_exclude_patterns(patterns, names) -> None:
+    """Raise ``ValueError`` naming every pattern of ``'weight_decay_exclude'`` that matches none of ``names``: a typo
+    must not silently keep the decay."""
+    names = list(names)
+    dead = [p for p in patterns or () if not any(fnmatch.fnmatchcase(n, p) for n in names)]
+    if dead:
+        raise ValueError(f"'weight_decay_exclude': pattern(s) {dead} match none of the model's parameters")
 
 
 def clip_factor(sumsq: float, thr: float):
@@ -112,11 +128,24 @@ class DgcMemory(Memory):
     ``clip_norm = c``: DGC's local gradient clipping, ahead of the weight decay.  Each tensor's g is replaced by
     ``fl32(g * fl32(thr / nrm))`` where its norm ``nrm`` (fp64, ``pairwise_sumsq`` over g in storage order, the order
     it has in a flat gradient bucket) is finite and > ``thr = c / sqrt(world_size)``.  Per tensor: the chunks of a
-    split parameter are one tensor here anyway.  With no ``clip_norm`` nothing is computed."""
+    split parameter are one tensor here anyway.  With no ``clip_norm`` nothing is computed.
 
-    def __init__(self, momentum: float = 0.9, weight_decay: float = 0.0, clip_norm=None, world_size: int = 1):
+    ``weight_decay_exclude``: ``fnmatch`` patterns; a tensor whose name matches one gets no weight decay (its parameter
+    is not read, so it need not be bound), as a param group with ``weight_decay=0`` would in torch's SGD.
+
+    ``nesterov=True``: Nesterov momentum.  The residual adds ``v = fl(d + fl(m * u))`` with the new u instead of u
+    (d: g after clipping and decay); u itself is torch's ``momentum_buffer``.  Torch's CPU step rounds ``d + m * u``
+    once (a fused multiply-add); here it is two roundings, as every other op of this memory.  A tensor's first step
+    starts from ``u = d``, so its residual starts from ``fl(d + fl(m * d))``."""
+
+    def __init__(self, momentum: float = 0.9, weight_decay: float = 0.0, clip_norm=None, world_size: int = 1,
+                 nesterov: bool = False, weight_decay_exclude=()):
         self.momentum = float(momentum)
         self.weight_decay = float(weight_decay)
+        self.nesterov = bool(nesterov)
+        if self.nesterov and self.momentum == 0.0:
+            raise ValueError("Nesterov momentum needs a momentum > 0")
+        self.weight_decay_exclude = tuple(weight_decay_exclude or ())
         self.clip_norm = None if clip_norm is None else float(clip_norm)
         self.world_size = int(world_size)
         self.clip_thr = None if clip_norm is None else self.clip_norm / math.sqrt(self.world_size)
@@ -164,13 +193,12 @@ class DgcMemory(Memory):
     def compensate(self, tensor, name):
         if self.clip_thr is not None:
             tensor = self._clip(tensor)
-        if self.weight_decay != 0.0:
+        if self.weight_decay != 0.0 and not decay_excluded(name, self.weight_decay_exclude):
             tensor = tensor + (self.weight_decay * self._weights(name, tensor.shape, tensor.dtype))
-        if name in self.momenta:
-            u = self.momentum * self.momenta[name] + tensor
-            tensor = self.residuals[name] + u
-        else:
-            u = tensor
+        d = tensor
+        u = self.momentum * self.momenta[name] + d if name in self.momenta else d
+        v = d + (self.momentum * u) if self.nesterov else u
+        tensor = self.residuals[name] + v if name in self.momenta else v
         self.momenta[name] = u
         return tensor
 

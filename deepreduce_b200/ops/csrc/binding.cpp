@@ -683,17 +683,21 @@ struct Engine {
     P.grad = reinterpret_cast<float*>(grad); P.resid = reinterpret_cast<float*>(resid);
   }
 
-  // 'dgc' memory: the fp32 momentum buffer (same element layout as the residual) and the momentum factor; 0 = none
-  // (the residual memory's kernels)
-  void set_momentum(int64_t mom, double momentum) {
-    P.mom = reinterpret_cast<float*>(mom); P.momentum = (float)momentum;
+  // 'dgc' memory: the fp32 momentum buffer (same element layout as the residual), the momentum factor and Nesterov
+  // momentum on or off; mom = 0: none (the residual memory's kernels)
+  void set_momentum(int64_t mom, double momentum, bool nesterov) {
+    TORCH_CHECK(!nesterov || (mom != 0 && momentum > 0.0), "set_momentum: Nesterov momentum needs a momentum > 0");
+    P.mom = reinterpret_cast<float*>(mom); P.momentum = (float)momentum; P.nesterov = nesterov ? 1 : 0;
   }
 
-  // 'dgc' weight decay: the device table of parameter addresses, one per plan tensor (EngineParams::wparams), and the
-  // factor; 0 = none (nothing is read)
-  void set_weight_decay(int64_t table, double weight_decay) {
-    TORCH_CHECK(weight_decay == 0.0 || table != 0, "set_weight_decay: weight decay needs the parameter table");
+  // 'dgc' weight decay: the device table of parameter addresses, one per plan tensor (EngineParams::wparams), the
+  // factor (0: none, nothing is read) and the device table of uint8 flags, one per plan tensor, 1 where the tensor takes
+  // the decay (EngineParams::decayed)
+  void set_weight_decay(int64_t table, double weight_decay, int64_t decayed) {
+    TORCH_CHECK(weight_decay == 0.0 || (table != 0 && decayed != 0),
+                "set_weight_decay: weight decay needs the parameter table and the per-tensor flags");
     P.wparams = reinterpret_cast<const unsigned long long*>(table); P.weight_decay = (float)weight_decay;
+    P.decayed = reinterpret_cast<const uint8_t*>(decayed);
   }
 
   // 'dgc' local gradient clipping: the scratch of the per-tile sums (fp64, one per tile) and of the factors (fp32, one

@@ -524,9 +524,11 @@ DR_D void clip_factors(const EngineParams& P) {
 //               before it waits for the ring so that the load overlaps the wait, and writes u back the same way.  u
 //               is not staged through the ring: the stage size, the ring depth and the shared-memory budget stay
 //               the same as the existing variants', so u costs no ring space and no extra TMA bookkeeping, and each
-//               element of u is read by exactly the thread that uses it.  With weight decay (P.weight_decay != 0,
-//               CTA-uniform) the thread reads its four elements of the parameter w the same way, next to u, and adds
-//               fl(weight_decay * w) to g before the momentum; with weight_decay == 0 nothing is read or added.
+//               element of u is read by exactly the thread that uses it.  With weight decay (P.weight_decay != 0 and
+//               the tensor's P.decayed[t], read once per tensor run, CTA-uniform) the thread reads its four elements of
+//               the parameter w the same way, next to u, and adds fl(weight_decay * w) to g before the momentum;
+//               otherwise (no decay, or an excluded parameter) nothing is read or added.  With P.nesterov
+//               (CTA-uniform) the residual adds fl(d + fl(momentum * u)) with the new u instead of u.
 // kClip = true : 'dgc' local gradient clipping.  clip_tile_sums and clip_factors have run (two grid barriers ago), and
 //               g = fl(g * f) with the tensor's factor f ahead of everything else, where f != 1.
 template <bool kTma, bool kFull, bool kB, bool kDgc, bool kClip = false>
@@ -643,6 +645,8 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
     const uint32_t guess = (do_hist && !single) ? __ldcg(&P.sel[cur].bin1) : 0xFFFFFFFFu;
     float clip_f = 1.0f;
     if constexpr (kClip) clip_f = __ldcg(P.clip_f + cur);                 // written by another CTA in this launch
+    bool dec = false;                                                      // CTA-uniform: this tensor takes the decay
+    if constexpr (kDgc) dec = P.weight_decay != 0.0f && __ldg(P.decayed + cur) != 0;
     uint32_t n_mine = 0;
     uint32_t keys[8];
     while (true) {                                                         // tiles of this tensor inside my range
@@ -661,7 +665,7 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
             const uint32_t e0 = off + tid * 4u;
             if (e0 < ti.n) {
               u_old = __ldcs(reinterpret_cast<const float4*>(P.mom + ti.base + e0));
-              if (P.weight_decay != 0.0f) {
+              if (dec) {
                 if constexpr (kB) w_bf16 = load_weights_bf16(P, cur, ti.local0 + e0, ti.n - e0);
                 else w = load_weights(P, cur, ti.local0 + e0, ti.n - e0);
               }
@@ -701,7 +705,7 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
                   g.z = __fmul_rn(g.z, clip_f); g.w = __fmul_rn(g.w, clip_f);
                 }
               }
-              if (wd != 0.0f) {                                            // d = fl(g + fl(wd * w)) replaces g
+              if (dec) {                                                   // d = fl(g + fl(wd * w)) replaces g
                 if constexpr (kB) w = widen_bf16x4(w_bf16);
                 g.x = __fadd_rn(g.x, __fmul_rn(wd, w.x)); g.y = __fadd_rn(g.y, __fmul_rn(wd, w.y));
                 g.z = __fadd_rn(g.z, __fmul_rn(wd, w.z)); g.w = __fadd_rn(g.w, __fmul_rn(wd, w.w));
@@ -710,6 +714,10 @@ DR_D void phase_accum(const EngineParams& P, Smem& sm) {
               u.x = __fadd_rn(__fmul_rn(mu, u_old.x), g.x); u.y = __fadd_rn(__fmul_rn(mu, u_old.y), g.y);
               u.z = __fadd_rn(__fmul_rn(mu, u_old.z), g.z); u.w = __fadd_rn(__fmul_rn(mu, u_old.w), g.w);
               __stcs(reinterpret_cast<float4*>(P.mom + ti.base + e0), u);
+              if (P.nesterov) {                                            // v = fl(d + fl(mu * u)) replaces u
+                u.x = __fadd_rn(g.x, __fmul_rn(mu, u.x)); u.y = __fadd_rn(g.y, __fmul_rn(mu, u.y));
+                u.z = __fadd_rn(g.z, __fmul_rn(mu, u.z)); u.w = __fadd_rn(g.w, __fmul_rn(mu, u.w));
+              }
               const float4 r = sr[tid];
               a.x = __fadd_rn(r.x, u.x); a.y = __fadd_rn(r.y, u.y); a.z = __fadd_rn(r.z, u.z); a.w = __fadd_rn(r.w, u.w);
             } else if (has_resid) {

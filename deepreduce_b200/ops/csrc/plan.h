@@ -139,7 +139,7 @@ constexpr uint32_t kArenaHdrWords = 128;
 // and the same 22-bit rule applies to it: a superset of the K smallest hashes, plus ~numel / 2^22 elements sharing the
 // threshold's prefix.  The set depends on (numel, K, epoch, salt) only, so every rank computes the same one.
 enum Phase : int {
-  kPhAccum = 0,      // r = beta*r + gamma*g (dgc: [g = f*g,] u = m*u + g [+ wd*w], r = r + u) ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
+  kPhAccum = 0,      // r = beta*r + gamma*g (dgc: [g = f*g,] d = g [+ wd*w], u = m*u + d, r = r + (nesterov ? d + m*u : u)) ; dense grad <- 0 ; zero slot ; candidate lists (keys >= history bound) ; hist digit 1
   kPhFallback = 1,   // (only if some bound was unsafe) digit 1 redone without the bound, candidate lists rebuilt in full
   kPhHist2 = 2,      // digit 2 of the candidate keys in the threshold bin
   kPhInsert = 3,     // selected candidates -> bloom filter + occupancy hint (bloom) / positive masks (raw, rle)
@@ -254,11 +254,18 @@ struct EngineParams {
   float momentum;
   int has_bf16_values;           // some tensor ships bf16 values (kVmodeBf16: only the <.., true> kernels carry that path)
   // 'dgc' weight decay (weight_decay != 0, the dgc kernels only): the accumulate phase adds weight_decay * w to the
-  // gradient ahead of the momentum, d = fl(g + fl(weight_decay * w)), with w read from the parameter itself.
+  // gradient of every plan tensor t with decayed[t] != 0 ahead of the momentum, d = fl(g + fl(weight_decay * w)), with w
+  // read from the parameter itself.  A tensor with decayed[t] == 0 (a parameter excluded from the decay) reads no w and
+  // adds nothing.  The factor stays one scalar (the constant bank, no register across the tile loop); per tensor only
+  // the on/off flag is read, once per tensor run.
   // wparams[t]: address of plan tensor t's first element in its parameter's storage (the bucket's dtype; a chunk of a
   // split parameter points at its offset).  Only the tensor's numel elements are read: the padding takes w = 0.
+  // These fields and the ones below are read by the dgc kernels only.
   const unsigned long long* wparams;  // [n_tensors]
   float weight_decay;
+  const uint8_t* decayed;             // [n_tensors] 1: the tensor takes the decay, 0: excluded (a chunk: its parameter's)
+  // 'dgc' Nesterov momentum (nesterov != 0): the residual adds v = fl(d + fl(momentum * u)) with the new u, not u
+  int nesterov;
   // 'dgc' local gradient clipping (clip_part != nullptr, the <.., true, .., true, true> kernels): the accumulate phase
   // first sums the squares of every parameter's gradient in fp64 by adjacent pairs (per tile into clip_part, then over
   // the parameter's tiles), and where nrm = sqrt(sum) is finite and > clip_thr it multiplies the gradient by

@@ -24,6 +24,8 @@ runs with ``weight_decay=0``.  The parameters are read in the order of their gra
 storage order, which DDP gives a dense parameter's gradient; their layouts must not change after DDP built its buckets.
 ``'clip_norm'`` clips each parameter's gradient inside the memory, in both routes, because the hook runs inside backward
 and no user code can clip in between; the norm is per parameter, summed in the gradient's order in the bucket.
+``'nesterov'`` and ``'weight_decay_exclude'`` apply in both routes too; the patterns match the module's parameter
+names, the names the checkpoint is keyed by, and a pattern that matches none of them raises.
 """
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -33,6 +35,7 @@ import torch.nn as nn
 
 from .ddp import (BUCKET_DTYPES, engine_split_numel, fused_path, grace_state_dict, load_grace_state_dict, make_engine,
                   make_grc, stage_plans)
+from ..grace.memory import check_exclude_patterns
 from .engine import BucketEngine, StatusPoller, total_stats
 from .plan import BucketPlan, split_large
 
@@ -127,6 +130,10 @@ class DeepReduceHookState:
         from ..config import warmup_from_params
         self.warmup = warmup_from_params(self.params)   # sparsity warm-up: stages counted in exchanges (hook calls)
         self._names: Dict[int, str] = {id(p): n for n, p in module.named_parameters()}
+        if self.params.get('memory') == 'dgc':     # a pattern that matches nothing is a typo: refuse it
+            # over the parameters DDP exchanges (those that require a gradient), as DeepReduceDDP checks them
+            check_exclude_patterns(self.params.get('weight_decay_exclude'),
+                                   [n for n, p in module.named_parameters() if p.requires_grad])
         self._layouts: List[_Layout] = []            # every engine not yet closed
         self._by_index: Dict[int, _Layout] = {}      # the layout a bucket index had last
         self._owner: Dict[int, _Layout] = {}         # id(parameter) -> the layout holding its residual
@@ -260,7 +267,8 @@ class DeepReduceHookState:
         # parameters' layouts are recorded here and must stay as DDP found them: a later change raises at the next step
         # calibration (inside make_engine) resets the residual: it runs before the carry below
         eng = make_engine(plan, self.params, device=buf.device, group=self.group, use_history=self.use_history,
-                          blocks_per_sm=self.blocks_per_sm, grad_dtype=buf.dtype, parameters=list(params), owner=owner)
+                          blocks_per_sm=self.blocks_per_sm, grad_dtype=buf.dtype, parameters=list(params), owner=owner,
+                          names=names)
         table = segment_table(segments, plan, owner)
         repack = ops.cuda_module().Repack(table, buf.numel(), plan.total_elems, eng.grad)
         lay = _Layout(key, index, list(params), names, list(segments), plan, eng, table, repack)

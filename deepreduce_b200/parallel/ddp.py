@@ -29,7 +29,7 @@ import torch.nn as nn
 
 from .. import spec
 from ..grace.helper import sparsifier_of
-from ..grace.memory import is_dense
+from ..grace.memory import check_exclude_patterns, decay_excluded, is_dense
 from ..wrappers import deepreduce_from_params
 from .engine import BucketEngine, StatusPoller, total_stats
 from .plan import BucketPlan
@@ -182,17 +182,26 @@ def engine_split_numel(params: dict, blocks_per_sm: int) -> int:
     return int(sn or 0)
 
 
-def engine_kwargs(params: dict) -> dict:
-    """The ``BucketEngine`` memory arguments for ``params``: beta, gamma, momentum, weight decay, clipping and averaging.  They
-    follow the per-tensor memory GRACE builds for the same dict: only ``ResidualMemory`` scales the gradient by gamma,
-    so 'none' and 'dgc' memory run with gamma = 1 ('dgc' accepts no other), and without a residual beta is 0."""
+def engine_kwargs(params: dict, names=None) -> dict:
+    """The ``BucketEngine`` memory arguments for ``params``: beta, gamma, momentum, Nesterov, weight decay, clipping and
+    averaging.  They follow the per-tensor memory GRACE builds for the same dict: only ``ResidualMemory`` scales the
+    gradient by gamma, so 'none' and 'dgc' memory run with gamma = 1 ('dgc' accepts no other), and without a residual
+    beta is 0.  With ``'weight_decay_exclude'``, ``names`` are the bucket's parameter names, one per parameter: those
+    that match a pattern get a decay factor of 0 (``weight_decays``)."""
     memory = params.get('memory', 'none')
-    return dict(beta=float(params.get('beta', 1.0)) if memory in ('residual', 'dgc') else 0.0,
-                gamma=float(params.get('gamma', 1.0)) if memory == 'residual' else 1.0,
-                average=params.get('average', True),
-                momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None,
-                weight_decay=float(params.get('weight_decay', 0.0)) if memory == 'dgc' else 0.0,
-                clip_norm=float(params['clip_norm']) if memory == 'dgc' and 'clip_norm' in params else None)
+    kw = dict(beta=float(params.get('beta', 1.0)) if memory in ('residual', 'dgc') else 0.0,
+              gamma=float(params.get('gamma', 1.0)) if memory == 'residual' else 1.0,
+              average=params.get('average', True),
+              momentum=float(params.get('momentum', 0.9)) if memory == 'dgc' else None,
+              weight_decay=float(params.get('weight_decay', 0.0)) if memory == 'dgc' else 0.0,
+              clip_norm=float(params['clip_norm']) if memory == 'dgc' and 'clip_norm' in params else None,
+              nesterov=memory == 'dgc' and params.get('nesterov', False) is True)
+    if memory == 'dgc' and params.get('weight_decay_exclude'):
+        if names is None:
+            raise ValueError("'weight_decay_exclude' matches parameter names: engine_kwargs needs the bucket's names")
+        wd = kw.pop('weight_decay')
+        kw['weight_decays'] = [0.0 if decay_excluded(n, params['weight_decay_exclude']) else wd for n in names]
+    return kw
 
 
 def stage_plans(numels, names, shapes, params: dict, warmup) -> List[BucketPlan]:
@@ -227,15 +236,16 @@ def switch_engine(old: BucketEngine, build) -> BucketEngine:
 
 
 def make_engine(plan: BucketPlan, params: dict, *, device, group, use_history: bool, blocks_per_sm: int,
-                grad_dtype: torch.dtype, parameters=None, owner=None, grad=None) -> BucketEngine:
+                grad_dtype: torch.dtype, parameters=None, owner=None, grad=None, names=None) -> BucketEngine:
     """The ``BucketEngine`` of one bucket for ``params`` (memory arguments from ``engine_kwargs``), with its tile
     partitions calibrated unless ``'calibrate_partition': False``.  ``parameters`` / ``owner``: the bucket's parameters
     and the plan tensors' owners (``split_large``), bound when the engine applies weight decay; ``owner`` also makes
     the chunks of a split parameter one tensor for ``'clip_norm'``.  ``grad``: the flat gradient buffer to adopt
-    (``BucketEngine``); the calibration overwrites it.  Collective at W > 1."""
+    (``BucketEngine``); the calibration overwrites it.  ``names``: the parameters' names, which
+    ``'weight_decay_exclude'`` matches (``engine_kwargs``).  Collective at W > 1."""
     eng = BucketEngine(plan, device=device, group=group, use_history=use_history, blocks_per_sm=blocks_per_sm,
-                       grad_dtype=grad_dtype, owner=owner, grad=grad, **engine_kwargs(params))
-    if eng.weight_decay != 0.0:
+                       grad_dtype=grad_dtype, owner=owner, grad=grad, **engine_kwargs(params, names))
+    if eng.reads_parameters:
         if parameters is None:
             raise ValueError("'weight_decay' reads the parameters: make_engine needs the bucket's parameters")
         eng.bind_parameters(parameters, owner)
@@ -288,6 +298,8 @@ class DeepReduceDDP:
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.named = [(n, p) for n, p in module.named_parameters() if p.requires_grad]
+        if self.params.get('memory') == 'dgc':     # a pattern that matches nothing is a typo: refuse it
+            check_exclude_patterns(self.params.get('weight_decay_exclude'), [n for n, _ in self.named])
         self.device = self.named[0][1].device
         self.is_cuda = self.device.type == "cuda"
         self.dense = self.params.get('compressor', 'none') in ('none', None)
@@ -344,7 +356,8 @@ class DeepReduceDDP:
                 self._plans.append(stage_plans(numels, names, shapes, self.params, self.warmup))
                 self._engine_args.append(dict(device=self.device, group=self.group, use_history=use_history,
                                               blocks_per_sm=blocks_per_sm, grad_dtype=dtype,
-                                              parameters=[p for _, p in items], owner=owner))
+                                              parameters=[p for _, p in items], owner=owner,
+                                              names=[n for n, _ in items]))
                 plan = self._plans[b][self.stage]
                 eng = make_engine(plan, self.params, **self._engine_args[b])
                 self.engines.append(eng)

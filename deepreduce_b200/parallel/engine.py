@@ -473,9 +473,38 @@ def clip_oracle(plan: BucketPlan, g: torch.Tensor, thr: float, owner: Optional[S
     return g
 
 
+def tensor_decays(plan: BucketPlan, weight_decay: float = 0.0, weight_decays: Optional[Sequence[float]] = None,
+                  owner: Optional[Sequence[int]] = None) -> list:
+    """The weight decay factor of every plan tensor: ``weight_decays[owner[j]]`` for plan tensor j when one factor per
+    parameter is given (``owner``: ``split_large``'s map, default one plan tensor each), else ``weight_decay``.  Every
+    factor must be a finite number >= 0."""
+    n = len(plan.tensors)
+    if weight_decays is None:
+        out = [weight_decay] * n
+    else:
+        owner = list(range(n)) if owner is None else [int(o) for o in owner]
+        if len(owner) != n or len(weight_decays) != (max(owner) + 1 if owner else 0):
+            raise ValueError(f"weight_decays: {len(weight_decays)} factors for owner {owner} of the plan's {n} tensors")
+        out = [weight_decays[o] for o in owner]
+    for wd in out:
+        if isinstance(wd, bool) or not isinstance(wd, (int, float)) or not math.isfinite(wd) or wd < 0:
+            raise ValueError(f"weight decay factors must be finite numbers >= 0 (got {wd!r})")
+    return [float(wd) for wd in out]
+
+
+def decay_oracle(plan: BucketPlan, g: torch.Tensor, w: torch.Tensor, decays: Sequence[float]) -> torch.Tensor:
+    """d = g + (decays[j] * w), two roundings, over every plan tensor j whose factor is not 0, its padding included
+    (where w is 0); the other tensors keep g as it is, and their w is never used (a NaN there changes nothing)."""
+    lam = torch.zeros(plan.total_elems, dtype=torch.float32)
+    ends = [t.elem_off for t in plan.tensors[1:]] + [plan.total_elems]
+    for t, end, wd in zip(plan.tensors, ends, decays):
+        lam[t.elem_off:end] = float(wd)
+    return torch.where(lam != 0, g + (lam * w), g)
+
+
 def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Sequence[torch.Tensor], *, beta=1.0,
                   gamma=1.0, average=True, seed=spec.DEFAULT_SEED, epoch=1, momentum=None, moms=None,
-                  weight_decay=0.0, weights=None, clip_norm=None, owner=None):
+                  weight_decay=0.0, weights=None, clip_norm=None, owner=None, nesterov=False, weight_decays=None):
     """One bucket step for W ranks on the CPU.  grads/resids: per-rank flat
     buffers (plan.total_elems).  Returns (dense_out, new_resids, slots).
 
@@ -487,15 +516,30 @@ def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Seque
     the padding), and g is replaced by d = g + (wd * w), two roundings, before the momentum.
 
     ``clip_norm`` c (with ``momentum``): ahead of that, each rank's gradient is clipped per parameter at c / sqrt(W)
-    (``clip_oracle``; ``owner`` maps the plan tensors to parameters as ``split_large`` returns it)."""
+    (``clip_oracle``; ``owner`` maps the plan tensors to parameters as ``split_large`` returns it).
+
+    ``weight_decays`` (with ``momentum``, instead of ``weight_decay``): one factor per parameter, mapped to the plan
+    tensors through ``owner`` (``tensor_decays``); a tensor whose factor is 0 keeps g (``decay_oracle``).
+
+    ``nesterov`` (with ``momentum`` > 0): Nesterov momentum, r = r + v with v = d + (momentum * u), the new u, instead
+    of r = r + u; u itself is unchanged."""
     W = len(grads)
     dgc = momentum is not None
     if dgc and (beta != 1.0 or gamma != 1.0 or moms is None or len(moms) != W):
         raise ValueError("engine_oracle: momentum needs beta = gamma = 1 and one momentum buffer per rank")
     if weight_decay != 0.0 and (not dgc or weights is None or len(weights) != W):
         raise ValueError("engine_oracle: weight_decay needs momentum and one parameter buffer per rank")
+    decays = None
+    if weight_decays is not None:
+        if weight_decay != 0.0:
+            raise ValueError("engine_oracle: give weight_decay or weight_decays, not both")
+        decays = tensor_decays(plan, 0.0, weight_decays, owner)
+        if any(decays) and (not dgc or weights is None or len(weights) != W):
+            raise ValueError("engine_oracle: weight_decays needs momentum and one parameter buffer per rank")
     if clip_norm is not None and not dgc:
         raise ValueError("engine_oracle: clip_norm needs momentum")
+    if nesterov and not (dgc and float(momentum) > 0.0):
+        raise ValueError("engine_oracle: nesterov needs a momentum > 0")
     out = torch.zeros(plan.total_elems, dtype=torch.float32)
     new_resids, slots, new_moms = [], [], []
     for r in range(W):
@@ -505,9 +549,11 @@ def engine_oracle(plan: BucketPlan, grads: Sequence[torch.Tensor], resids: Seque
             g = clip_oracle(plan, g, float(clip_norm) / math.sqrt(W), owner)
         if weight_decay != 0.0:
             g = g + (float(weight_decay) * weights[r].detach().cpu().float())
+        elif decays is not None and any(decays):
+            g = decay_oracle(plan, g, weights[r].detach().cpu().float(), decays)
         if dgc:
             u = float(momentum) * moms[r].detach().cpu().float() + g
-            acc_flat = res + u
+            acc_flat = res + (g + (float(momentum) * u) if nesterov else u)
         else:
             acc_flat = beta * res + gamma * g if beta != 0.0 else gamma * g
         slot = np.zeros(plan.payload_words, dtype=np.uint32)
@@ -687,7 +733,8 @@ class BucketEngine:
                  hist_shift: int = 22, shard: Optional[bool] = None, transport: Optional[str] = None,
                  peer_timeout_ms: Optional[int] = None, fault: int = 0, grad_dtype: torch.dtype = torch.float32,
                  momentum: Optional[float] = None, weight_decay: float = 0.0, clip_norm: Optional[float] = None,
-                 owner: Optional[Sequence[int]] = None, grad: Optional[torch.Tensor] = None):
+                 owner: Optional[Sequence[int]] = None, grad: Optional[torch.Tensor] = None, nesterov: bool = False,
+                 weight_decays: Optional[Sequence[float]] = None):
         # grad: adopt this flat gradient buffer (``plan.total_elems`` of ``grad_dtype`` on ``device``) instead of
         # allocating one, so that views into it (``p.grad``) stay valid across engines of the same layout (the sparsity
         # warm-up's stage switch); calibrate_partition scribbles on it like on an own buffer
@@ -711,7 +758,25 @@ class BucketEngine:
         if wd != 0 and momentum is None:
             raise ValueError("weight_decay is added inside the 'dgc' memory: it needs momentum")
         self.weight_decay = float(wd)
+        # weight_decays: one factor per original parameter (``owner``'s numbering) instead of weight_decay: one value
+        # for all, or 0 for the parameters excluded from the decay ('weight_decay_exclude'); decays: the factor of
+        # every plan tensor
+        if weight_decays is not None and wd != 0:
+            raise ValueError("give weight_decay or weight_decays, not both")
+        self.decays = tensor_decays(plan, self.weight_decay, weight_decays, owner)
+        if any(self.decays) and momentum is None:
+            raise ValueError("weight_decays are added inside the 'dgc' memory: they need momentum")
+        self.reads_parameters = any(self.decays)     # some tensor takes the decay: phase 0 reads its parameter
+        if len(set(d for d in self.decays if d != 0.0)) > 1:
+            raise ValueError(f"weight_decays: one factor for every parameter, or 0 to exclude one (got "
+                             f"{sorted(set(self.decays))})")
         self._bound = None                       # (parameters, owner, data_ptrs, strides) of the last bind_parameters
+        # nesterov=True ('dgc' only, momentum > 0): r = r + (d + m*u) with the new u (engine_oracle(nesterov=True))
+        if not isinstance(nesterov, bool):
+            raise ValueError(f"nesterov must be True or False (got {nesterov!r})")
+        if nesterov and not (momentum is not None and float(momentum) > 0.0):
+            raise ValueError("nesterov needs the 'dgc' momentum, with a momentum > 0")
+        self.nesterov = nesterov
         # clip_norm=c ('dgc' only): DGC's local gradient clipping of every parameter at c / sqrt(W), ahead of the weight
         # decay; ``owner`` (split_large) makes the chunks of a split parameter one norm (engine_oracle(clip_norm=...))
         c = clip_norm
@@ -793,9 +858,11 @@ class BucketEngine:
             self.ctx.set_scratch(self.pos_mask.data_ptr(), self.dec_mask.data_ptr(), self.cand.data_ptr(),
                                  self.cand_cnt.data_ptr())
             if self.mom is not None:
-                self.ctx.set_momentum(self.mom.data_ptr(), self.momentum)
-            # one parameter address per plan tensor (bind_parameters); the kernel reads it only when weight_decay != 0
+                self.ctx.set_momentum(self.mom.data_ptr(), self.momentum, self.nesterov)
+            # one parameter address per plan tensor (bind_parameters); the kernel reads it only where the decay is on
+            # and the tensor's flag in ``decayed`` is set
             self.wparams = torch.zeros(nT, dtype=torch.int64, device=dev)
+            self.decayed = torch.tensor([d != 0.0 for d in self.decays], dtype=torch.uint8, device=dev)
             self.clip_thr = None
             if self.clip_norm is not None:
                 self.clip_thr = self.clip_norm / math.sqrt(self.world)
@@ -1048,17 +1115,17 @@ class BucketEngine:
                 raise ValueError(f"bind_parameters: parameter {i} has {p.numel()} elements, the plan {done[i]}")
         self.wparams.copy_(torch.tensor(ptrs, dtype=torch.int64))
         self._bound = (params, owner, [p.data_ptr() for p in params], [tuple(p.stride()) for p in params])
-        self.ctx.set_weight_decay(self.wparams.data_ptr(), self.weight_decay)
+        self.ctx.set_weight_decay(self.wparams.data_ptr(), max(self.decays), self.decayed.data_ptr())
 
     def refresh_parameters(self):
         """Before a launch: rebuild the parameter table if a bound parameter's storage moved (``p.data = ...``).  The
         check is a host-side comparison of data pointers; it raises if weight decay is on and nothing is bound.  A moved
         parameter must keep the strides it was bound with: the bucket holds its gradient in that storage order (e.g.
         ``model.to(memory_format=...)`` after the buckets were built raises here)."""
-        if self.weight_decay == 0.0:
+        if not self.reads_parameters:
             return
         if self._bound is None:
-            raise RuntimeError("weight_decay > 0 reads the parameters: call bind_parameters() before the first step")
+            raise RuntimeError("weight decay > 0 reads the parameters: call bind_parameters() before the first step")
         params, owner, ptrs, layouts = self._bound
         if any(p.data_ptr() != q for p, q in zip(params, ptrs)):
             changed = [i for i, (p, l) in enumerate(zip(params, layouts)) if tuple(p.stride()) != l]

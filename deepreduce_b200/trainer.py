@@ -41,7 +41,8 @@ class Trainer:
             # 'memory': 'dgc' accumulates the momentum before the exchange (momentum correction): the optimizer then
             # runs without one, whatever ``momentum`` says.  A user optimizer must do the same.  With 'weight_decay'
             # in the dict the memory adds the decay ahead of that momentum, and the dict's value replaces
-            # ``weight_decay`` here: the optimizer runs without it.
+            # ``weight_decay`` here: the optimizer runs without it ('weight_decay_exclude' and 'nesterov' live in the
+            # memory as well).
             if params.get('memory') == 'dgc':
                 momentum = 0.0
                 if 'weight_decay' in params:

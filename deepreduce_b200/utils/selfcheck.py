@@ -86,7 +86,7 @@ def _bits_equal_across_ranks(x: torch.Tensor, group=None) -> bool:
 def multi_gpu_check(engine, seed: int = 4242) -> dict:
     """Run one checked exchange step on ``engine`` (a live ``BucketEngine``; its residual / epoch advance by one
     step).  Returns ``{"status": "ok" | "FAILED: ...", ...details}``; collective — every rank must call it."""
-    from ..parallel.engine import clip_oracle
+    from ..parallel.engine import clip_oracle, decay_oracle
     W, rank, plan = engine.world, engine.rank, engine.plan
     dev = engine.device
     gen = torch.Generator(device=dev).manual_seed(seed + 1000 * rank)
@@ -96,8 +96,14 @@ def multi_gpu_check(engine, seed: int = 4242) -> dict:
     g = g.to(engine.grad.dtype).float()         # bf16 engine: the widened bf16 gradient is what the engine accumulates
     if engine.mom is not None:                  # 'dgc': the momentum is compensated, then added to the residual
         c = clip_oracle(plan, g, engine.clip_thr, engine.owner) if engine.clip_thr is not None else g
-        d = c + (engine.weight_decay * engine.parameter_buffer()) if engine.weight_decay != 0.0 else c
-        acc = engine.resid + (engine.momentum * engine.mom + d)
+        if engine.weight_decay != 0.0:
+            d = c + (engine.weight_decay * engine.parameter_buffer())
+        elif engine.reads_parameters:                # per-parameter factors ('weight_decay_exclude')
+            d = decay_oracle(plan, c.cpu(), engine.parameter_buffer().cpu(), engine.decays).to(dev)
+        else:
+            d = c
+        u = engine.momentum * engine.mom + d
+        acc = engine.resid + ((d + (engine.momentum * u)) if engine.nesterov else u)
     else:
         acc = engine.beta * engine.resid + engine.gamma * g if engine.beta != 0.0 else engine.gamma * g
     engine.grad.copy_(g)
